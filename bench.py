@@ -1,11 +1,12 @@
 #!/usr/bin/env python
 """bench.py — images/sec of the BiSeNet-R18 training step (1024x1024, 19 classes, bf16, batch 16/GPU, OHEM).
 
-    python bench.py --gpus N --steps K --warmup W            # B200-native path (libtsb)
+    python bench.py --gpus N --steps K --warmup W            # H100-native path (libtsb)
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as .npy
     python bench.py --impl reference --gpus N --steps K ...  # reference CPU arm (oracle port on host cores)
 
 One "step" = zero_grad → forward (3 OHEM losses) → backward → gradient all-reduce (N>1) → fused SGD step, i.e.
-/root/reference/model/bisenet/cityscapes.bisenet.R18/train.py:116-142 on synthetic data (SURVEY.md §8d).
+TorchSeg model/bisenet/cityscapes.bisenet.R18/train.py:116-142 on synthetic data (SURVEY.md §8d).
 Prints ONE JSON line (rank 0). See the task contract for the keys.
 """
 import argparse
@@ -37,7 +38,8 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured (sustained)")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s
+    return dict(hbm_gbs=3350.0, tflops=989.0, src="H100 SXM data sheet")
 
 
 # ------------------------------------------------------------------------------------------------ data
@@ -447,6 +449,21 @@ def run_reference_arm(args):
     print(json.dumps(line))
 
 
+# ------------------------------------------------------------------------------------------------ outputs
+DUMP_PARAM_SAMPLE = 1 << 20   # parameter entries written by --dump-outputs (fixed seed → same entries every run)
+
+
+def dump_outputs(out_dir, loss, model):
+    """What the timed step hands back: its loss, and the parameters it updated (a fixed, seeded sample, fp32)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    params = torch.cat([p.detach().float().reshape(-1) for p in model.parameters()]).cpu().numpy()
+    idx = np.sort(np.random.default_rng(0).choice(params.size, min(DUMP_PARAM_SAMPLE, params.size), replace=False))
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([loss], dtype=np.float32))
+    np.save(os.path.join(out_dir, "params_sample.npy"), params[idx].astype(np.float32))
+    np.save(os.path.join(out_dir, "params_sample_index.npy"), idx.astype(np.float64))
+
+
 # ------------------------------------------------------------------------------------------------ main arm
 def main():
     global BATCH_PER_GPU, MODEL, H, W, NUM_CLASSES, IGNORE, STEP_GFLOP_PER_IMG, METRIC, WORKLOAD
@@ -465,6 +482,9 @@ def main():
                          "engine.graph.GraphedTrainStep; the eager time is reported beside it)")
     ap.add_argument("--pipeline", action="store_true", help="secondary line: device input pipeline throughput, 1 GPU")
     ap.add_argument("--eval", action="store_true", help="secondary line: evaluator forward throughput (BN folding), 1 GPU")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (loss, a fixed seeded sample of "
+                         "the updated parameters) to DIR/<name>.npy")
     ap.add_argument("--default-stream", action="store_true",
                     help="run on the legacy default stream (default: a non-blocking side stream, which whole-step graph capture needs)")
     args = ap.parse_args()
@@ -597,6 +617,8 @@ def main():
         ms, clk = max_over_ranks(e0.elapsed_time(e1)), clk_g
         launches = gstep.launches_per_step * args.steps
         final_loss = float(loss.item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, final_loss, model)
 
     # ---------------- measurement pass B (separate, NOT part of `value`): every conv launch bracketed by CUDA events on
     # the launch stream → roofline.achieved = algorithmic conv FLOPs / summed conv kernel time
@@ -672,7 +694,7 @@ def main():
             "config": {"workload": WORKLOAD,
                        "batch_per_gpu": BATCH_PER_GPU, "global_batch": BATCH_PER_GPU * world, "parallelism": "dp%d" % world,
                        "sync_bn": world > 1, "optimizer": "fused flat SGD (momentum 0.9, poly LR, reference wd / lr groups)",
-                       "l2_policy": "inputs larger than L2 (activations >> 126 MB per step), no explicit flush",
+                       "l2_policy": "inputs larger than L2 (activations >> 50 MB per step), no explicit flush",
                        "final_loss": final_loss,
                        "step_launch": step_launch,
                        "sync_bn_exchange": (None if world == 1 else ("NVLink peer-memory kernel (tsb_p2p_allreduce_sum)" if ops._sync.get("p2p") is not None else "NCCL all-reduce per layer")),
@@ -689,7 +711,7 @@ def main():
                          "traffic_note": "dram__bytes_read+write summed over the conv launches of ONE step (%s); algorithmic minimum ~5.9 GB/step" % traffic_src,
                          "flops_per_step": min(prof["flops"], algo_flops) / prof_steps,
                          "launched_flops_per_step": prof["flops"] / prof_steps,
-                         "kernel": "tcgen05 implicit-GEMM conv kernels (igemm_v2_kernel fprop/dgrad/stem + wgrad kernels), all launches of the step",
+                         "kernel": "wgmma implicit-GEMM conv kernels (igemm_v2_kernel fprop/dgrad/stem + wgrad kernels), all launches of the step",
                          "launches": prof["launches"], "kernel_ms_per_step": prof["ms"] / prof_steps,
                          "measured_in": "separate instrumented pass of %d eager steps (not the `value` region)" % prof_steps,
                          "peak_source": peaks["src"]},
@@ -707,7 +729,7 @@ def main():
                     nb = max(2, nb // 2)
                     ref_gpu[mode] = gpu_reference_steps(device, nb, H, W, 3, 2, mode)
             best = max(v["value"] for v in ref_gpu.values())
-            line["reference_gpu"] = {"kind": "port", "what": "oracle restatement of the reference step (stock torch.nn + cuDNN, cudnn.benchmark=True, torch.optim.SGD) on the same B200",
+            line["reference_gpu"] = {"kind": "port", "what": "oracle restatement of the reference step (stock torch.nn + cuDNN, cudnn.benchmark=True, torch.optim.SGD) on the same GPU",
                                      "fp32": ref_gpu["fp32"], "bf16_autocast_channels_last": ref_gpu["bf16"],
                                      "speedup_vs_fp32": value / ref_gpu["fp32"]["value"], "speedup_vs_best": value / best}
             threads = pick_threads()

@@ -1,5 +1,5 @@
 /*
- * libtsb — C ABI of the B200-native (sm_100a) semantic-segmentation training hot path.
+ * libtsb — C ABI of the H100-native (sm_90a) semantic-segmentation training hot path.
  *
  * Drop-in boundary for the training step of yu-changqian/TorchSeg ("furnace"): every entry point
  * replaces one lowering that the reference obtains from torch.nn / ATen / cuDNN / apex on the path
@@ -13,6 +13,12 @@
  *   - no allocation, no host synchronisation, no global mutable state inside (except a cached
  *     driver entry point and SM count);
  *   - work is enqueued on the cudaStream_t passed in (pass 0 for the legacy default stream);
+ *   - entry points that sum per-CTA partials (conv statistics and weight gradients, BN reductions, channel-attention
+ *     gradient, adaptive pooling, bias gradient) take `float* ws, long long ws_floats`: a caller-owned fp32
+ *     workspace that holds one slot per CTA; the slots are summed in a fixed order, so results are identical from run
+ *     to run. A workspace may only be used by one call at a time: give each stream its own, or order the calls.
+ *     24 Mi floats (96 MB) covers every shape of the shipped networks; a too-small workspace is an error (the
+ *     weight-gradient kernels instead fall back to one split, which needs none);
  *   - the device is the calling thread's current device;
  *   - return 0 on success, a negative TSB_ERR_* on failure; tsb_last_error() returns a thread-local
  *     human-readable message;
@@ -41,9 +47,9 @@ const char* tsb_last_error(void);
 int tsb_version(void);          /* 10000*major + 100*minor + patch */
 /* number of kernels launched by this library from the calling process since load (all threads) */
 long long tsb_launch_count(void);
-/* debug / A-B switches of the convolution path: key 1 = UMMA descriptor base_offset for row-shifted taps,
- * 2 = allow row tiles, 3 = allow resident weights, 4 = use the persistent kernel (0 → first-generation kernel),
- * 5 = wgrad waves, 6 = OHEM register hoisting, 7 = weight-sharing tile pairs, 8 = nine-tap wgrad kernel */
+/* debug / A-B switches: key 1 = wgmma descriptor base_offset for row-shifted taps, 2 = allow row tiles,
+ * 3 = allow resident weights, 5 = wgrad waves, 6 = OHEM register hoisting, 8 = nine-tap wgrad kernel,
+ * 10 = exact-class-count OHEM band kernels */
 int tsb_debug_set(int key, int value);
 
 /* ================================================================================================
@@ -123,8 +129,8 @@ int tsb_bilinear_fwd_nhwc_to_nchw(const void* in, int idtype, int ics, float* ou
  * and nn.MaxPool2d(3,2,1) (furnace/base_model/resnet.py:132). NHWC bf16.
  * ============================================================================================== */
 /* out fp32 [N, S, S, C] (bins [floor(i*H/S), ceil((i+1)*H/S)) ), S==1 is the global pool */
-int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, int H, int W, int S, float* out,
-                             tsb_stream_t stream);
+int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, int H, int W, int S, float* out, float* ws,
+                             long long ws_floats, tsb_stream_t stream);
 /* din(bf16) (+)= dout[n, bin(h), bin(w), c] / bin_area  (S==1 → broadcast of dout/(H*W)) */
 int tsb_adaptive_avgpool_bwd(const float* dout, int N, int C, int H, int W, int S, void* din, int ics,
                              int accumulate, tsb_stream_t stream);
@@ -142,7 +148,8 @@ int tsb_maxpool3x3s2_bwd(const void* argmax, const void* dout, int ocs, void* di
  * stats and finalize (NCCL, outside this library).
  * ============================================================================================== */
 /* per-channel sum and sum of squares of x (bf16 NHWC), accumulated into fp32 sum[C], sumsq[C] (caller zeroes) */
-int tsb_bn_stats(const void* x, int cs, long long npix, int C, float* sum, float* sumsq, tsb_stream_t stream);
+int tsb_bn_stats(const void* x, int cs, long long npix, int C, float* sum, float* sumsq, float* ws, long long ws_floats,
+                 tsb_stream_t stream);
 /* mean/invstd from (sum,sumsq,count); scale=gamma*invstd, shift=beta-mean*scale; running stats update
  * (momentum, unbiased variance — SURVEY App. A3). running_* may be NULL. */
 int tsb_bn_finalize(const float* sum, const float* sumsq, double count, int C, const float* gamma,
@@ -156,7 +163,7 @@ int tsb_bn_apply(const void* x, int xcs, const float* scale, const float* shift,
  * residual input) and the read of y is saved; scale/shift are then required. */
 int tsb_bn_bwd_reduce(const void* dy, int dycs, const void* y, int ycs, const void* x, int xcs, const float* mean,
                       const float* invstd, int relu, long long npix, int C, float* sum_dz, float* sum_dz_xhat,
-                      const float* scale, const float* shift, tsb_stream_t stream);
+                      const float* scale, const float* shift, float* ws, long long ws_floats, tsb_stream_t stream);
 /* backward pass 2: dx = gamma*invstd*(dz - sum_dz/cnt - xhat*sum_dz_xhat/cnt); optional dres = dz;
  * optional dgamma_acc[c] += sum_dz_xhat[c], dbeta_acc[c] += sum_dz[c] (parameter gradients, folded into this pass);
  * y == NULL with relu: mask recomputed from scale/shift as in tsb_bn_bwd_reduce */
@@ -176,7 +183,7 @@ int tsb_chan_scale_fwd(const void* x, int xcs, const float* a, float base, const
                        int ycs, int N, int HW, int C, tsb_stream_t stream);
 /* dx = dy*(base+sig); da[n,c] += Σ_hw dy*x*sig*(1-sig)  (da fp32 [N,C], caller zeroes); dadd == dy */
 int tsb_chan_scale_bwd(const void* dy, int dycs, const void* x, int xcs, const float* a, float base, void* dx,
-                       int dxcs, float* da, int N, int HW, int C, tsb_stream_t stream);
+                       int dxcs, float* da, int N, int HW, int C, float* ws, long long ws_floats, tsb_stream_t stream);
 
 /* ================================================================================================
  * Layout / precision packing
@@ -226,8 +233,8 @@ int tsb_transpose_pad(const void* in, int idtype, int ics, void* out_bf16, int o
                       tsb_stream_t stream);
 
 /* ================================================================================================
- * Convolution as im2col-free implicit GEMM on tcgen05 tensor cores (TMA → 128B-swizzled smem →
- * tcgen05.mma, fp32 accumulators in TMEM) — replaces nn.Conv2d inside ConvBnRelu (seg_oprs.py:29-31),
+ * Convolution as im2col-free implicit GEMM on Hopper tensor cores (TMA → 128B-swizzled smem →
+ * wgmma, fp32 accumulators in registers) — replaces nn.Conv2d inside ConvBnRelu (seg_oprs.py:29-31),
  * conv3x3 (resnet.py:11-14), the 1x1 heads (bisenet network.py:156-161) and their cuDNN
  * dgrad / wgrad. bf16 operands, fp32 accumulation.
  *
@@ -245,7 +252,7 @@ typedef struct {
 /* fprop: y = conv(x, w) (+bias[k]) ; optional per-channel batch statistics of the ROUNDED output
  * accumulated into sum[K], sumsq[K] (fp32, caller zeroes) — the BN-statistics epilogue. */
 int tsb_conv2d_fprop(const tsb_conv_shape* s, const void* x, int xcs, const void* w, const float* bias, void* y,
-                     int ydtype, int ycs, float* sum, float* sumsq, tsb_stream_t stream);
+                     int ydtype, int ycs, float* sum, float* sumsq, float* ws, long long ws_floats, tsb_stream_t stream);
 /* inference form with the BatchNorm FOLDED into the weights (evaluator path, furnace/engine/evaluator.py:255-275 runs the
  * network in eval mode): y = relu?(conv(x, w_folded) + bias (+ res)) in the conv epilogue — no raw tensor, no BN pass.
  * res (optional, bf16) must be laid out exactly like y (rescs == ycs): the shortcut of a residual block. */
@@ -256,18 +263,19 @@ int tsb_conv2d_fprop_fused(const tsb_conv_shape* s, const void* x, int xcs, cons
 int tsb_conv2d_dgrad(const tsb_conv_shape* s, const void* dy, int dycs, const void* wt, void* dx, int dxcs,
                      int accumulate, tsb_stream_t stream);
 /* wgrad: dw[K,R,S,C] (fp32, KRSC) += Σ_pixels dy ⊗ x  (red.global.add.f32; caller zeroes or accumulates) */
-int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs, const void* dy, int dycs, float* dw,
-                     tsb_stream_t stream);
+int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs, const void* dy, int dycs, float* dw, float* ws,
+                     long long ws_floats, tsb_stream_t stream);
 /* stride-2 C_in=3 stem (7x7 pad 3 or 3x3 pad 1, same packed weight format) on the s2d-packed image (tsb_pack_image_s2d / tsb_pack_stem_weight):
  * xs2d [N,H/2,W/2+4,16] bf16, wp [K,4,4,16] bf16 → y [N,H/2,W/2,K]. */
 int tsb_conv_stem_fprop(const void* xs2d, int N, int H, int W, const void* wp, int K, void* y, int ycs, float* sum,
-                        float* sumsq, tsb_stream_t stream);
+                        float* sumsq, float* ws, long long ws_floats, tsb_stream_t stream);
 int tsb_conv_stem_fprop_fused(const void* xs2d, int N, int H, int W, const void* wp, int K, const float* bias, int relu,
                               void* y, int ycs, tsb_stream_t stream);
-int tsb_conv_stem_wgrad(const void* xs2d, int N, int H, int W, const void* dy, int dycs, int K, float* dwp,
-                        tsb_stream_t stream);
+int tsb_conv_stem_wgrad(const void* xs2d, int N, int H, int W, const void* dy, int dycs, int K, float* dwp, float* ws,
+                        long long ws_floats, tsb_stream_t stream);
 /* column sums: db[k] += Σ_pixels dy[pix,k] (bias gradient of the 1x1 classifier heads) */
-int tsb_bias_grad(const void* dy, int dycs, long long npix, int K, float* db, tsb_stream_t stream);
+int tsb_bias_grad(const void* dy, int dycs, long long npix, int K, float* db, float* ws, long long ws_floats,
+                  tsb_stream_t stream);
 
 /* ================================================================================================
  * Optimiser — fused flat-buffer momentum SGD replacing torch.optim.SGD.step (train.py:86-89,142) with

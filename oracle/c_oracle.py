@@ -1,6 +1,6 @@
 """ctypes/numpy wrapper of oracle/tsb_oracle.c (bit-exact OHEM + bilinear restatement).
 
-ORACLE — test infrastructure only. Cites: /root/reference/furnace/seg_opr/loss_opr.py:68-98.
+ORACLE — test infrastructure only. Cites: TorchSeg furnace/seg_opr/loss_opr.py:68-98.
 """
 import ctypes
 import os

@@ -1,8 +1,8 @@
 """ORACLE — test infrastructure only.
 
 numpy restatement of the reference's training-time input pipeline for one sample
-(/root/reference/model/bisenet/cityscapes.bisenet.R18/dataloader.py:11-33 `TrainPre.__call__`, built from
-/root/reference/furnace/utils/img_utils.py: random_mirror :140-145, random_scale :118-125, normalize :181-187,
+(TorchSeg model/bisenet/cityscapes.bisenet.R18/dataloader.py:11-33 `TrainPre.__call__`, built from
+TorchSeg furnace/utils/img_utils.py: random_mirror :140-145, random_scale :118-125, normalize :181-187,
 generate_random_crop_pos :44-60, random_crop_pad_to_shape :24-41 / pad_image_to_shape :63-78) and of the two OpenCV
 routines it calls on uint8 data.
 
@@ -115,7 +115,7 @@ def train_pre(img_rgb, gt, params, crop_size, mean, std, gt_down_sampling=1):
 
 
 # --------------------------------------------------------------------------------------------------
-# DFN border labels — /root/reference/model/dfn/cityscapes.dfn.R101_v1c/dataloader.py:15-29:
+# DFN border labels — TorchSeg model/dfn/cityscapes.dfn.R101_v1c/dataloader.py:15-29:
 #   no255_gt = gt with 255 → 0; cgt = cv2.Canny(no255_gt, 5, 5, apertureSize=7); cgt = cv2.dilate(cgt, 7x7 rect); 255 → 1
 # OpenCV's Canny for apertureSize = 7 (imgproc/src/canny.cpp): thresholds /16 then floor (5 → 0), dx / dy =
 # Sobel(ksize 7, scale 1/16, BORDER_REPLICATE) as int16 (round half to even), magnitude |dx| + |dy| with a zero border,

@@ -1,7 +1,8 @@
 """ORACLE — test infrastructure only.
 
-Imports the UNMODIFIED reference modules live from /root/reference (authoring container only; the GPU
-box has no /root/reference) with the three in-memory shims of SURVEY.md App. C:
+Imports the UNMODIFIED reference modules live from a TorchSeg checkout named by TSB_REFERENCE_DIR (used by
+tools/make_golden.py and tools/make_live_golden.py to regenerate tests/golden) with the three in-memory shims of
+SURVEY.md App. C:
   1. import utils.pyt_utils before engine.logger (circular import),
   2. exec loss_opr.py with `1 - valid_mask` → `~valid_mask` (bool-tensor subtraction, torch >= 1.2),
   3. a stand-in `config` module (easydict is absent and config.py needs a cwd containing 'TorchSeg').
@@ -13,12 +14,12 @@ import os
 import sys
 import types
 
-REF = os.environ.get("TSB_REFERENCE_DIR", "/root/reference")
+REF = os.environ.get("TSB_REFERENCE_DIR", "")
 FURNACE = os.path.join(REF, "furnace")
 
 
 def available():
-    return os.path.isdir(FURNACE)
+    return bool(REF) and os.path.isdir(FURNACE)
 
 
 class _Cfg(dict):

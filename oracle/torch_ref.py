@@ -13,7 +13,7 @@ import torch.nn.functional as F
 
 # --------------------------------------------------------------------------------------------------
 # optional bf16-storage emulation: the SAME fp32 math, but values are rounded to bf16 (forward AND the
-# gradient flowing back) at the points where the B200 path stores bf16 — conv weights, raw conv outputs,
+# gradient flowing back) at the points where the libtsb path stores bf16 — conv weights, raw conv outputs,
 # activations, pooled / resized maps. Separates "kernel bug" from "bf16 storage policy" in end-to-end tests.
 # --------------------------------------------------------------------------------------------------
 class _RoundBF16(torch.autograd.Function):
@@ -43,7 +43,7 @@ def qw(w):
 
 
 # --------------------------------------------------------------------------------------------------
-# ProbOhemCrossEntropy2d.forward — /root/reference/furnace/seg_opr/loss_opr.py:68-98
+# ProbOhemCrossEntropy2d.forward — TorchSeg furnace/seg_opr/loss_opr.py:68-98
 # (with `1 - mask` → `~mask`, the torch>=1.2 shim of SURVEY.md App. C2)
 # --------------------------------------------------------------------------------------------------
 def ohem_ce(pred, target, ignore_label=255, thresh=0.7, min_kept=256, weight=None, return_aux=False):
@@ -105,7 +105,7 @@ def _bn(x, sd, prefix, eps, momentum, training, stats=None):
 
 def conv_bn_relu(x, sd, prefix, stride, pad, dilation=1, has_bn=True, has_relu=True, eps=1e-5, momentum=0.1,
                  training=True, stats=None):
-    """ConvBnRelu.forward — /root/reference/furnace/seg_opr/seg_oprs.py:39-46"""
+    """ConvBnRelu.forward — TorchSeg furnace/seg_opr/seg_oprs.py:39-46"""
     x = q(F.conv2d(x, qw(sd[prefix + ".conv.weight"]), sd.get(prefix + ".conv.bias"), stride, pad, dilation))
     if has_bn:
         x = _bn(x, sd, prefix + ".bn", eps, momentum, training, stats)
@@ -115,7 +115,7 @@ def conv_bn_relu(x, sd, prefix, stride, pad, dilation=1, has_bn=True, has_relu=T
 
 
 def basic_block(x, sd, prefix, stride, has_down, eps, momentum, training, stats=None):
-    """BasicBlock.forward — /root/reference/furnace/base_model/resnet.py:33-53"""
+    """BasicBlock.forward — TorchSeg furnace/base_model/resnet.py:33-53"""
     out = q(F.conv2d(x, qw(sd[prefix + ".conv1.weight"]), None, stride, 1))
     out = q(F.relu(_bn(out, sd, prefix + ".bn1", eps, momentum, training, stats)))
     out = q(F.conv2d(out, qw(sd[prefix + ".conv2.weight"]), None, 1, 1))
@@ -148,7 +148,7 @@ def attention_refinement(x, sd, prefix, eps, momentum, training, stats=None):
     se = q(F.adaptive_avg_pool2d(fm, 1))
     se = conv_bn_relu(se, sd, prefix + ".channel_attention.1", 1, 0, has_relu=False, eps=eps, momentum=momentum,
                       training=training, stats=stats)
-    return fm * torch.sigmoid(se)  # rounded by the caller after `+ last_fm` (one fused kernel on the B200 path)
+    return fm * torch.sigmoid(se)  # rounded by the caller after `+ last_fm` (one fused kernel on the libtsb path)
 
 
 def feature_fusion(x1, x2, sd, prefix, eps, momentum, training, stats=None):
@@ -168,7 +168,7 @@ def bisenet_head_logits(x, sd, prefix, eps, momentum, training, stats=None):
 
 
 def bisenet_r18_forward(data, sd, eps=1e-5, momentum=0.1, training=True, stats=None):
-    """BiSeNet.forward wiring — /root/reference/model/bisenet/cityscapes.bisenet.R18/network.py:75-111.
+    """BiSeNet.forward wiring — TorchSeg model/bisenet/cityscapes.bisenet.R18/network.py:75-111.
     Returns the three LOW-resolution logit tensors (aux0 @1/16 scale 16, aux1 @1/8, main @1/8) and features."""
     kw = dict(eps=eps, momentum=momentum, training=training, stats=stats)
     sp = conv_bn_relu(q(data), sd, "spatial_path.conv_7x7", 2, 3, **kw)
@@ -207,7 +207,7 @@ def bisenet_r18_loss(data, label, sd, min_kept, ignore_label=255, thresh=0.7, ep
 
 # --------------------------------------------------------------------------------------------------
 # BASELINE configs[0]: FCN-32s on a ResNet-18 backbone (plumbing case, CPU) — the reference ships FCN with
-# R101_v1c (/root/reference/model/fcn/voc.fcn32s.R101_v1c/network.py:13-68); the R18 variant keeps the same
+# R101_v1c (TorchSeg model/fcn/voc.fcn32s.R101_v1c/network.py:13-68); the R18 variant keeps the same
 # head/loss wiring with resnet18(deep_stem=False) and heads _FCNHead(512,.) / _FCNHead(256,.) (SURVEY §8 a15).
 # Dropout2d(0.1) is disabled (p=0) so the case is deterministic.
 # --------------------------------------------------------------------------------------------------
@@ -247,10 +247,10 @@ def fcn_r101_loss(data, label, sd, layers=(3, 4, 23, 3), aux_ratio=0.5, ignore_l
 
 
 # --------------------------------------------------------------------------------------------------
-# PSPNet-R101_v1c dilated-8 — /root/reference/model/pspnet/ade.pspnet.R101_v1c/network.py:14-109
+# PSPNet-R101_v1c dilated-8 — TorchSeg model/pspnet/ade.pspnet.R101_v1c/network.py:14-109
 # --------------------------------------------------------------------------------------------------
 def bottleneck(x, sd, prefix, stride, dil2, has_down, down_stride, eps, momentum, training, stats=None):
-    """Bottleneck.forward — /root/reference/furnace/base_model/resnet.py:78-101 (conv2 carries stride / dilation)"""
+    """Bottleneck.forward — TorchSeg furnace/base_model/resnet.py:78-101 (conv2 carries stride / dilation)"""
     out = q(F.conv2d(x, qw(sd[prefix + ".conv1.weight"])))
     out = q(F.relu(_bn(out, sd, prefix + ".bn1", eps, momentum, training, stats)))
     out = q(F.conv2d(out, qw(sd[prefix + ".conv2.weight"]), None, stride, dil2, dil2))
@@ -312,7 +312,7 @@ def pyramid_pooling_logits(x, sd, prefix, eps, momentum, training, scales=(1, 2,
 def _up8(x, data):
     """pspnet / psanet network.py:46-49: F.interpolate(scale_factor=8, bilinear, align_corners=True). For inputs whose
     size is not a multiple of 8 (BASELINE.json's 713 / 473 crops; the reference's own 480 is) the x8 map does not match
-    the label, so — identically in this oracle and in the B200 networks — the target is the INPUT size (`size=`), which
+    the label, so — identically in this oracle and in the libtsb networks — the target is the INPUT size (`size=`), which
     is the same operation whenever both are defined (align_corners: src = dst·(in-1)/(out-1))."""
     H, W = data.shape[2:]
     if x.shape[2] * 8 == H and x.shape[3] * 8 == W:
@@ -336,7 +336,7 @@ def pspnet_loss(data, label, sd, layers=(3, 4, 23, 3), aux_ratio=0.4, ignore_lab
 # DFN (model/dfn/cityscapes.dfn.R101_v1c/network.py)
 # --------------------------------------------------------------------------------------------------
 def refine_residual(x, sd, prefix, has_relu, eps, momentum, training, stats=None):
-    """RefineResidual.forward — /root/reference/furnace/seg_opr/seg_oprs.py:182-188"""
+    """RefineResidual.forward — TorchSeg furnace/seg_opr/seg_oprs.py:182-188"""
     x = q(F.conv2d(x, qw(sd[prefix + ".conv_1x1.weight"])))
     t = conv_bn_relu(x, sd, prefix + ".cbr", 1, 1, eps=eps, momentum=momentum, training=training, stats=stats)
     t = q(F.conv2d(t, qw(sd[prefix + ".conv_refine.weight"]), None, 1, 1))
@@ -344,7 +344,7 @@ def refine_residual(x, sd, prefix, has_relu, eps, momentum, training, stats=None
 
 
 def bn_refine(x, sd, prefix, has_relu, eps, momentum, training, stats=None):
-    """BNRefine.forward — /root/reference/furnace/seg_opr/seg_oprs.py:157-162"""
+    """BNRefine.forward — TorchSeg furnace/seg_opr/seg_oprs.py:157-162"""
     t = conv_bn_relu(x, sd, prefix + ".conv_bn_relu", 1, 1, eps=eps, momentum=momentum, training=training, stats=stats)
     t = q(F.conv2d(t, qw(sd[prefix + ".conv_refine.weight"]), None, 1, 1))
     return q(F.relu(t + x)) if has_relu else q(t + x)

@@ -103,3 +103,50 @@ def pipeline_case_dfn(H=100, W=160, crop=(96, 128), seed=2):
     gt[rng.random((H, W)) < 0.03] = 255
     return (bgr, gt, crop, [0.5, 0.75, 1, 1.5, 1.75, 2.0], np.array([0.485, 0.456, 0.406]),
             np.array([0.229, 0.224, 0.225]))
+
+
+# ---- live-reference cases pinned by tests/golden/live_reference.npz (tools/make_live_golden.py) ----
+OHEM_SAMPLE = 2000   # gradient entries stored per OHEM case
+
+
+def metric_inputs():
+    """seeded predictions for the metric functions, incl. ignore labels (255 → outside [0, n_cl), -1 for ADE) and
+    classes that never occur"""
+    import numpy as np
+    rng = np.random.default_rng(5)
+    n_cl = 19
+    gt = rng.integers(0, 17, size=(3, 64, 80))          # classes 17, 18 never occur → NaN IoU, skipped by nanmean
+    gt[:, :5] = 255
+    pred = np.where(rng.random(gt.shape) < 0.7, np.clip(gt, 0, 16), rng.integers(0, 17, size=gt.shape))
+    lab = rng.integers(-1, 150, size=(48, 64))
+    pr = np.where(rng.random(lab.shape) < 0.6, np.clip(lab, 0, 149), rng.integers(0, 150, size=lab.shape))
+    return n_cl, pred, gt, pr, lab
+
+
+def eval_net():
+    """small deterministic network for the Evaluator comparison"""
+    class Net(torch.nn.Module):
+        def __init__(self):
+            super().__init__()
+            torch.manual_seed(0)
+            self.c1 = torch.nn.Conv2d(3, 8, 3, padding=1)
+            self.c2 = torch.nn.Conv2d(8, 5, 3, padding=2, dilation=2)
+
+        def forward(self, x):
+            return torch.log_softmax(self.c2(torch.relu(self.c1(x))) * 3.0, dim=1)
+    return Net().double().float()
+
+
+def eval_image():
+    import numpy as np
+    return np.random.default_rng(3).integers(0, 256, size=(150, 210, 3), dtype=np.uint8)
+
+
+def _eval_kw():
+    import numpy as np
+    return dict(dataset=None, class_num=5, image_mean=np.array([0.485, 0.456, 0.406]),
+                image_std=np.array([0.229, 0.224, 0.225]), network=None, multi_scales=[0.75, 1.0, 1.5], is_flip=True,
+                devices=[0])
+
+
+EVAL_KW = _eval_kw()

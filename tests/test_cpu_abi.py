@@ -45,11 +45,11 @@ def test_argument_validation_without_gpu(lib):
     shp = ConvShape(1, 8, 8, 64, 64, 3, 3, 1, 1, 1, 7, 7)
     buf = ctypes.create_string_buffer(64)
     rc = lib.tsb_conv2d_fprop(ctypes.byref(shp), ctypes.addressof(buf), 64, ctypes.addressof(buf), None,
-                              ctypes.addressof(buf), 1, 64, None, None, None)
+                              ctypes.addressof(buf), 1, 64, None, None, None, 0, None)
     assert rc == -1 and b"inconsistent" in lib.tsb_last_error()
     shp = ConvShape(1, 8, 8, 48, 64, 3, 3, 1, 1, 1, 8, 8)   # C not a multiple of 64
     rc = lib.tsb_conv2d_fprop(ctypes.byref(shp), ctypes.addressof(buf), 48, ctypes.addressof(buf), None,
-                              ctypes.addressof(buf), 1, 64, None, None, None)
+                              ctypes.addressof(buf), 1, 64, None, None, None, 0, None)
     assert rc == -1 and b"multiple of 64" in lib.tsb_last_error()
 
 

@@ -76,7 +76,7 @@ def test_parse_devices_and_engine_cli(monkeypatch, tmp_path):
 def test_fcn_r18_plumbing_cpu(tmp_path, monkeypatch):
     """BASELINE configs[0]: FCN-32s R18, 2 x 256 x 256, CPU, 1 process — the train.py sequence (Engine, group_weight,
     SGD, PolyLR, checkpoint save / link / restore) with the loss evaluated by the oracle restatement on the
-    module's own parameters (the B200 kernels do not run on a CPU)."""
+    module's own parameters (the CUDA kernels do not run on a CPU)."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     from golden_cases import fcn_case
     from oracle import torch_ref
@@ -133,8 +133,9 @@ def test_fcn_r18_plumbing_cpu(tmp_path, monkeypatch):
 
 # ------------------------------------------------------------------------------------------------- world_size 2
 def _worker(rank, world, port, q):
+    # the gloo (CPU) path: on a host with fewer GPUs than ranks the Engine would pick NCCL and a missing device
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
+                      LOCAL_RANK=str(rank), CUDA_VISIBLE_DEVICES="")
     sys.path.insert(0, ROOT)
     import torch.distributed as dist
     from torchseg_b200.engine.engine import Engine

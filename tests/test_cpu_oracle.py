@@ -1,5 +1,5 @@
-"""CPU tests: the oracle against the golden vectors generated from the LIVE reference (tools/make_golden.py),
-against the live reference itself when /root/reference is present, and the two oracle restatements (C and
+"""CPU tests: the oracle against the golden vectors generated from the LIVE reference (tools/make_golden.py,
+tools/make_live_golden.py), and the two oracle restatements (C and
 torch) against each other."""
 import hashlib
 import json
@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from golden_cases import ohem_case, bisenet_case, fcn_case, fcn_r101_case, pspnet_case, dfn_case, psanet_case, OHEM_REGIMES
+from golden_cases import EVAL_KW, eval_image, eval_net, metric_inputs
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLD = json.load(open(os.path.join(HERE, "golden", "reference_outputs.json")))
@@ -206,186 +207,111 @@ def test_bilinear_oracle_matches_aten():
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# live reference (authoring container only)
+# the reference modules' own outputs, stored by tools/make_live_golden.py (tests/golden/live_reference.npz)
 # ---------------------------------------------------------------------------------------------------------------
-def _live():
-    from oracle import reference_live as rl
-    if not rl.available():
-        pytest.skip("/root/reference not present (GPU box): pinned by tests/golden instead")
-    return rl
+LIVE = np.load(os.path.join(HERE, "golden", "live_reference.npz"))
 
 
 def test_oracle_vs_live_reference_ohem():
-    rl = _live()
     from oracle import c_oracle
-    lo = rl.load_loss_opr()
     for regime in ["A", "B", "C", "D"]:
         for seed in (1, 2, 3):
+            k = "ohem_%s%d_" % (regime, seed)
             logits, labels, min_kept = ohem_case(regime, seed=seed, H=32, W=40)
-            crit = lo.ProbOhemCrossEntropy2d(ignore_label=255, thresh=0.7, min_kept=min_kept, use_weight=False)
-            x = logits.clone().requires_grad_(True)
-            loss = crit(x, labels)
-            loss.backward()
-            kept_ref = (x.grad.abs().sum(dim=1) > 0).reshape(-1).numpy()
             out = c_oracle.ohem(logits.numpy(), labels.numpy(), 255, 0.7, min_kept, want_grad=True)
-            assert np.array_equal(out["kept"], kept_ref), (regime, seed)
-            assert abs(out["loss"] - float(loss)) < 1e-5 * abs(float(loss))
-            assert np.max(np.abs(out["dlogits"] - x.grad.numpy())) < 1e-6
+            assert np.array_equal(out["kept"], LIVE[k + "kept"]), (regime, seed)
+            loss = float(LIVE[k + "loss"])
+            assert abs(out["loss"] - loss) < 1e-5 * abs(loss)
+            assert np.max(np.abs(out["dlogits"].reshape(-1)[LIVE[k + "grad_idx"]] - LIVE[k + "grad"])) < 1e-6
 
 
 def test_oracle_vs_live_reference_bisenet_exact():
-    rl = _live()
     from oracle import torch_ref
-    net = rl.load_network('bisenet/cityscapes.bisenet.R18')
-    lo = rl.load_loss_opr()
+    from torchseg_b200.networks import BiSeNet
     x, y, min_kept, seed = bisenet_case(N=2, HW=64, seed=5)
     torch.manual_seed(seed)
-    crit = lo.ProbOhemCrossEntropy2d(ignore_label=255, thresh=0.7, min_kept=min_kept, use_weight=False)
-    m = net.BiSeNet(19, True, crit, None, torch.nn.BatchNorm2d)
-    m.train()
+    m = BiSeNet(19, True, None, None, torch.nn.BatchNorm2d)   # same seed → the reference's initial weights
     sd = {k: v.detach().clone() for k, v in m.state_dict().items()}
     for k, v in sd.items():
         if v.is_floating_point() and "running" not in k:
             v.requires_grad_(True)
-    loss_ref = m(x, y)
-    loss_ref.backward()
     loss, _ = torch_ref.bisenet_r18_loss(x, y, sd, min_kept)
     loss.backward()
-    assert float(loss) == float(loss_ref)
-    for n, p in m.named_parameters():
-        assert torch.equal(p.grad, sd[n].grad), n
+    assert float(loss) == float(LIVE["bisenet_loss"])
+    for n, (norm, idx, vals) in json.loads(str(LIVE["bisenet_grads"])).items():
+        flat = sd[n].grad.reshape(-1).double().numpy()
+        assert abs(np.linalg.norm(flat) - norm) <= 1e-5 * norm, n
+        assert np.max(np.abs(flat[idx] - np.array(vals))) <= 1e-5 * max(norm, 1e-30), n
 
 
 def test_module_key_names_match_reference():
     """checkpoint compatibility: our BiSeNet exposes exactly the reference's state_dict keys and shapes (App. D)"""
-    rl = _live()
     from torchseg_b200.networks import BiSeNet
-    net = rl.load_network('bisenet/cityscapes.bisenet.R18')
-    ref = net.BiSeNet(19, True, None, None, torch.nn.BatchNorm2d).state_dict()
+    ref = json.loads(str(LIVE["bisenet_keys"]))
     ours = BiSeNet(19, True, None, None, torch.nn.BatchNorm2d).state_dict()
-    assert list(ref.keys()) == list(ours.keys())
-    for k in ref:
-        assert ref[k].shape == ours[k].shape, k
+    assert [k for k, _ in ref] == list(ours.keys())
+    for k, shape in ref:
+        assert list(ours[k].shape) == shape, k
 
 
 def test_metric_functions_vs_live_reference():
     """seg_opr.metric (confusion matrix / IoU / ADE intersection-union) against the reference's metric.py on seeded
     predictions, incl. ignore labels (255 → outside [0, n_cl), -1 for ADE) and classes that never occur"""
-    import importlib.util
     from torchseg_b200.seg_opr import metric as mine
-    rl = _live()
-    spec = importlib.util.spec_from_file_location("ref_metric", os.path.join(rl.REF, "furnace", "seg_opr", "metric.py"))
-    ref = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(ref)
-    rng = np.random.default_rng(5)
-    n_cl = 19
-    gt = rng.integers(0, 17, size=(3, 64, 80))          # classes 17, 18 never occur → NaN IoU, skipped by nanmean
-    gt[:, :5] = 255
-    pred = np.where(rng.random(gt.shape) < 0.7, np.clip(gt, 0, 16), rng.integers(0, 17, size=gt.shape))
+    n_cl, pred, gt, pr, lab = metric_inputs()
+    h2, l2, c2 = LIVE["metric_hist"], int(LIVE["metric_labeled"]), int(LIVE["metric_correct"])
     h1, l1, c1 = mine.hist_info(n_cl, pred, gt)
-    h2, l2, c2 = ref.hist_info(n_cl, pred, gt)
     assert np.array_equal(h1, h2) and l1 == l2 and c1 == c2
-    for a, b in zip(mine.compute_score(h1, c1, l1), ref.compute_score(h2, c2, l2)):
-        assert np.allclose(a, b, equal_nan=True)
+    for i, a in enumerate(mine.compute_score(h1, c1, l1)):
+        assert np.allclose(a, LIVE["metric_score_%d" % i], equal_nan=True)
     ht, lt, ct = mine.hist_info_torch(n_cl, torch.from_numpy(pred), torch.from_numpy(gt))
     assert np.array_equal(ht.numpy(), h2) and int(lt) == l2 and int(ct) == c2
     # ADE protocol
-    lab = rng.integers(-1, 150, size=(48, 64))
-    pr = np.where(rng.random(lab.shape) < 0.6, np.clip(lab, 0, 149), rng.integers(0, 150, size=lab.shape))
     i1, u1 = mine.intersectionAndUnion(pr, lab, 150)
-    i2, u2 = ref.intersectionAndUnion(pr, lab, 150)
-    assert np.array_equal(i1, i2) and np.array_equal(u1, u2)
-    for a, b in zip(mine.meanIoU(np.stack([i1, i1], 1), np.stack([u1, u1], 1)), ref.meanIoU(np.stack([i2, i2], 1), np.stack([u2, u2], 1))):
-        assert np.allclose(a, b, equal_nan=True)
-    for a, b in zip(mine.pixelAccuracy(pr, lab), ref.pixelAccuracy(pr, lab)):
-        assert a == b
-    assert mine.mean_pixel_accuracy([3, 4], [5, 6]) == ref.mean_pixel_accuracy([3, 4], [5, 6])
-    assert mine.accuracy(pr, lab)[0] == ref.accuracy(pr, lab)[0]
+    assert np.array_equal(i1, LIVE["metric_inter"]) and np.array_equal(u1, LIVE["metric_union"])
+    for i, a in enumerate(mine.meanIoU(np.stack([i1, i1], 1), np.stack([u1, u1], 1))):
+        assert np.allclose(a, LIVE["metric_miou_%d" % i], equal_nan=True)
+    assert np.array_equal(np.asarray(mine.pixelAccuracy(pr, lab), dtype=np.float64), LIVE["metric_pixacc"])
+    assert mine.mean_pixel_accuracy([3, 4], [5, 6]) == float(LIVE["metric_mpa"])
+    assert mine.accuracy(pr, lab)[0] == float(LIVE["metric_acc"])
 
 
 def test_evaluator_sliding_and_whole_eval_vs_live_reference(monkeypatch):
     """engine.evaluator (batched sliding-window evaluation) against the reference Evaluator run on the CPU with a small
     deterministic network: same window grid, same summed (not averaged) overlap handling, same flip / multi-scale
     accumulation, same cv2 resizes → identical arg-max maps and matching scores"""
-    rl = _live()
-    ref_mod = rl.load_evaluator()
     from torchseg_b200.engine.evaluator import Evaluator
     monkeypatch.setattr(torch.Tensor, "cuda", lambda self, *a, **k: self, raising=False)
-
-    class Net(torch.nn.Module):
-        def __init__(self):
-            super().__init__()
-            torch.manual_seed(0)
-            self.c1 = torch.nn.Conv2d(3, 8, 3, padding=1)
-            self.c2 = torch.nn.Conv2d(8, 5, 3, padding=2, dilation=2)
-
-        def forward(self, x):
-            return torch.log_softmax(self.c2(torch.relu(self.c1(x))) * 3.0, dim=1)
-
-    class RefWrap(object):       # the reference calls .eval() / .to(get_device()) (-1 on the CPU) on its val_func
-        def __init__(self, m):
-            self.m = m
-
-        def eval(self):
-            self.m.eval()
-
-        def to(self, *a):
-            return self
-
-        def __call__(self, x):
-            return self.m(x)
-
-    net = Net().double().float()
-    mean, std = np.array([0.485, 0.456, 0.406]), np.array([0.229, 0.224, 0.225])
-    rng = np.random.default_rng(3)
-    img = rng.integers(0, 256, size=(150, 210, 3), dtype=np.uint8)
-    kw = dict(dataset=None, class_num=5, image_mean=mean, image_std=std, network=None, multi_scales=[0.75, 1.0, 1.5],
-              is_flip=True, devices=[0])
-    mine = Evaluator(crop_batch=3, **kw)
-    mine.val_func = net
-
-    class _DS(object):
-        def get_length(self):
-            return 0
-    kw_ref = dict(kw, dataset=_DS())
-    ref = ref_mod.Evaluator(**kw_ref)
-    ref.val_func = RefWrap(net)
+    mine = Evaluator(crop_batch=3, **EVAL_KW)
+    mine.val_func = eval_net()
+    img = eval_image()
     # sliding evaluation: crop 96 on a 150x210 image → 2x3 .. 3x5 windows per scale, incl. the single-window scale path
-    p_ref = ref.sliding_eval(img, 96, 2 / 3.0, None)
     p_mine = mine.sliding_eval(img, 96, 2 / 3.0, None)
-    assert p_ref.shape == p_mine.shape == (150, 210)
-    assert (p_ref == p_mine).mean() > 0.999
-    s_ref = ref.scale_process(img, (150, 210), 96, 2 / 3.0, None)
+    assert p_mine.shape == (150, 210)
+    assert (LIVE["eval_sliding"] == p_mine).mean() > 0.999
     s_mine = mine.scale_process(img, (150, 210), 96, 2 / 3.0, None)
-    assert np.abs(s_ref - s_mine).max() < 1e-4 * np.abs(s_ref).max()
+    assert np.abs(s_mine.reshape(-1)[LIVE["eval_scale_idx"]] - LIVE["eval_scale"]).max() < 1e-4 * float(LIVE["eval_scale_absmax"])
     assert mine.window_grid(150, 210, 96, 2 / 3.0) == [(0, 0), (0, 64), (0, 114), (54, 0), (54, 64), (54, 114)]
     # small image → single padded window
-    small = img[:80, :70]
-    assert np.array_equal(ref.sliding_eval(small, 96, 2 / 3.0, None), mine.sliding_eval(small, 96, 2 / 3.0, None))
+    assert np.array_equal(LIVE["eval_small"], mine.sliding_eval(img[:80, :70], 96, 2 / 3.0, None))
     # whole-image evaluation with padding to a fixed input size and resize to an output size
-    w_ref = ref.whole_eval(img, (75, 105), (160, 224), None)
-    w_mine = mine.whole_eval(img, (75, 105), (160, 224), None)
-    assert (w_ref == w_mine).mean() > 0.999
+    assert (LIVE["eval_whole"] == mine.whole_eval(img, (75, 105), (160, 224), None)).mean() > 0.999
     # grey-scale input path
-    g = img[:, :, :1]
-    assert (ref.whole_eval(g, None, None, None) == mine.whole_eval(g, None, None, None)).mean() > 0.999
+    assert (LIVE["eval_grey"] == mine.whole_eval(img[:, :, :1], None, None, None)).mean() > 0.999
 
 
 def test_oracle_dfn_blocks_vs_live_reference_modules():
-    """RefineResidual / BNRefine / ChannelAttention restatements against the live reference modules (bit-exact, fp32)"""
+    """RefineResidual / BNRefine / ChannelAttention restatements against the reference modules' outputs (bit-exact, fp32)"""
     from oracle import torch_ref as tr
-    rl = _live()
-    so = rl.load_seg_oprs()
-    torch.manual_seed(3)
-    x = torch.randn(2, 16, 9, 11)
+
+    def sd_of(key):
+        return {"m." + k: torch.tensor(v, dtype=torch.float32 if isinstance(v, list) else None)
+                for k, v in json.loads(str(LIVE[key])).items()}
+    x, x2 = torch.from_numpy(LIVE["dfn_x"]), torch.from_numpy(LIVE["dfn_x2"])
     for relu in (True, False):
-        m = so.BNRefine(16, 16, 3, has_relu=relu).train()
-        sd = {"m." + k: v.detach().clone() for k, v in m.state_dict().items()}
-        assert torch.equal(tr.bn_refine(x, sd, "m", relu, 1e-5, 0.1, True), m(x))
-        m = so.RefineResidual(16, 24, 3, has_relu=relu).train()
-        sd = {"m." + k: v.detach().clone() for k, v in m.state_dict().items()}
-        assert torch.equal(tr.refine_residual(x, sd, "m", relu, 1e-5, 0.1, True), m(x))
-    m = so.ChannelAttention(32, 16, 1)
-    sd = {"m." + k: v.detach().clone() for k, v in m.state_dict().items()}
-    x2 = torch.randn(2, 16, 9, 11)
-    assert torch.allclose(tr.channel_attention(x, x2, sd, "m"), m(x, x2), atol=1e-6)
+        out = tr.bn_refine(x, sd_of("dfn_bnrefine_%d_sd" % relu), "m", relu, 1e-5, 0.1, True)
+        assert torch.equal(out, torch.from_numpy(LIVE["dfn_bnrefine_%d_out" % relu]))
+        out = tr.refine_residual(x, sd_of("dfn_refres_%d_sd" % relu), "m", relu, 1e-5, 0.1, True)
+        assert torch.equal(out, torch.from_numpy(LIVE["dfn_refres_%d_out" % relu]))
+    out = tr.channel_attention(x, x2, sd_of("dfn_ca_sd"), "m")
+    assert torch.allclose(out, torch.from_numpy(LIVE["dfn_ca_out"]), atol=1e-6)

@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 BiSeNet-R18 training step against the oracle (oracle/torch_ref.py, pinned to
+"""End-to-end parity of the libtsb BiSeNet-R18 training step against the oracle (oracle/torch_ref.py, pinned to
 the live reference).
 
 Two layers of evidence, because a randomly initialised batch-stat BN network amplifies bf16-level noise by

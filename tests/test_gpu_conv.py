@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05 implicit-GEMM convolution (fprop / dgrad / wgrad / stem) against
+"""GPU parity tests of the wgmma implicit-GEMM convolution (fprop / dgrad / wgrad / stem) against
 F.conv2d autograd in fp32 on bf16-rounded operands. Tolerance 1e-2 of the output scale (bf16 path)."""
 import pytest
 import torch
@@ -25,8 +25,8 @@ CASES = [
     (1, 64, 7, 260, 128, 3, 2, 1, 1),      # row tiles, stride 2 (parity views), Q = 130
     (1, 64, 3, 300, 64, 3, 1, 4, 4),       # row tiles + dilation 4 (span 8)
     (1, 128, 4, 256, 64, 1, 1, 0, 1),      # 1x1 → flat GEMM, resident weights
-    # >= 2 tiles per CTA with streamed weights → weight-sharing tile PAIRS (two accumulators per B tile), odd tails
-    (8, 128, 64, 128, 128, 3, 1, 1, 1),    # 512 row tiles over 148 CTAs (3 or 4 each)
+    # >= 2 tiles per CTA with streamed weights, odd tails
+    (8, 128, 64, 128, 128, 3, 1, 1, 1),    # 512 row tiles over 132 CTAs (3 or 4 each)
     (4, 128, 40, 136, 256, 3, 1, 2, 2),    # two N tiles, dilation 2, ragged width (2 tiles per row)
     (4, 1024, 48, 128, 256, 1, 1, 0, 1),   # 1x1 with streamed weights (flat GEMM), 4 stages
 ]
@@ -131,11 +131,11 @@ def test_stem_7x7(cuda, HW, R):
     y = ops.nhwc_empty(N, K, H // 2, W // 2)
     stats = torch.zeros(2, K, device=cuda)
     ops.call("tsb_conv_stem_fprop", ops.ptr(xs), N, H, W, ops.ptr(wp), K, ops.ptr(y), K, ops.ptr(stats[0]), ops.ptr(stats[1]),
-             ops.stream())
+             *ops.det_ws(), ops.stream())
     torch.cuda.synchronize()
     assert rel_err(y, y_ref) < 1e-2
     dwp = torch.zeros((K, 4, 64), device=cuda)
-    ops.call("tsb_conv_stem_wgrad", ops.ptr(xs), N, H, W, ops.ptr(ops.to_nhwc(gy.to(cuda))), K, K, ops.ptr(dwp), ops.stream())
+    ops.call("tsb_conv_stem_wgrad", ops.ptr(xs), N, H, W, ops.ptr(ops.to_nhwc(gy.to(cuda))), K, K, ops.ptr(dwp), *ops.det_ws(), ops.stream())
     dw = torch.zeros((K, R, R, 3), device=cuda)
     ops.call("tsb_unpack_stem_wgrad", ops.ptr(dwp), K, R, ops.ptr(dw), ops.stream())
     torch.cuda.synchronize()
@@ -162,11 +162,11 @@ def test_conv_full_size_linearity(cuda):
 
 
 # BASELINE.json configs[1] layer shapes (batch 16 @ 1024 x 1024 input): the tile choices that only exist at this size —
-# row tiles, persistent CTAs with resident / streamed / PAIRED weights, the nine-tap wgrad kernel, stride-2 parity views
+# row tiles, persistent CTAs with resident / streamed weights, the nine-tap wgrad kernel, stride-2 parity views
 FULL_SIZE = [
     (16, 64, 256, 256, 64, 3, 1, 1, 1),     # layer1 (resident weights, row tiles; nine-tap wgrad, K = 64)
     (16, 64, 256, 256, 128, 3, 2, 1, 1),    # layer2.0.conv1 (stride 2)
-    (16, 128, 128, 128, 128, 3, 1, 1, 1),   # layer2 (streamed weights, tile pairs)
+    (16, 128, 128, 128, 128, 3, 1, 1, 1),   # layer2 (streamed weights)
     (16, 256, 64, 64, 256, 3, 1, 1, 1),     # layer3
     (16, 512, 32, 32, 512, 3, 1, 1, 1),     # layer4 (TW = 32, TH = 2 tiles in the nine-tap wgrad)
     (16, 128, 128, 128, 256, 3, 1, 1, 1),   # aux head 3x3
@@ -252,6 +252,43 @@ def test_stem_odd_image_size(cuda, HW, R):
     wp = torch.empty((K, 4, 4, 16), dtype=torch.bfloat16, device=cuda)
     ops.call("tsb_pack_stem_weight", ops.ptr(wk), K, R, ops.ptr(wp), ops.stream())
     y = ops.nhwc_empty(N, K, He // 2, We // 2)
-    ops.call("tsb_conv_stem_fprop", ops.ptr(xs), N, He, We, ops.ptr(wp), K, ops.ptr(y), K, None, None, ops.stream())
+    ops.call("tsb_conv_stem_fprop", ops.ptr(xs), N, He, We, ops.ptr(wp), K, ops.ptr(y), K, None, None, *ops.det_ws(), ops.stream())
     torch.cuda.synchronize()
     assert rel_err(y, y_ref) < 1e-2
+
+
+@pytest.mark.parametrize("case", [(2, 64, 32, 32, 64, 3, 1, 1, 1), (1, 64, 7, 260, 128, 3, 2, 1, 1),
+                                  (2, 256, 16, 16, 256, 1, 1, 0, 1)], ids=["taps", "rows", "generic"])
+def test_wgrad_without_workspace_adds_in_place(cuda, case):
+    """with no reduction workspace the weight gradient runs as one pixel split that adds straight into dW: same result as
+    the split path (up to summation order), and it accumulates onto what dW already holds"""
+    import ctypes
+    from torchseg_b200 import ops
+    N, C, H, W, K, R, stride, pad, dil = case
+    g = torch.Generator(device="cuda").manual_seed(14)
+    P, Q = ops.conv_out_size(H, R, stride, pad, dil), ops.conv_out_size(W, R, stride, pad, dil)
+    x = ops.to_nhwc(torch.randn(N, C, H, W, device=cuda, generator=g))
+    gy = ops.to_nhwc(torch.randn(N, K, P, Q, device=cuda, generator=g))
+    ref = torch.zeros((K, R, R, C), dtype=torch.float32, device=cuda)
+    ops.conv_wgrad(x, gy, K, R, stride, pad, dil, ref)
+    base = torch.randn((K, R, R, C), device=cuda, generator=g)
+    dw = base.clone()
+    shp = ops.make_shape(N, H, W, C, K, R, stride, pad, dil)
+    ops.call("tsb_conv2d_wgrad", ctypes.byref(shp), ops.ptr(x), ops.cs_of(x), ops.ptr(gy), ops.cs_of(gy), ops.ptr(dw), None, 0,
+             ops.stream())
+    assert rel_err(dw - base, ref) < 1e-4
+
+
+def test_conv_statistics_need_a_workspace(cuda):
+    """per-CTA statistics without a workspace are refused, not summed into a buffer the caller does not own"""
+    import ctypes
+    from torchseg_b200 import ops
+    N, C, H, W, K = 1, 64, 8, 8, 64
+    x = ops.to_nhwc(torch.randn(N, C, H, W, device=cuda))
+    wb = torch.zeros((K, 3, 3, C), dtype=torch.bfloat16, device=cuda)
+    y = ops.nhwc_empty(N, K, H, W)
+    stats = torch.zeros(2, K, device=cuda)
+    shp = ops.make_shape(N, H, W, C, K, 3, 1, 1, 1)
+    with pytest.raises(RuntimeError, match="workspace"):
+        ops.call("tsb_conv2d_fprop", ctypes.byref(shp), ops.ptr(x), ops.cs_of(x), ops.ptr(wb), None, ops.ptr(y), 1, K,
+                 ops.ptr(stats[0]), ops.ptr(stats[1]), None, 0, ops.stream())

@@ -1,5 +1,5 @@
 """FCN-32s (SURVEY §8 a15) on the GPU: BASELINE configs[0] (R18, 2 x 256 x 256, 19 classes) and the shipped R101_v1c
-variant (/root/reference/model/fcn/voc.fcn32s.R101_v1c/network.py:13-68, VOC 21 classes) — teacher-forced head and
+variant (TorchSeg model/fcn/voc.fcn32s.R101_v1c/network.py:13-68, VOC 21 classes) — teacher-forced head and
 whole training step against the oracle (pinned to the live reference by tests/test_cpu_oracle.py)."""
 import pytest
 import torch

@@ -3,7 +3,7 @@ training step of the libtsb path against the oracle (oracle/torch_ref.py, bit-id
 run ON THE SAME GPU under stock torch.nn + cuDNN in strict fp32 (TF32 off) — SURVEY.md §8c "On the GPU box", north_star
 "outputs match the reference PyTorch/cuDNN path".
 
-The row-tile / PAIR / persistent conv paths, the band OHEM kernels and the multi-wave streaming kernels only run at this
+The row-tile / resident-weight / persistent conv paths, the band OHEM kernels and the multi-wave streaming kernels only run at this
 size, so this is where they are checked against the oracle (the small-shape tests exercise other tile choices).
 Tolerances: loss 1e-2 (north_star, bf16); gradients of the business layers (heads, FFM, ARMs, refines, global context,
 spatial path) norm_err <= 2e-2 per conv / classifier weight; BN running statistics 1e-2; the OHEM kept count of every
@@ -71,7 +71,7 @@ def test_bisenet_full_size_step_matches_oracle_cuda(cuda):
             v.grad = None
         torch.cuda.synchronize()
         torch.cuda.empty_cache()
-        # the SAME fp32 oracle with bf16 STORAGE emulated (values rounded to bf16 wherever the B200 path stores bf16:
+        # the SAME fp32 oracle with bf16 STORAGE emulated (values rounded to bf16 wherever the libtsb path stores bf16:
         # conv weights, raw conv outputs, activations — forward and backward). |fp32 − bf16-storage| is the spread that
         # the storage policy alone produces at this size; the libtsb step has to sit inside it.
         torch_ref.set_bf16_emulation(True)

@@ -234,7 +234,7 @@ def test_bn_kernels(cuda, relu, res):
     gam, bet = gamma.to(cuda), beta.to(cuda)
     stats = torch.zeros(2, C, device=cuda)
     npix = N * H * W
-    ops.call("tsb_bn_stats", ops.ptr(xd), C, npix, C, ops.ptr(stats[0]), ops.ptr(stats[1]), ops.stream())
+    ops.call("tsb_bn_stats", ops.ptr(xd), C, npix, C, ops.ptr(stats[0]), ops.ptr(stats[1]), *ops.det_ws(), ops.stream())
     aux = torch.empty(4, C, device=cuda)
     rmd, rvd = torch.zeros(C, device=cuda), torch.ones(C, device=cuda)
     ops.call("tsb_bn_finalize", ops.ptr(stats[0]), ops.ptr(stats[1]), float(npix), C, ops.ptr(gam), ops.ptr(bet), 1e-5,
@@ -248,7 +248,7 @@ def test_bn_kernels(cuda, relu, res):
     # residual layers read the mask from y; the others recompute it from x*scale+shift (y = NULL)
     ymask = ops.ptr(yd) if (relu and res) else None
     ops.call("tsb_bn_bwd_reduce", ops.ptr(gyd), C, ymask, C, ops.ptr(xd), C, ops.ptr(aux[0]), ops.ptr(aux[1]),
-             int(relu), npix, C, ops.ptr(red[0]), ops.ptr(red[1]), ops.ptr(aux[2]), ops.ptr(aux[3]), ops.stream())
+             int(relu), npix, C, ops.ptr(red[0]), ops.ptr(red[1]), ops.ptr(aux[2]), ops.ptr(aux[3]), *ops.det_ws(), ops.stream())
     dx = ops.nhwc_empty(N, C, H, W); dres = ops.nhwc_empty(N, C, H, W)
     ops.call("tsb_bn_bwd_apply", ops.ptr(gyd), C, ymask, C, ops.ptr(xd), C, ops.ptr(aux[0]), ops.ptr(aux[1]),
              ops.ptr(gam), ops.ptr(red[0]), ops.ptr(red[1]), float(npix), int(relu), ops.ptr(dx), C,

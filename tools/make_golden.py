@@ -1,4 +1,4 @@
-"""Generate tests/golden/*.json from the LIVE reference (/root/reference, authoring container only).
+"""Generate tests/golden/*.json from the LIVE reference (a TorchSeg checkout named by TSB_REFERENCE_DIR).
 
 The reference ships no golden vectors (SURVEY.md §4); these fixtures pin the oracle to outputs of the reference
 modules themselves on seeded synthetic inputs. Inputs are regenerated from seeds (torch CPU generator), only
@@ -26,7 +26,7 @@ def sha(t):
 
 
 def main():
-    assert rl.available(), "needs /root/reference"
+    assert rl.available(), "needs the reference checkout (TSB_REFERENCE_DIR)"
     torch.set_num_threads(8)
     lo = rl.load_loss_opr()
     gold = {"ohem": {}, "torch": torch.__version__}

@@ -1,5 +1,5 @@
 """a handful of launches of the hot kernels at BASELINE size for `ncu --set full` (keep it short: ncu replays ~40x)
-   ncu --set full --clock-control none --import-source on -k regex:'igemm|wgrad|ohem' -s <skip> -c <n> -o gpurun_out/prof python tools/prof_one.py"""
+   ncu --set full --clock-control none --import-source on -k regex:'igemm|wgrad|ohem' -s <skip> -c <n> -o prof python tools/prof_one.py"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

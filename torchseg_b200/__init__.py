@@ -1,4 +1,4 @@
-"""torchseg_b200 — B200-native (sm_100a) training hot path behind the TorchSeg / furnace API.
+"""torchseg_b200 — H100-native (sm_90a) training hot path behind the TorchSeg / furnace API.
 
 The package mirrors the reference's import names for the path (seg_opr.seg_oprs, seg_opr.loss_opr,
 base_model, engine.engine, engine.lr_policy, utils.init_func, utils.pyt_utils, apex.parallel); compute goes

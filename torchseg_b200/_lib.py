@@ -39,17 +39,17 @@ _SIGS = {
     "tsb_bilinear_fwd": [P, I, I, P, I, I, I, I, I, I, I, I, P],
     "tsb_bilinear_bwd": [P, I, I, P, I, I, I, I, I, I, I, I, I, P],
     "tsb_bilinear_fwd_nhwc_to_nchw": [P, I, I, P, I, I, I, I, I, I, P],
-    "tsb_adaptive_avgpool_fwd": [P, I, I, I, I, I, I, P, P],
+    "tsb_adaptive_avgpool_fwd": [P, I, I, I, I, I, I, P, P, L, P],
     "tsb_adaptive_avgpool_bwd": [P, I, I, I, I, I, P, I, I, P],
     "tsb_maxpool3x3s2_fwd": [P, I, P, I, P, I, I, I, I, P],
     "tsb_maxpool3x3s2_bwd": [P, P, I, P, I, I, I, I, I, P],
-    "tsb_bn_stats": [P, I, L, I, P, P, P],
+    "tsb_bn_stats": [P, I, L, I, P, P, P, L, P],
     "tsb_bn_finalize": [P, P, D, I, P, P, F, F, P, P, P, P, P, P, P],
     "tsb_bn_apply": [P, I, P, P, P, I, I, P, I, L, I, P],
-    "tsb_bn_bwd_reduce": [P, I, P, I, P, I, P, P, I, L, I, P, P, P, P, P],
+    "tsb_bn_bwd_reduce": [P, I, P, I, P, I, P, P, I, L, I, P, P, P, P, P, L, P],
     "tsb_bn_bwd_apply": [P, I, P, I, P, I, P, P, P, P, P, D, I, P, I, P, I, L, I, P, P, P, P, P],
     "tsb_chan_scale_fwd": [P, I, P, F, P, I, P, I, I, I, I, P],
-    "tsb_chan_scale_bwd": [P, I, P, I, P, F, P, I, P, I, I, I, P],
+    "tsb_chan_scale_bwd": [P, I, P, I, P, F, P, I, P, I, I, I, P, L, P],
     "tsb_pack_image_s2d": [P, I, I, I, P, P],
     "tsb_pack_weight": [P, I, I, I, I, P, P, P],
     "tsb_pack_stem_weight": [P, I, I, P, P],
@@ -62,14 +62,14 @@ _SIGS = {
     "tsb_softmax_rows_bwd": [P, I, P, I, P, I, L, I, I, P],
     "tsb_transpose_pad": [P, I, I, P, I, I, I, I, P],
     "tsb_relu_bwd": [P, I, P, I, P, I, L, I, P],
-    "tsb_conv2d_fprop": [P, P, I, P, P, P, I, I, P, P, P],
+    "tsb_conv2d_fprop": [P, P, I, P, P, P, I, I, P, P, P, L, P],
     "tsb_conv2d_fprop_fused": [P, P, I, P, P, P, I, I, P, I, I, P],
     "tsb_conv_stem_fprop_fused": [P, I, I, I, P, I, P, I, P, I, P],
     "tsb_conv2d_dgrad": [P, P, I, P, P, I, I, P],
-    "tsb_conv2d_wgrad": [P, P, I, P, I, P, P],
-    "tsb_conv_stem_fprop": [P, I, I, I, P, I, P, I, P, P, P],
-    "tsb_conv_stem_wgrad": [P, I, I, I, P, I, I, P, P],
-    "tsb_bias_grad": [P, I, L, I, P, P],
+    "tsb_conv2d_wgrad": [P, P, I, P, I, P, P, L, P],
+    "tsb_conv_stem_fprop": [P, I, I, I, P, I, P, I, P, P, P, L, P],
+    "tsb_conv_stem_wgrad": [P, I, I, I, P, I, I, P, P, L, P],
+    "tsb_bias_grad": [P, I, L, I, P, P, L, P],
     "tsb_sgd_flat": [P, P, P, L, P, P, P, I, F, F, I, P],
     "tsb_sgd_flat_pack": [P, P, P, L, P, P, P, I, F, F, I, P, P],
     "tsb_pack_wt_multi": [P, P, P, P, I, I, P],
@@ -134,6 +134,22 @@ def ptr(t):
 def stream():
     import torch
     return torch.cuda.current_stream().cuda_stream
+
+
+DET_WS_FLOATS = 24 << 20   # 96 MB: every shape of the shipped networks (include/tsb.h)
+_det_ws = {}
+
+
+def det_ws():
+    """(pointer, floats) of the reduction workspace of the current stream. include/tsb.h: a workspace serves one call at
+    a time, so each stream gets its own (allocated once, through the caching allocator, so also inside a graph capture)."""
+    import torch
+    st = torch.cuda.current_stream()
+    key = (st.device_index, st.cuda_stream)
+    ws = _det_ws.get(key)
+    if ws is None:
+        ws = _det_ws[key] = torch.empty(DET_WS_FLOATS, dtype=torch.float32, device=st.device)
+    return ws.data_ptr(), ws.numel()
 
 
 def dt(t):

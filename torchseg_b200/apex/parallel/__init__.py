@@ -1,4 +1,4 @@
-"""B200-native replacements of the two apex entry points the reference train.py scripts import.
+"""libtsb replacements of the two apex entry points the reference train.py scripts import.
 
 * SyncBatchNorm — parameter holder only (subclass of nn.BatchNorm2d so isinstance-based init_weight /
   group_weight keep working); the statistics exchange happens inside ops.ConvBNActFn as ONE all-reduce of the

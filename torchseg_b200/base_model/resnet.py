@@ -1,5 +1,5 @@
 """ResNet v1 / v1c backbone with the reference's constructor and attribute names
-(/root/reference/furnace/base_model/resnet.py); forward runs the fused libtsb path."""
+(TorchSeg furnace/base_model/resnet.py); forward runs the fused libtsb path."""
 import torch
 import torch.nn as nn
 

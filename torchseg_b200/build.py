@@ -1,7 +1,7 @@
-"""Build libtsb.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libtsb.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 Usage: python -m torchseg_b200.build [--force]
-The .so lands in torchseg_b200/lib/ (git-ignored, but shipped to the GPU box by gpurun).
+The .so lands in torchseg_b200/lib/ and the objects in torchseg_b200/build/ (both git-ignored).
 """
 import hashlib
 import os
@@ -14,10 +14,10 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libtsb.so")
-SOURCES = ["tsb_api.cu", "ohem.cu", "resize_pool.cu", "bn.cu", "pack_opt.cu", "conv_tcgen05.cu", "conv_v2.cu", "conv_wgrad_taps.cu", "psa.cu", "p2p.cu", "data_pipeline.cu", "ce_up.cu"]
+SOURCES = ["tsb_api.cu", "ohem.cu", "resize_pool.cu", "bn.cu", "pack_opt.cu", "conv_igemm.cu", "conv_v2.cu", "conv_wgrad_taps.cu", "psa.cu", "p2p.cu", "data_pipeline.cu", "ce_up.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr",
 ]
 
@@ -59,7 +59,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout + r.stderr)

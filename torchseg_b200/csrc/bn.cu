@@ -1,19 +1,22 @@
-// Training-mode BatchNorm pieces on NHWC bf16 activations (fp32 statistics), sm_100a.
-// Replaces norm_layer(...) of ConvBnRelu (/root/reference/furnace/seg_opr/seg_oprs.py:34,42), the
-// BasicBlock bn1/bn2 + residual add + ReLU (/root/reference/furnace/base_model/resnet.py:33-53) and the
+// Training-mode BatchNorm pieces on NHWC bf16 activations (fp32 statistics), sm_90a.
+// Replaces norm_layer(...) of ConvBnRelu (TorchSeg furnace/seg_opr/seg_oprs.py:34,42), the
+// BasicBlock bn1/bn2 + residual add + ReLU (TorchSeg furnace/base_model/resnet.py:33-53) and the
 // statistics half of apex SyncBatchNorm (train.py:54-55).  All HBM-bound: 16-byte vector accesses,
-// per-channel reductions through shared memory + one fp32 atomic per (CTA, channel).
+// per-channel reductions through shared memory + one workspace slot per CTA, summed in CTA order (tsb_det_reduce).
 #include "nhwc_vec.cuh"
-#include "sm100_ptx.cuh"
 
 namespace {
-using sm100::red_add_v4;
 constexpr int kThreads = 256;
+
+// Per-CTA partial sums go to slot blockIdx.x of the deterministic workspace (tsb_det_reduce sums the slots in order).
+__device__ __forceinline__ void store_part_v4(float* base, long long stride, float a, float b, float c, float d) {
+    *reinterpret_cast<float4*>(base + blockIdx.x * stride) = make_float4(a, b, c, d);
+}
 
 // Generic per-channel column reduction over [npix, C] with NACC accumulators per channel.
 // Functor: f(pix, c8, float acc[NACC][8]) accumulates one 8-channel vector of one pixel.
 template <int NACC, typename F>
-__device__ __forceinline__ void column_reduce(long long npix, int C8, float* const (&outs)[NACC], F f) {
+__device__ __forceinline__ void column_reduce(long long npix, int C8, float* const (&outs)[NACC], long long part_stride, F f) {
     extern __shared__ float s_buf[];  // [lanes][groups][NACC][8]
     const int groups = min(C8, kThreads);
     const int lanes = kThreads / groups;
@@ -46,7 +49,7 @@ __device__ __forceinline__ void column_reduce(long long npix, int C8, float* con
 #pragma unroll
                     for (int k = 0; k < 4; ++k) s[k] += s_buf[(l * groups + g) * NACC * 8 + quad * 4 + k];
                 }
-                red_add_v4(outs[quad / 2] + cg * 8 + (quad % 2) * 4, s[0], s[1], s[2], s[3]);
+                store_part_v4(outs[quad / 2] + cg * 8 + (quad % 2) * 4, part_stride, s[0], s[1], s[2], s[3]);
             }
         }
         __syncthreads();
@@ -54,9 +57,9 @@ __device__ __forceinline__ void column_reduce(long long npix, int C8, float* con
 }
 
 __global__ void __launch_bounds__(kThreads)
-bn_stats_kernel(const __nv_bfloat16* __restrict__ x, int cs, long long npix, int C8, float* sum, float* sumsq) {
+bn_stats_kernel(const __nv_bfloat16* __restrict__ x, int cs, long long npix, int C8, float* sum, float* sumsq, long long part_stride) {
     float* const outs[2] = {sum, sumsq};
-    column_reduce<2>(npix, C8, outs, [&](long long p, int cg, float (&acc)[2][8]) {
+    column_reduce<2>(npix, C8, outs, part_stride, [&](long long p, int cg, float (&acc)[2][8]) {
         float v[8];
         Vec8<__nv_bfloat16>::load(x + p * cs + cg * 8, v);
 #pragma unroll
@@ -160,7 +163,7 @@ __global__ void __launch_bounds__(kThreads)
 bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_bfloat16* __restrict__ y, int ycs,
                      const __nv_bfloat16* __restrict__ x, int xcs, const float* __restrict__ mean,
                      const float* __restrict__ invstd, const float* __restrict__ scale, const float* __restrict__ shift,
-                     long long npix, int C8, float* sum_dz, float* sum_dz_xhat) {
+                     long long npix, int C8, float* sum_dz, float* sum_dz_xhat, long long part_stride) {
     // inner loop: acc0 += dz, acc1 += dz*x (no per-pixel parameter loads); Σ dz·x̂ = invstd·(acc1 − mean·acc0) is
     // formed once per (block, channel) when the partial sums are flushed.
     extern __shared__ float s_buf[];  // [lanes][groups][2][8]
@@ -234,9 +237,7 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_
             }
         }
         __syncthreads();
-        // flush: one 16-byte red.global.add.v4.f32 per 4 channels and accumulator. All CTAs of the grid hit the same
-        // 2*C floats, i.e. a handful of L2 slices: scalar atomics (2*C*grid = 150 k for C = 64) serialised there and
-        // cost a fixed ~20 us per launch; the vector form issues a quarter of the operations.
+        // flush: one 16-byte store per 4 channels and accumulator into this CTA's workspace slot
         if (cg < C8 && lane < lanes) {
             for (int h = lane; h < 2; h += lanes) {
                 float t0[4] = {0.f, 0.f, 0.f, 0.f}, t1[4] = {0.f, 0.f, 0.f, 0.f};
@@ -250,8 +251,8 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_
                 const int c = cg * 8 + h * 4;
                 const float4 m = __ldg(reinterpret_cast<const float4*>(mean + c));
                 const float4 is = __ldg(reinterpret_cast<const float4*>(invstd + c));
-                red_add_v4(sum_dz + c, t0[0], t0[1], t0[2], t0[3]);
-                red_add_v4(sum_dz_xhat + c, is.x * (t1[0] - m.x * t0[0]), is.y * (t1[1] - m.y * t0[1]),
+                store_part_v4(sum_dz + c, part_stride, t0[0], t0[1], t0[2], t0[3]);
+                store_part_v4(sum_dz_xhat + c, part_stride, is.x * (t1[0] - m.x * t0[0]), is.y * (t1[1] - m.y * t0[1]),
                            is.z * (t1[2] - m.z * t0[2]), is.w * (t1[3] - m.w * t0[3]));
             }
         }
@@ -415,7 +416,7 @@ chan_scale_bwd_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv
             for (int slot = lane; slot < 8; slot += lanes) {
                 float s = 0.f;
                 for (int l = 0; l < lanes; ++l) s += s_buf[(l * groups + g) * 8 + slot];
-                atomicAdd(da + (long long)n * C8 * 8 + cg * 8 + slot, s);
+                da[blockIdx.x * (long long)gridDim.y * C8 * 8 + (long long)n * C8 * 8 + cg * 8 + slot] = s;   // workspace slot
             }
         }
         __syncthreads();
@@ -440,13 +441,17 @@ static inline int colred_grid(long long npix, int C8) {
 
 #define TSB_VEC_OK(C, cs, ptr) ((C) % 8 == 0 && (cs) % 8 == 0 && tsb_aligned16(ptr))
 
-extern "C" int tsb_bn_stats(const void* x, int cs, long long npix, int C, float* sum, float* sumsq, tsb_stream_t stream) {
+extern "C" int tsb_bn_stats(const void* x, int cs, long long npix, int C, float* sum, float* sumsq, float* ws,
+                            long long ws_floats, tsb_stream_t stream) {
     TSB_REQUIRE(x && sum && sumsq && npix > 0, "tsb_bn_stats: bad args");
     TSB_REQUIRE(TSB_VEC_OK(C, cs, x), "tsb_bn_stats: C and cs must be multiples of 8");
     int C8 = C / 8;
-    bn_stats_kernel<<<colred_grid(npix, C8), kThreads, colred_smem(C8, 2), (cudaStream_t)stream>>>((const __nv_bfloat16*)x, cs, npix, C8, sum, sumsq);
+    const int grid = colred_grid(npix, C8);
+    TSB_REQUIRE(ws && (long long)grid * 2 * C <= ws_floats, "tsb_bn_stats: workspace needs %lld floats", (long long)grid * 2 * C);
+    bn_stats_kernel<<<grid, kThreads, colred_smem(C8, 2), (cudaStream_t)stream>>>((const __nv_bfloat16*)x, cs, npix, C8, ws, ws + C, 2LL * C);
     TSB_CUDA_CHECK_LAUNCH("bn_stats");
-    return TSB_OK;
+    int rc = tsb_det_reduce(sum, ws, grid, C, 2LL * C, (cudaStream_t)stream);
+    return rc ? rc : tsb_det_reduce(sumsq, ws + C, grid, C, 2LL * C, (cudaStream_t)stream);
 }
 
 extern "C" int tsb_bn_finalize(const float* sum, const float* sumsq, double count, int C, const float* gamma,
@@ -476,18 +481,22 @@ extern "C" int tsb_bn_apply(const void* x, int xcs, const float* scale, const fl
 
 extern "C" int tsb_bn_bwd_reduce(const void* dy, int dycs, const void* y, int ycs, const void* x, int xcs,
                                  const float* mean, const float* invstd, int relu, long long npix, int C, float* sum_dz,
-                                 float* sum_dz_xhat, const float* scale, const float* shift, tsb_stream_t stream) {
+                                 float* sum_dz_xhat, const float* scale, const float* shift, float* ws, long long ws_floats,
+                                 tsb_stream_t stream) {
     TSB_REQUIRE(dy && x && mean && invstd && sum_dz && sum_dz_xhat && npix > 0, "tsb_bn_bwd_reduce: bad args");
     const int mode = !relu ? 0 : (y ? 1 : 2);
     TSB_REQUIRE(mode != 2 || (scale && shift), "tsb_bn_bwd_reduce: relu without y needs scale and shift");
     TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && (mode != 1 || TSB_VEC_OK(C, ycs, y)), "tsb_bn_bwd_reduce: alignment");
     int C8 = C / 8;
     cudaStream_t st = (cudaStream_t)stream;
-#define L(M) bn_bwd_reduce_kernel<M><<<colred_grid(npix, C8), kThreads, colred_smem(C8, 2), st>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)y, ycs, (const __nv_bfloat16*)x, xcs, mean, invstd, scale, shift, npix, C8, sum_dz, sum_dz_xhat)
+    const int grid = colred_grid(npix, C8);
+    TSB_REQUIRE(ws && (long long)grid * 2 * C <= ws_floats, "tsb_bn_bwd_reduce: workspace needs %lld floats", (long long)grid * 2 * C);
+#define L(M) bn_bwd_reduce_kernel<M><<<grid, kThreads, colred_smem(C8, 2), st>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)y, ycs, (const __nv_bfloat16*)x, xcs, mean, invstd, scale, shift, npix, C8, ws, ws + C, 2LL * C)
     if (mode == 0) L(0); else if (mode == 1) L(1); else L(2);
 #undef L
     TSB_CUDA_CHECK_LAUNCH("bn_bwd_reduce");
-    return TSB_OK;
+    int rc = tsb_det_reduce(sum_dz, ws, grid, C, 2LL * C, st);
+    return rc ? rc : tsb_det_reduce(sum_dz_xhat, ws + C, grid, C, 2LL * C, st);
 }
 
 extern "C" int tsb_bn_bwd_apply(const void* dy, int dycs, const void* y, int ycs, const void* x, int xcs,
@@ -531,7 +540,8 @@ extern "C" int tsb_chan_scale_fwd(const void* x, int xcs, const float* a, float 
 }
 
 extern "C" int tsb_chan_scale_bwd(const void* dy, int dycs, const void* x, int xcs, const float* a, float base, void* dx,
-                                  int dxcs, float* da, int N, int HW, int C, tsb_stream_t stream) {
+                                  int dxcs, float* da, int N, int HW, int C, float* ws, long long ws_floats,
+                                  tsb_stream_t stream) {
     TSB_REQUIRE(dy && x && a && dx && da && N > 0 && HW > 0, "tsb_chan_scale_bwd: bad args");
     TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, dxcs, dx) && tsb_aligned16(a), "tsb_chan_scale_bwd: alignment");
     int C8 = C / 8;
@@ -541,7 +551,8 @@ extern "C" int tsb_chan_scale_bwd(const void* dy, int dycs, const void* x, int x
     int cap = (tsb_num_sms() * 8 + N - 1) / N;
     if (chunks > cap) chunks = cap;
     if (chunks < 1) chunks = 1;
-    chan_scale_bwd_kernel<<<dim3(chunks, N), kThreads, colred_smem(C8, 1), (cudaStream_t)stream>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)x, xcs, a, base, (__nv_bfloat16*)dx, dxcs, da, HW, C8);
+    TSB_REQUIRE(ws && (long long)chunks * N * C <= ws_floats, "tsb_chan_scale_bwd: workspace needs %lld floats", (long long)chunks * N * C);
+    chan_scale_bwd_kernel<<<dim3(chunks, N), kThreads, colred_smem(C8, 1), (cudaStream_t)stream>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)x, xcs, a, base, (__nv_bfloat16*)dx, dxcs, ws, HW, C8);
     TSB_CUDA_CHECK_LAUNCH("chan_scale_bwd");
-    return TSB_OK;
+    return tsb_det_reduce(da, ws, chunks, (long long)N * C, (long long)N * C, (cudaStream_t)stream);
 }

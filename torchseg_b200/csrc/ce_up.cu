@@ -1,6 +1,6 @@
 // Fused bilinear up-sampling (align_corners=True, to an explicit output size) + cross-entropy with ignore index for MANY
 // classes (32 < C <= 152: ADE20K's 150) — replaces `F.interpolate(...)` → `log_softmax` → `nn.CrossEntropyLoss` of the PSPNet /
-// PSANet heads (/root/reference/model/pspnet/ade.pspnet.R101_v1c/network.py:46-57, psanet network.py:46-55) without ever
+// PSANet heads (TorchSeg model/pspnet/ade.pspnet.R101_v1c/network.py:46-57, psanet network.py:46-55) without ever
 // writing the [B,150,H,W] fp32 logits: materialised, those cost ~24 GB of HBM traffic per head and step at 16 x 713 x 713
 // (write, two reads, gradient write, gradient read).
 //

@@ -1,26 +1,25 @@
-// Persistent implicit-GEMM convolution (fprop / dgrad / stem), second generation.
+// Persistent implicit-GEMM convolution (fprop / dgrad / stem) on Hopper wgmma (sm_90a).
 //
-// Versus igemm_kmajor_kernel (conv_tcgen05.cu):
-//   * persistent CTAs (one per SM) striding over output tiles of one N-tile → prologue (barriers, TMEM alloc,
-//     descriptor prefetch) paid once, BN statistics accumulated in shared memory across all tiles of the CTA;
+//   * persistent CTAs (one per SM) striding over output tiles of one N-tile → prologue (barriers, descriptor prefetch)
+//     paid once, BN statistics accumulated in registers across all tiles of the CTA;
 //   * the B operand (packed weights of this N-tile) stays RESIDENT in shared memory when it fits (C=64 layers,
 //     1x1 convs, stems) instead of being re-fetched from L2 for every tile;
 //   * ROW tiles (TH = 1, TW = 128): the horizontal taps of one filter row share ONE TMA box of TW+span pixels; the
-//     taps are addressed by shifting the UMMA descriptor start by whole 128-byte rows (descriptor base_offset =
-//     (addr >> 7) & 7), cutting the L2→SM activation traffic of a 3x3 layer 3x;
-//   * two TMEM accumulator buffers: the epilogue of tile i overlaps the MMAs of tile i+1.
+//     taps are addressed by shifting the wgmma descriptor start by whole 128-byte rows, cutting the L2→SM activation
+//     traffic of a 3x3 layer 3x.
+// Warp roles: warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of the 128-pixel tile: wgmma into register
+// accumulators, then the epilogue straight from the fragments), warp 8 = TMA producer.
 #include "conv_common.cuh"
 #include "conv_v2.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
-using namespace sm100;
+using namespace sm90;
 using namespace convhost;
 
 namespace {
 
-__device__ __forceinline__ uint32_t r_as_u(float f) { return __float_as_uint(f); }
-
-constexpr int kThreads = 384;  // 4 control warps + 8 epilogue warps
+constexpr int kConsumers = 2;                          // warpgroups
+constexpr int kThreads = kConsumers * 128 + 32;        // + one producer warp
 constexpr int kMaxStages = 8;
 constexpr int kAStageBytes = 17 * 1024;  // (128 + 8) pixel rows x 128 B, rounded up to a 1024-byte multiple
 
@@ -42,22 +41,24 @@ struct alignas(64) V2Params {
     int P, Q;
     long long out_n_stride, out_p_stride, out_q_stride, out_base;
     int k_real, k_store, out_f32, accumulate;
-    int wide_io;   // every output pixel row is 32-byte aligned → 256-bit epilogue loads / stores
     int relu;      // inference epilogue: y = max(acc + bias (+ res), 0)
     const void* res;   // optional bf16 residual with the OUTPUT's addressing (same strides / base), added before the ReLU
     const float* bias;
     float* sum;
     float* sumsq;
+    float* part;   // [gridDim.x][2][k_real] per-CTA statistics, summed in CTA order by tsb_det_reduce
     void* out;
     // shared-memory plan
     int nstages, stage_bytes, res_bytes, use_base_offset;
 };
 
-// PAIR (streamed B, BN = 128 only): two pixel tiles share every weight tile — one stage carries two A boxes and the B
-// taps, the issuer runs the MMAs of both tiles against the same B operand (four TMEM accumulators, 512 columns). The
-// L2→SM traffic per FLOP of the weight-streaming layers drops ~37 % (3x3: 82 KB per 12.6 MFLOP instead of 65 KB per
-// 6.3); at the measured ~43 B/clk/SM of TMA ingest that traffic, not the tensor pipe, bounds these layers.
-template <int BN, bool RES, bool PAIR>
+template <int BN>
+__device__ __forceinline__ void wgmma_kmajor(float (&d)[BN / 2], uint64_t da, uint64_t db) {
+    if constexpr (BN == 64) wgmma_m64n64<0, 0>(d, da, db, 1u);
+    else wgmma_m64n128<0, 0>(d, da, db, 1u);
+}
+
+template <int BN, bool RES>
 __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_constant__ V2Params p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -66,36 +67,25 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
     uint8_t* tail = stages + p.nstages * p.stage_bytes;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
     uint64_t* empty_bar = full_bar + kMaxStages;
-    uint64_t* tmem_full = empty_bar + kMaxStages;  // [2]
-    uint64_t* tmem_empty = tmem_full + 2;          // [2]
-    uint64_t* b_ready = tmem_empty + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(b_ready + 1);
-    float* s_stats = reinterpret_cast<float*>(tail + 256);  // [2*BN]
-    uint32_t* s_tr = reinterpret_cast<uint32_t*>(tail + 256 + 2 * BN * 4);  // [8 warps][32][17] bf16x2 transposition
+    uint64_t* b_ready = empty_bar + kMaxStages;
+    float* s_stats = reinterpret_cast<float*>(tail + 256);  // [consumer warp][2*BN]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n0 = blockIdx.y * BN;
     const int my_tiles = (p.m_tiles > (int)blockIdx.x) ? (p.m_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-    const int iters_per_tile = p.ngroups * p.kchunks;
     constexpr int kBTile = BN * 128;
+    constexpr int kProducer = kConsumers * 4;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducer && lane == 0) {
         tma_prefetch_desc(&p.mapB);
         tma_prefetch_desc(&p.mapA[0]);
-        for (int s = 0; s < p.nstages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], 8); }
+        for (int s = 0; s < p.nstages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumers * 4); }
         mbar_init(b_ready, 1);
         fence_barrier_init();
-    } else if (warp == 2) {
-        tmem_alloc<(PAIR ? 4 : 2) * BN>(tmem_ptr);
-        for (int i = lane; i < 2 * BN; i += 32) s_stats[i] = 0.f;
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
+    if (warp == kProducer) {
         if (lane == 0 && my_tiles > 0) {
             if (RES) {  // weights of this N-tile: loaded once per CTA
                 mbar_arrive_expect_tx(b_ready, (uint32_t)(p.ntaps_total * p.kchunks * kBTile));
@@ -105,47 +95,9 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
                             tma_load_2d(res_b + (p.groups[g].tap_idx[t] * p.kchunks + kc) * kBTile, &p.mapB, b_ready,
                                         p.groups[g].bk[t] + kc * 64, n0);
             }
-            if (PAIR) {
-                // one ring; pair j = local tiles (2j, 2j+1): A0 | A1 | B taps per stage
-                int sl = 0;
-                uint32_t ph = 0;
-                const int npairs = (my_tiles + 1) >> 1;
-                for (int j = 0; j < npairs; ++j) {
-                    int q0[2], p0[2], nimg[2];
-#pragma unroll
-                    for (int u = 0; u < 2; ++u) {
-                        const int li = (2 * j + u < my_tiles) ? 2 * j + u : 2 * j;   // odd tail: duplicate tile, never stored
-                        const int tile = blockIdx.x + li * gridDim.x;
-                        q0[u] = (tile % p.tiles_w) * p.TW;
-                        p0[u] = ((tile / p.tiles_w) % p.tiles_h) * p.TH;
-                        nimg[u] = tile / (p.tiles_w * p.tiles_h);
-                    }
-                    for (int g = 0; g < p.ngroups; ++g) {
-                        const int gmap = p.groups[g].map, ntaps = p.groups[g].ntaps;
-                        const uint32_t bytes = 2u * (uint32_t)p.a_bytes[gmap] + (uint32_t)(ntaps * kBTile);
-                        for (int kc = 0; kc < p.kchunks; ++kc) {
-                            mbar_wait(&empty_bar[sl], ph ^ 1u);
-                            uint8_t* a_s = stages + sl * p.stage_bytes;
-                            mbar_arrive_expect_tx(&full_bar[sl], bytes);
-                            tma_load_4d(a_s, &p.mapA[gmap], &full_bar[sl], kc * 64, q0[0] + p.groups[g].dw0, p0[0] + p.groups[g].dh, nimg[0]);
-                            tma_load_4d(a_s + kAStageBytes, &p.mapA[gmap], &full_bar[sl], kc * 64, q0[1] + p.groups[g].dw0, p0[1] + p.groups[g].dh, nimg[1]);
-                            for (int t = 0; t < ntaps; ++t)
-                                tma_load_2d(a_s + 2 * kAStageBytes + t * kBTile, &p.mapB, &full_bar[sl], p.groups[g].bk[t] + kc * 64, n0);
-                            if (++sl == p.nstages) { sl = 0; ph ^= 1u; }
-                        }
-                    }
-                }
-            } else {
-            // two stage rings (one per MMA-issuing thread) when there are >= 4 stages: tile i uses ring i & 1
-            const bool dual_p = p.nstages >= 4;
-            const int half_p = dual_p ? p.nstages / 2 : p.nstages;
-            int cs0 = 0, cs1 = 0;
-            uint32_t cp0 = 0, cp1 = 0;
+            int sl = 0;
+            uint32_t ph = 0;
             for (int i = 0; i < my_tiles; ++i) {
-                const bool r1 = dual_p && (i & 1);
-                int sl = r1 ? cs1 : cs0;
-                uint32_t ph = r1 ? cp1 : cp0;
-                const int sbase = r1 ? half_p : 0;
                 const int tile = blockIdx.x + i * gridDim.x;
                 const int tw_i = tile % p.tiles_w;
                 const int th_i = (tile / p.tiles_w) % p.tiles_h;
@@ -156,327 +108,155 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
                     const int cw = q0 + p.groups[g].dw0, chh = p0 + p.groups[g].dh;
                     const uint32_t bytes = (uint32_t)p.a_bytes[gmap] + (RES ? 0u : (uint32_t)(ntaps * kBTile));
                     for (int kc = 0; kc < p.kchunks; ++kc) {
-                        const int s = sbase + sl;
-                        mbar_wait(&empty_bar[s], ph ^ 1u);
-                        uint8_t* a_s = stages + s * p.stage_bytes;
-                        mbar_arrive_expect_tx(&full_bar[s], bytes);
-                        tma_load_4d(a_s, &p.mapA[gmap], &full_bar[s], kc * 64, cw, chh, n_img);
+                        mbar_wait(&empty_bar[sl], ph ^ 1u);
+                        uint8_t* a_s = stages + sl * p.stage_bytes;
+                        mbar_arrive_expect_tx(&full_bar[sl], bytes);
+                        tma_load_4d(a_s, &p.mapA[gmap], &full_bar[sl], kc * 64, cw, chh, n_img);
                         if (!RES) {
                             for (int t = 0; t < ntaps; ++t)
-                                tma_load_2d(a_s + kAStageBytes + t * kBTile, &p.mapB, &full_bar[s], p.groups[g].bk[t] + kc * 64, n0);
+                                tma_load_2d(a_s + kAStageBytes + t * kBTile, &p.mapB, &full_bar[sl], p.groups[g].bk[t] + kc * 64, n0);
                         }
-                        if (++sl == half_p) { sl = 0; ph ^= 1u; }
+                        if (++sl == p.nstages) { sl = 0; ph ^= 1u; }
                     }
                 }
-                if (r1) { cs1 = sl; cp1 = ph; } else { cs0 = sl; cp0 = ph; }
             }
-            }  // !PAIR
         }
-    } else if (warp == 1 || warp == 3) {
-        // TWO MMA-issuing threads (one elected lane each): warp 1 takes the even local tiles (TMEM buffer 0), warp 3
-        // the odd ones (buffer 1). A single thread cannot issue N=64 MMAs fast enough to keep the tensor pipe busy;
-        // the per-MMA work is reduced to two 64-bit descriptor adds.
-        // Each issuing thread owns its own stage ring (single producer / single consumer per ring), so the mbarrier
-        // parity waits can never alias an older phase whatever the K-loop length. With < 4 stages warp 1 works alone.
-        const bool dual = !PAIR && p.nstages >= 4;
-        const int half = dual ? p.nstages / 2 : p.nstages;
-        const int par = (warp == 3) ? 1 : 0;
-        const int tstep = dual ? 2 : 1;
-        if (lane == 0 && my_tiles > par && (dual || warp == 1)) {
-            constexpr uint32_t idesc = make_idesc_bf16(128, BN, false, false);
-            // descriptor with a zero start address: LBO = 16 B, SBO = 1024 B, version 1, SWIZZLE_128B
-            const uint64_t desc_hi = make_smem_desc_sw128(0, 16, 1024);
-            const uint32_t stages_u32 = smem_u32(stages);
-            const uint32_t res_u32 = smem_u32(res_b);
-            if (RES) { mbar_wait(b_ready, 0); tc_fence_after(); }
-            const int sbase = (dual && par) ? half : 0;
-            int sl = 0;
-            uint32_t ph = 0;
-            if (PAIR) {
-                const int npairs = (my_tiles + 1) >> 1;
-                for (int j = 0; j < npairs; ++j) {
-                    const int pb = j & 1;
-                    mbar_wait(&tmem_empty[pb], (((uint32_t)j >> 1) & 1u) ^ 1u);  // epilogue drained both tiles of pair j-2
-                    tc_fence_after();
-                    const uint32_t d0 = tmem_base + (uint32_t)(pb * 2) * BN, d1 = d0 + BN;
-                    uint32_t acc = 0;
-                    for (int g = 0; g < p.ngroups; ++g) {
-                        const int ntaps = p.groups[g].ntaps;
-                        for (int kc = 0; kc < p.kchunks; ++kc) {
-                            mbar_wait(&full_bar[sl], ph);
-                            tc_fence_after();
-                            const uint32_t a_lo = (stages_u32 + (uint32_t)(sl * p.stage_bytes)) >> 4;
-#pragma unroll
-                            for (int t = 0; t < 3; ++t) {
-                                if (t < ntaps) {
-                                    const uint64_t da0 = desc_hi | (uint64_t)(a_lo + (uint32_t)p.groups[g].row_off[t] * 8u);
-                                    const uint64_t da1 = da0 + (uint64_t)(kAStageBytes >> 4);
-                                    const uint64_t db = desc_hi | (uint64_t)(a_lo + (uint32_t)((2 * kAStageBytes + t * kBTile) >> 4));
-                                    umma_bf16(d0, da0, db, idesc, acc);
-                                    umma_bf16(d0, da0 + 2, db + 2, idesc, 1u);
-                                    umma_bf16(d0, da0 + 4, db + 4, idesc, 1u);
-                                    umma_bf16(d0, da0 + 6, db + 6, idesc, 1u);
-                                    umma_bf16(d1, da1, db, idesc, acc);
-                                    umma_bf16(d1, da1 + 2, db + 2, idesc, 1u);
-                                    umma_bf16(d1, da1 + 4, db + 4, idesc, 1u);
-                                    umma_bf16(d1, da1 + 6, db + 6, idesc, 1u);
-                                    acc = 1u;
-                                }
-                            }
-                            umma_commit(&empty_bar[sl]);
-                            if (++sl == p.nstages) { sl = 0; ph ^= 1u; }
-                        }
-                    }
-                    umma_commit(&tmem_full[pb]);
-                }
-            } else {
-            for (int i = par; i < my_tiles; i += tstep) {
-                const int buf = i & 1;
-                mbar_wait(&tmem_empty[buf], (((uint32_t)i >> 1) & 1u) ^ 1u);  // epilogue drained this buffer
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + buf * BN;
-                uint32_t acc = 0;
-                for (int g = 0; g < p.ngroups; ++g) {
-                    const int ntaps = p.groups[g].ntaps;
-                    for (int kc = 0; kc < p.kchunks; ++kc) {
-                        const int s = sbase + sl;
-                        mbar_wait(&full_bar[s], ph);
-                        tc_fence_after();
-                        const uint32_t a_lo = (stages_u32 + (uint32_t)(s * p.stage_bytes)) >> 4;
-#pragma unroll
-                        for (int t = 0; t < 3; ++t) {
-                            if (t < ntaps) {
-                                const uint64_t da = desc_hi | (uint64_t)(a_lo + (uint32_t)p.groups[g].row_off[t] * 8u);
-                                const uint32_t b_lo = RES ? (res_u32 + (uint32_t)((p.groups[g].tap_idx[t] * p.kchunks + kc) * kBTile)) >> 4
-                                                          : a_lo + (uint32_t)((kAStageBytes + t * kBTile) >> 4);
-                                const uint64_t db = desc_hi | (uint64_t)b_lo;
-                                umma_bf16(d_tmem, da, db, idesc, acc);
-                                umma_bf16(d_tmem, da + 2, db + 2, idesc, 1u);
-                                umma_bf16(d_tmem, da + 4, db + 4, idesc, 1u);
-                                umma_bf16(d_tmem, da + 6, db + 6, idesc, 1u);
-                                acc = 1u;
-                            }
-                        }
-                        umma_commit(&empty_bar[s]);
-                        if (++sl == half) { sl = 0; ph ^= 1u; }
-                    }
-                }
-                umma_commit(&tmem_full[buf]);
-            }
-            }  // !PAIR
-        }
-    } else if (warp >= 4) {
-        // 8 epilogue warps. TMEM lane quarter = warp % 4 (hardware rule); the column range is split by (warp-4)/4:
-        //   BN = 64 : each warp owns ONE 32-column chunk of every tile → BN statistics are plain per-thread running
-        //             sums over all tiles of the CTA (no shuffles / atomics per tile), reduced once at the end;
-        //   BN = 128: each warp owns a 64-column half (2 chunks) with a per-tile shuffle reduce-scatter.
-        const int quarter = warp & 3;
-        const int chalf = (warp - 4) >> 2;
-        const int m = quarter * 32 + lane;
+    } else {
+        // consumer warpgroup c owns pixel rows [64c, 64c + 64) of every tile; thread fragment rows m0 and m0 + 8
+        const int c = warp >> 2, wq = warp & 3;
+        const int m0 = c * 64 + wq * 16 + (lane >> 2);
+        const int cq = 2 * (lane & 3);                 // first of the thread's two columns in every 8-column group
         const bool do_stats = (p.sum != nullptr);
-        constexpr bool kRunning = (BN == 64);
-        constexpr int kChunksPerWarp = kRunning ? 1 : 2;
-        float run1[kRunning ? 32 : 2], run2[kRunning ? 32 : 2];
+        const uint64_t desc_hi = desc_hi_sw128(16, 1024);   // K-major, 8-row groups 1024 B apart
+        const uint32_t stages_lo = smem_u32(stages) >> 4;
+        const uint32_t res_lo = smem_u32(res_b) >> 4;
+        float run1[BN / 4], run2[BN / 4];   // running column sums over all tiles of the CTA (columns 8j + cq + e)
 #pragma unroll
-        for (int q = 0; q < (kRunning ? 32 : 2); ++q) { run1[q] = 0.f; run2[q] = 0.f; }
+        for (int q = 0; q < BN / 4; ++q) { run1[q] = 0.f; run2[q] = 0.f; }
+        if (RES && my_tiles > 0) mbar_wait(b_ready, 0);
+        int sl = 0;
+        uint32_t ph = 0;
         for (int i = 0; i < my_tiles; ++i) {
+            float acc[BN / 2];
+#pragma unroll
+            for (int q = 0; q < BN / 2; ++q) acc[q] = 0.f;
+            for (int g = 0; g < p.ngroups; ++g) {
+                const int ntaps = p.groups[g].ntaps;
+                for (int kc = 0; kc < p.kchunks; ++kc) {
+                    mbar_wait(&full_bar[sl], ph);
+                    fence_operands(acc);
+                    wgmma_fence();
+                    const uint32_t st_lo = stages_lo + (uint32_t)(sl * p.stage_bytes >> 4);
+#pragma unroll
+                    for (int t = 0; t < 3; ++t) {
+                        if (t < ntaps) {
+                            const uint32_t a_lo = st_lo + (uint32_t)c * 512u + (uint32_t)p.groups[g].row_off[t] * 8u;
+                            const uint32_t b_lo = RES ? res_lo + (uint32_t)((p.groups[g].tap_idx[t] * p.kchunks + kc) * kBTile >> 4)
+                                                      : st_lo + (uint32_t)((kAStageBytes + t * kBTile) >> 4);
+#pragma unroll
+                            for (int k = 0; k < 4; ++k)   // 16 bf16 = 32 B = 2 descriptor units inside the swizzle atom
+                                wgmma_kmajor<BN>(acc, desc_at(desc_hi, a_lo + 2 * k, p.use_base_offset),
+                                                 desc_at(desc_hi, b_lo + 2 * k, 0));
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_operands(acc);
+                    // wait_group covers only this warp's MMAs: every consumer warp releases the stage
+                    if (lane == 0) mbar_arrive(&empty_bar[sl]);
+                    if (++sl == p.nstages) { sl = 0; ph ^= 1u; }
+                }
+            }
             const int tile = blockIdx.x + i * gridDim.x;
             const int tw_i = tile % p.tiles_w;
             const int th_i = (tile / p.tiles_w) % p.tiles_h;
             const int n_img = tile / (p.tiles_w * p.tiles_h);
-            const int pp = th_i * p.TH + (m >> p.tw_shift), qq = tw_i * p.TW + (m & (p.TW - 1));
-            const bool valid = (pp < p.P) && (qq < p.Q);
-            const long long pix_off = p.out_base + (long long)n_img * p.out_n_stride + (long long)pp * p.out_p_stride +
-                                      (long long)qq * p.out_q_stride;
-            // PAIR: accumulator (i & 3) of four, full/empty barriers per pair; otherwise buffer i & 1 of two
-            const int buf = PAIR ? ((i >> 1) & 1) : (i & 1);
-            const int acc_slot = PAIR ? (((i >> 1) & 1) * 2 + (i & 1)) : (i & 1);
-            const bool wait_full = PAIR ? ((i & 1) == 0) : true;
-            const bool last_of_buf = PAIR ? ((i & 1) == 1 || i == my_tiles - 1) : true;
-            if (iters_per_tile > 0 && wait_full) {
-                mbar_wait(&tmem_full[buf], (PAIR ? ((uint32_t)i >> 2) : ((uint32_t)i >> 1)) & 1u);
-                tc_fence_after();
-            }
-            const uint32_t taddr = tmem_base + acc_slot * BN + ((uint32_t)(quarter * 32) << 16);
-#pragma unroll 1
-            for (int jj = 0; jj < kChunksPerWarp; ++jj) {
-                const int j = chalf * kChunksPerWarp + jj;
-                uint32_t r[32];
-                if (iters_per_tile > 0) {
-                    tmem_ld_32x32b_x32(taddr + j * 32, r);
-                    tmem_ld_wait();
-                } else {
 #pragma unroll
-                    for (int q = 0; q < 32; ++q) r[q] = 0u;
-                }
-                if (jj == kChunksPerWarp - 1 && last_of_buf) {  // this warp's TMEM reads of the tile (pair) are done
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-                }
-                const int col0 = n0 + j * 32;
-                float v[32];
+            for (int h = 0; h < 2; ++h) {
+                const int m = m0 + 8 * h;
+                const int pp = th_i * p.TH + (m >> p.tw_shift), qq = tw_i * p.TW + (m & (p.TW - 1));
+                const bool valid = (pp < p.P) && (qq < p.Q);
+                const long long pix_off = p.out_base + (long long)n_img * p.out_n_stride + (long long)pp * p.out_p_stride +
+                                          (long long)qq * p.out_q_stride;
 #pragma unroll
-                for (int q = 0; q < 32; ++q) v[q] = __uint_as_float(r[q]);
-                if (p.bias != nullptr) {
-#pragma unroll
-                    for (int q = 0; q < 32; ++q)
-                        if (col0 + q < p.k_real) v[q] += __ldg(p.bias + col0 + q);
-                }
-                if (p.res != nullptr && valid) {     // folded-BN inference tail of a residual block: + shortcut
-                    const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.res) + pix_off + col0;
-#pragma unroll
-                    for (int g = 0; g < 4; ++g)
-                        if (col0 + g * 8 < p.k_store) {
-                            float rv[8];
-                            unpack8(*reinterpret_cast<const uint4*>(rp + g * 8), rv);
-#pragma unroll
-                            for (int q = 0; q < 8; ++q) v[g * 8 + q] += rv[q];
-                        }
-                }
-                if (p.relu) {
-#pragma unroll
-                    for (int q = 0; q < 32; ++q) v[q] = fmaxf(v[q], 0.f);
-                }
-                if (p.out_f32) {
-                    float* o = reinterpret_cast<float*>(p.out) + pix_off + col0;
-                    if (valid) {
-#pragma unroll
-                        for (int g = 0; g < 4; ++g) {
-                            if (p.wide_io && col0 + g * 8 + 8 <= p.k_store) {     // 8 floats = one full 32-byte sector
-                                stg_v8(o + g * 8,
-                                       make_uint4(r_as_u(v[g * 8]), r_as_u(v[g * 8 + 1]), r_as_u(v[g * 8 + 2]), r_as_u(v[g * 8 + 3])),
-                                       make_uint4(r_as_u(v[g * 8 + 4]), r_as_u(v[g * 8 + 5]), r_as_u(v[g * 8 + 6]), r_as_u(v[g * 8 + 7])));
-                            } else {
-#pragma unroll
-                                for (int hh = 0; hh < 2; ++hh)
-                                    if (col0 + g * 8 + hh * 4 < p.k_store)
-                                        *reinterpret_cast<float4*>(o + g * 8 + hh * 4) =
-                                            make_float4(v[g * 8 + hh * 4], v[g * 8 + hh * 4 + 1], v[g * 8 + hh * 4 + 2], v[g * 8 + hh * 4 + 3]);
-                            }
-                        }
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int col = n0 + 8 * j + cq;     // even; k_store is a multiple of 8, so col + 1 is in range too
+                    float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                    if (p.bias != nullptr) {
+                        if (col < p.k_real) v0 += __ldg(p.bias + col);
+                        if (col + 1 < p.k_real) v1 += __ldg(p.bias + col + 1);
                     }
-                } else {
-                    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + pix_off + col0;
-                    if (p.accumulate && valid) {
-#pragma unroll
-                        for (int g2 = 0; g2 < 2; ++g2) {
-                            if (p.wide_io && col0 + g2 * 16 + 16 <= p.k_store) {
-                                uint4 ua, ub;
-                                ldg_v8(o + g2 * 16, ua, ub);
-                                float old[8];
-                                unpack8(ua, old);
-#pragma unroll
-                                for (int q = 0; q < 8; ++q) v[g2 * 16 + q] += old[q];
-                                unpack8(ub, old);
-#pragma unroll
-                                for (int q = 0; q < 8; ++q) v[g2 * 16 + 8 + q] += old[q];
-                            } else {
-#pragma unroll
-                                for (int hh = 0; hh < 2; ++hh)
-                                    if (col0 + g2 * 16 + hh * 8 < p.k_store) {
-                                        float old[8];
-                                        uint4 u = *reinterpret_cast<const uint4*>(o + g2 * 16 + hh * 8);
-                                        unpack8(u, old);
-#pragma unroll
-                                        for (int q = 0; q < 8; ++q) v[g2 * 16 + hh * 8 + q] += old[q];
-                                    }
-                            }
-                        }
+                    const bool st = valid && col < p.k_store;
+                    if (p.res != nullptr && st) {     // folded-BN inference tail of a residual block: + shortcut
+                        const uint32_t u = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + pix_off + col);
+                        v0 += bf16lo(u);
+                        v1 += bf16hi(u);
                     }
-#pragma unroll
-                    for (int q = 0; q < 32; ++q) v[q] = bf16_round(v[q]);
-                    if (valid) {
-#pragma unroll
-                        for (int g2 = 0; g2 < 2; ++g2) {
-                            if (p.wide_io && col0 + g2 * 16 + 16 <= p.k_store) {   // 16 bf16 = one full 32-byte sector
-                                stg_v8(o + g2 * 16, pack8(&v[g2 * 16]), pack8(&v[g2 * 16 + 8]));
-                            } else {
-#pragma unroll
-                                for (int hh = 0; hh < 2; ++hh)
-                                    if (col0 + g2 * 16 + hh * 8 < p.k_store)
-                                        *reinterpret_cast<uint4*>(o + g2 * 16 + hh * 8) = pack8(&v[g2 * 16 + hh * 8]);
-                            }
-                        }
-                    }
-                }
-                if (do_stats) {
-                    if (kRunning) {
-                        if (valid) {
-#pragma unroll
-                            for (int q = 0; q < 32; ++q) { run1[q] += v[q]; run2[q] = fmaf(v[q], v[q], run2[q]); }
-                        }
+                    if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                    if (p.out_f32) {
+                        if (st) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix_off + col) = make_float2(v0, v1);
                     } else {
-                        // column sums through a bf16x2 shared-memory transposition (conflict-free: pitch 17 words);
-                        // lane c then owns column c and keeps running sums over all tiles of the CTA
-                        uint32_t* tr = s_tr + (warp - 4) * (32 * 17);
-                        __syncwarp();
-#pragma unroll
-                        for (int q = 0; q < 16; ++q) tr[lane * 17 + q] = valid ? pack_bf16(v[2 * q], v[2 * q + 1]) : 0u;
-                        __syncwarp();
-                        float a1 = 0.f, a2 = 0.f;
-                        const int wq = lane >> 1;
-                        const bool hi = (lane & 1) != 0;
-#pragma unroll
-                        for (int rr = 0; rr < 32; ++rr) {
-                            const uint32_t u = tr[rr * 17 + wq];
-                            const float f = hi ? bf16hi(u) : bf16lo(u);
-                            a1 += f;
-                            a2 = fmaf(f, f, a2);
+                        uint32_t* o = reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + pix_off + col);
+                        if (p.accumulate && st) {
+                            const uint32_t u = *o;
+                            v0 += bf16lo(u);
+                            v1 += bf16hi(u);
                         }
-                        run1[jj] += a1;
-                        run2[jj] += a2;
+                        // round once to bf16; statistics are taken of the rounded values the next layer will see
+                        const uint32_t u = pack_bf16(v0, v1);
+                        v0 = bf16lo(u);
+                        v1 = bf16hi(u);
+                        if (st) *o = u;
+                    }
+                    if (do_stats && valid) {
+                        run1[2 * j] += v0; run2[2 * j] = fmaf(v0, v0, run2[2 * j]);
+                        run1[2 * j + 1] += v1; run2[2 * j + 1] = fmaf(v1, v1, run2[2 * j + 1]);
                     }
                 }
             }
         }
         if (do_stats) {
-            if (kRunning) {  // one warp reduce-scatter per CTA instead of one per tile
+            // lanes with the same lane % 4 hold the same columns: reduce over lane / 4, then across warps in smem
 #pragma unroll
-                for (int off = 16; off >= 1; off >>= 1) {
-                    const bool upper = (lane & off) != 0;
+            for (int q = 0; q < BN / 4; ++q) {
 #pragma unroll
-                    for (int q = 0; q < (kRunning ? off : 0); ++q) {
-                        float send1 = upper ? run1[q] : run1[q + off];
-                        float keep1 = upper ? run1[q + off] : run1[q];
-                        float send2 = upper ? run2[q] : run2[q + off];
-                        float keep2 = upper ? run2[q + off] : run2[q];
-                        run1[q] = keep1 + __shfl_xor_sync(0xffffffffu, send1, off);
-                        run2[q] = keep2 + __shfl_xor_sync(0xffffffffu, send2, off);
-                    }
-                }
-                atomicAdd(&s_stats[chalf * 32 + lane], run1[0]);
-                atomicAdd(&s_stats[BN + chalf * 32 + lane], run2[0]);
-            } else {
-#pragma unroll
-                for (int jj = 0; jj < 2; ++jj) {
-                    atomicAdd(&s_stats[(chalf * 2 + jj) * 32 + lane], run1[jj]);
-                    atomicAdd(&s_stats[BN + (chalf * 2 + jj) * 32 + lane], run2[jj]);
+                for (int off = 4; off < 32; off <<= 1) {
+                    run1[q] += __shfl_xor_sync(0xffffffffu, run1[q], off);
+                    run2[q] += __shfl_xor_sync(0xffffffffu, run2[q], off);
                 }
             }
-            asm volatile("bar.sync 1, 256;" ::: "memory");  // the eight epilogue warps only
-            for (int i = threadIdx.x - 128; i < BN; i += 256) {
+            // fixed summation order everywhere (no float atomics): per-warp slots, summed in warp order; the CTA's
+            // totals go to its workspace slot and tsb_det_reduce adds the slots in CTA order
+            if (lane < 4) {
+                float* sw = s_stats + warp * 2 * BN;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        sw[8 * j + cq + e] = run1[2 * j + e];
+                        sw[BN + 8 * j + cq + e] = run2[2 * j + e];
+                    }
+            }
+            asm volatile("bar.sync 1, %0;" ::"n"(kConsumers * 128) : "memory");  // the consumer warpgroups only
+            float* part = p.part + (long long)blockIdx.x * 2 * p.k_real;
+            for (int i = threadIdx.x; i < BN; i += kConsumers * 128) {
                 if (n0 + i < p.k_real) {
-                    atomicAdd(p.sum + n0 + i, s_stats[i]);
-                    atomicAdd(p.sumsq + n0 + i, s_stats[BN + i]);
+                    float t1 = 0.f, t2 = 0.f;
+                    for (int w = 0; w < kConsumers * 4; ++w) { t1 += s_stats[w * 2 * BN + i]; t2 += s_stats[w * 2 * BN + BN + i]; }
+                    part[n0 + i] = t1;
+                    part[p.k_real + n0 + i] = t2;
                 }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc<(PAIR ? 4 : 2) * BN>(tmem_base);
     }
 }
 
 // ------------------------------------------------------------------------------------------------
 // wgrad, row-tile variant: the horizontal taps of one filter row share ONE activation box.
 //   dW[co, (s, ci)] += Σ_px dY[px, co] · X[px + s·step, ci]      for the ntaps (<= 3) taps of the group
-// A = dYᵀ (MN-major, 2 boxes of 64 out-channels), B = ONE box of 64+span pixels x 64 in-channels (MN-major); the
-// taps are the N-groups of a single UMMA B descriptor whose leading-dimension byte offset is step·128 B (the same
-// smem rows, shifted) → N = 64·ntaps without re-loading the activations per tap.
+// A = dYᵀ (MN-major, 2 boxes of 64 out-channels, one per consumer warpgroup), B = ONE box of 64+span pixels x 64
+// in-channels (MN-major); tap t reads the same smem rows shifted by t·step pixels, so the activations are loaded once
+// for all taps of the row. K = 64 pixels per stage.
 // ------------------------------------------------------------------------------------------------
 constexpr int kWrStages = 8;
 constexpr int kWrABytes = 2 * 64 * 128;   // two 64-channel dY boxes of 64 pixels
@@ -495,16 +275,17 @@ struct alignas(64) WrParams {
     int TW;
     int K, C;
     long long dw_row_stride;
-    float* dw;
+    float* dw;                // dW-shaped slice per split (workspace), part_stride apart; or dW itself when `add`
+    long long part_stride;
+    int add;                  // one split: add in place
+    int use_base_offset;
 };
 
-__global__ void __launch_bounds__(256, 1) wgrad_rows_kernel(const __grid_constant__ WrParams p) {
+__global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_constant__ WrParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kWrStages * kWrStageBytes);
     uint64_t* empty_bar = full_bar + kWrStages;
-    uint64_t* tmem_full = empty_bar + kWrStages;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int co0 = blockIdx.y * 128;
     const int g = blockIdx.z / p.cchunks, cc = blockIdx.z - g * p.cchunks;
@@ -512,22 +293,17 @@ __global__ void __launch_bounds__(256, 1) wgrad_rows_kernel(const __grid_constan
     const int t_begin = blockIdx.x * p.tiles_per_split;
     const int t_end = min(p.total_tiles, t_begin + p.tiles_per_split);
     const int total_iters = t_end - t_begin;
+    constexpr int kProducer = kConsumers * 4;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducer && lane == 0) {
         tma_prefetch_desc(&p.mapA);
         tma_prefetch_desc(&p.mapB[G.map]);
-        for (int s = 0; s < kWrStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full, 1);
+        for (int s = 0; s < kWrStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumers * 4); }
         fence_barrier_init();
-    } else if (warp == 2) {
-        tmem_alloc<256>(tmem_ptr);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
+    if (warp == kProducer) {
         if (lane == 0) {
             for (int it = 0; it < total_iters; ++it) {
                 const int s = it % kWrStages;
@@ -545,73 +321,64 @@ __global__ void __launch_bounds__(256, 1) wgrad_rows_kernel(const __grid_constan
                 tma_load_4d(a_s + kWrABytes, &p.mapB[G.map], &full_bar[s], cc * 64, q0 + G.dw0, row + G.dh, n_img);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_bf16(128, 64 * G.ntaps, true, true);
-            const uint32_t b_lbo = (uint32_t)(G.ntaps > 1 ? G.step * 128 : 128);
-            const uint64_t da_hi = make_smem_desc_sw128(0, 64 * 128, 1024);
-            const uint64_t db_hi = make_smem_desc_sw128(0, b_lbo, 1024);
-            const uint32_t base_lo = smem_u32(smem) >> 4;
-            int s = 0;
-            uint32_t ph = 0, acc = 0;
-            for (int it = 0; it < total_iters; ++it) {
-                mbar_wait(&full_bar[s], ph);
-                tc_fence_after();
-                const uint32_t a_lo = base_lo + (uint32_t)(s * (kWrStageBytes >> 4));
-                const uint64_t da = da_hi | (uint64_t)a_lo;
-                const uint64_t db = db_hi | (uint64_t)(a_lo + (kWrABytes >> 4));
-                // one MMA consumes 16 pixels = 2048 B = 128 descriptor units
-                umma_bf16(tmem_base, da, db, idesc, acc);
-                umma_bf16(tmem_base, da + 128, db + 128, idesc, 1u);
-                umma_bf16(tmem_base, da + 256, db + 256, idesc, 1u);
-                umma_bf16(tmem_base, da + 384, db + 384, idesc, 1u);
-                acc = 1u;
-                umma_commit(&empty_bar[s]);
-                if (++s == kWrStages) { s = 0; ph ^= 1u; }
-            }
-            if (total_iters > 0) umma_commit(tmem_full);
-        }
-    } else if (warp >= 4 && total_iters > 0) {
-        const int ew = warp - 4;
-        const int co = co0 + ew * 32 + lane;
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16);
-        for (int t = 0; t < G.ntaps; ++t) {
-            float* dst = p.dw + (long long)co * p.dw_row_stride + (long long)G.tap_idx[t] * p.C + cc * 64;
-#pragma unroll 1
-            for (int half = 0; half < 2; ++half) {
-                uint32_t r[32];
-                tmem_ld_32x32b_x32(taddr + t * 64 + half * 32, r);
-                tmem_ld_wait();
-                if (co < p.K) {
+    } else {   // every split stores its (possibly all-zero) tile: the slices are summed in split order afterwards
+        const int c = warp >> 2, wq = warp & 3;
+        const uint64_t desc_hi = desc_hi_sw128(64 * 128, 1024);   // MN-major: 8-pixel groups 1024 B apart
+        const uint32_t base_lo = smem_u32(smem) >> 4;
+        float acc[3][32];
 #pragma unroll
-                    for (int q = 0; q < 8; ++q)
-                        red_add_v4(dst + half * 32 + q * 4, __uint_as_float(r[q * 4]), __uint_as_float(r[q * 4 + 1]),
-                                   __uint_as_float(r[q * 4 + 2]), __uint_as_float(r[q * 4 + 3]));
+        for (int t = 0; t < 3; ++t)
+#pragma unroll
+            for (int q = 0; q < 32; ++q) acc[t][q] = 0.f;
+        int s = 0;
+        uint32_t ph = 0;
+        for (int it = 0; it < total_iters; ++it) {
+            mbar_wait(&full_bar[s], ph);
+#pragma unroll
+            for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
+            wgmma_fence();
+            const uint32_t a_lo = base_lo + (uint32_t)(s * (kWrStageBytes >> 4)) + (uint32_t)c * 512u;
+            const uint32_t b_lo = base_lo + (uint32_t)(s * (kWrStageBytes >> 4)) + (kWrABytes >> 4);
+#pragma unroll
+            for (int t = 0; t < 3; ++t) {
+                if (t < G.ntaps) {
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)   // one MMA consumes 16 pixels = 2048 B = 128 descriptor units
+                        wgmma_m64n64<1, 1>(acc[t], desc_at(desc_hi, a_lo + 128 * k, 0),
+                                           desc_at(desc_hi, b_lo + (uint32_t)(t * G.step * 8) + 128 * k, p.use_base_offset), 1u);
                 }
             }
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
+            // wait_group covers only this warp's MMAs: every consumer warp releases the stage
+            if (lane == 0) mbar_arrive(&empty_bar[s]);
+            if (++s == kWrStages) { s = 0; ph ^= 1u; }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc<256>(tmem_base);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int co = co0 + c * 64 + wq * 16 + (lane >> 2) + 8 * h;
+            if (co >= p.K) continue;
+#pragma unroll
+            for (int t = 0; t < 3; ++t) {
+                if (t >= G.ntaps) continue;
+                float* dst = p.dw + blockIdx.x * p.part_stride + (long long)co * p.dw_row_stride + (long long)G.tap_idx[t] * p.C + cc * 64 +
+                             2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) put_f2(dst + 8 * j, acc[t][4 * j + 2 * h], acc[t][4 * j + 2 * h + 1], p.add);
+            }
+        }
     }
 }
 
-int g_use_base_offset = 0;  // measured on B200: the swizzle XOR is taken from the absolute smem address bits, so row-shifted starts need NO base_offset
 int g_allow_rows = 1;
 int g_allow_resident = 1;
-int g_wgrad_waves = 2;
-int g_allow_wide_io = 1;  // tsb_debug_set key 9: 256-bit epilogue loads / stores
-int g_allow_pair = 1;   // tsb_debug_set key 7: weight-sharing tile pairs in the streamed BN = 128 conv kernel
 
-template <int BN, bool RES, bool PAIR = false>
+template <int BN, bool RES>
 int launch_v2(const V2Params& prm, int grid_x, int n_tiles, size_t smem, cudaStream_t st) {
-    { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(igemm_v2_kernel<BN, RES, PAIR>), smem); if (rc_) return rc_; }
-    igemm_v2_kernel<BN, RES, PAIR><<<dim3(grid_x, n_tiles), kThreads, smem, st>>>(prm);
+    { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(igemm_v2_kernel<BN, RES>), smem); if (rc_) return rc_; }
+    igemm_v2_kernel<BN, RES><<<dim3(grid_x, n_tiles), kThreads, smem, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("igemm_v2");
     return TSB_OK;
 }
@@ -621,15 +388,12 @@ int launch_v2(const V2Params& prm, int grid_x, int n_tiles, size_t smem, cudaStr
 extern int g_tsb_ohem_hoist;
 extern int g_tsb_ohem_exact;
 extern "C" int tsb_debug_set(int key, int value) {
-    if (key == 1) g_use_base_offset = value;
+    if (key == 1) convv2::g_use_base_offset = value;
     else if (key == 2) g_allow_rows = value;
     else if (key == 3) g_allow_resident = value;
-    else if (key == 4) convv2::g_enabled = value;
-    else if (key == 5) { g_wgrad_waves = value; convv2::g_wgrad_waves_x = value; }
+    else if (key == 5) convv2::g_wgrad_waves = value;
     else if (key == 6) g_tsb_ohem_hoist = value;
-    else if (key == 7) g_allow_pair = value;
     else if (key == 8) convv2::g_allow_taps = value;
-    else if (key == 9) g_allow_wide_io = value;
     else if (key == 10) g_tsb_ohem_exact = value;
     else return TSB_ERR_ARG;
     return TSB_OK;
@@ -637,8 +401,8 @@ extern "C" int tsb_debug_set(int key, int value) {
 
 namespace convv2 {
 
-int g_enabled = 1;
-int g_wgrad_waves_x = 2;
+int g_wgrad_waves = 2;
+int g_use_base_offset = 0;  // H100 takes the 128B-swizzle phase from the absolute shared address: row-shifted starts need no base_offset
 
 int launch(const Desc& d, cudaStream_t st) {
     V2Params prm;
@@ -723,26 +487,16 @@ int launch(const Desc& d, cudaStream_t st) {
     prm.bias = d.bias; prm.sum = d.sum; prm.sumsq = d.sumsq; prm.out = d.out;
     prm.relu = d.relu; prm.res = d.res;
     prm.use_base_offset = g_use_base_offset;
-    {
-        const long long es = d.out_f32 ? 4 : 2;
-        const bool al = (reinterpret_cast<uintptr_t>(d.out) % 32 == 0) && (d.out_base * es) % 32 == 0 && (d.out_n_stride * es) % 32 == 0 &&
-                        (d.out_p_stride * es) % 32 == 0 && (d.out_q_stride * es) % 32 == 0;
-        prm.wide_io = (g_allow_wide_io && al) ? 1 : 0;
-    }
     // ---- shared-memory plan
     const int kBTile = BN * 128;
     const long long res_need = (long long)d.ntaps * d.kchunks * kBTile;
     const bool resident = g_allow_resident && res_need <= 112 * 1024 && prm.m_tiles > 0;
-    const int tail = 256 + 2 * BN * 4 + 8 * 32 * 17 * 4;
+    const int tail = 256 + kConsumers * 4 * 2 * BN * 4;
     const int budget = 227 * 1024 - 1024 /*align*/ - tail;
     int max_group_taps = 1;
     for (int g = 0; g < ng; ++g) if (prm.groups[g].ntaps > max_group_taps) max_group_taps = prm.groups[g].ntaps;
     prm.res_bytes = resident ? (int)res_need : 0;
-    int grid_pre = tsb_num_sms() / n_tiles;
-    if (grid_pre < 1) grid_pre = 1;
-    // pair mode: streamed weights, BN = 128, at least two tiles per CTA (otherwise the second accumulator idles)
-    const bool pair = g_allow_pair && !resident && BN == 128 && prm.m_tiles >= 2 * grid_pre;
-    prm.stage_bytes = (pair ? 2 : 1) * kAStageBytes + (resident ? 0 : max_group_taps * kBTile);
+    prm.stage_bytes = kAStageBytes + (resident ? 0 : max_group_taps * kBTile);
     int ns = (budget - prm.res_bytes) / prm.stage_bytes;
     if (ns > kMaxStages) ns = kMaxStages;
     TSB_REQUIRE(ns >= 2, "conv_v2: shared-memory plan needs at least 2 stages");
@@ -752,9 +506,18 @@ int launch(const Desc& d, cudaStream_t st) {
     if (grid_x < 1) grid_x = 1;
     if (grid_x > prm.m_tiles) grid_x = prm.m_tiles;
     if (grid_x < 1) grid_x = 1;
-    if (BN == 64) return resident ? launch_v2<64, true>(prm, grid_x, n_tiles, smem, st) : launch_v2<64, false>(prm, grid_x, n_tiles, smem, st);
-    if (pair) return launch_v2<128, false, true>(prm, grid_x, n_tiles, smem, st);
-    return resident ? launch_v2<128, true>(prm, grid_x, n_tiles, smem, st) : launch_v2<128, false>(prm, grid_x, n_tiles, smem, st);
+    if (d.sum != nullptr) {
+        TSB_REQUIRE(d.ws && (long long)grid_x * 2 * d.k_real <= d.ws_floats, "conv: statistics workspace needs %lld floats",
+                    (long long)grid_x * 2 * d.k_real);
+        prm.part = d.ws;
+    }
+    int rc2 = (BN == 64) ? (resident ? launch_v2<64, true>(prm, grid_x, n_tiles, smem, st) : launch_v2<64, false>(prm, grid_x, n_tiles, smem, st))
+                         : (resident ? launch_v2<128, true>(prm, grid_x, n_tiles, smem, st) : launch_v2<128, false>(prm, grid_x, n_tiles, smem, st));
+    if (rc2 || d.sum == nullptr) return rc2;
+    rc2 = tsb_det_reduce(d.sum, prm.part, grid_x, d.k_real, 2LL * d.k_real, st);
+    if (rc2) return rc2;
+    // the sumsq slots follow the sum slots of the same CTA: a stride of 2·k_real between CTAs
+    return tsb_det_reduce(d.sumsq, prm.part + d.k_real, grid_x, d.k_real, 2LL * d.k_real, st);
 }
 
 
@@ -819,19 +582,25 @@ int launch_wgrad_rows(const WgradDesc& d, cudaStream_t st) {
     prm.tiles_h = d.P;
     prm.total_tiles = prm.tiles_w * prm.tiles_h * d.N;
     prm.K = d.K; prm.C = d.C; prm.dw_row_stride = d.dw_row_stride; prm.dw = d.dw;
+    prm.use_base_offset = g_use_base_offset;
     const int co_tiles = (d.K + 127) / 128;
     const int zdim = ng * prm.cchunks;
     int base = zdim * co_tiles;
     int want = (g_wgrad_waves * tsb_num_sms() + base - 1) / base;
     int max_splits = (prm.total_tiles + 15) / 16;
     if (want > max_splits) want = max_splits;
+    const long long n_dw = (long long)d.K * d.dw_row_stride;
+    if (want > (d.ws ? d.ws_floats / n_dw : 0)) want = (int)(d.ws ? d.ws_floats / n_dw : 0);
     if (want < 1) want = 1;
     prm.tiles_per_split = (prm.total_tiles + want - 1) / want;
     int splits = (prm.total_tiles + prm.tiles_per_split - 1) / prm.tiles_per_split;
+    prm.add = splits == 1;
+    prm.dw = prm.add ? d.dw : d.ws;
+    prm.part_stride = prm.add ? 0 : n_dw;
     { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(wgrad_rows_kernel), kWrSmem); if (rc_) return rc_; }
-    wgrad_rows_kernel<<<dim3(splits, co_tiles, zdim), 256, kWrSmem, st>>>(prm);
+    wgrad_rows_kernel<<<dim3(splits, co_tiles, zdim), kThreads, kWrSmem, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("wgrad_rows");
-    return TSB_OK;
+    return prm.add ? TSB_OK : tsb_det_reduce(d.dw, prm.dw, splits, n_dw, n_dw, st);
 }
 
 }  // namespace convv2

@@ -31,6 +31,8 @@ struct Desc {
     void* out;
     int relu;          // inference epilogue (folded BN): ReLU after bias (+ res)
     const void* res;   // bf16 residual addressed exactly like `out`
+    float* ws;         // caller's workspace for the per-CTA statistics (needed when sum != nullptr)
+    long long ws_floats;
 };
 
 struct WgradDesc {
@@ -41,10 +43,12 @@ struct WgradDesc {
     int ntaps;
     long long dw_row_stride;
     float* dw;
+    float* ws;         // caller's workspace: one dW-shaped slice per pixel split (one split, adding in place, when it is too small)
+    long long ws_floats;
 };
 
-extern int g_enabled;
-extern int g_wgrad_waves_x;
+extern int g_wgrad_waves;
+extern int g_use_base_offset;   // tsb_debug_set key 1
 extern int g_allow_taps;
 int launch(const Desc& d, cudaStream_t st);
 int launch_wgrad_rows(const WgradDesc& d, cudaStream_t st);

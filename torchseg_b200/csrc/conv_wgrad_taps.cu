@@ -2,33 +2,29 @@
 //
 //   dW[co, (r,s), ci] = Σ_px dY[px, co] · X[px + ((r-1)·dil, (s-1)·dil), ci]
 //
-// GEMM roles (swapped with respect to wgrad_rows_kernel): the M side carries (tap, ci), the N side carries co:
-//   A = X   : MN-major straight out of NHWC shared-memory rows (64 input channels = 128 B per pixel); ONE UMMA
-//             descriptor covers TWO taps — its two 64-row M-groups are the same pixel rows shifted by the tap distance
-//             (leading-dimension byte offset = dil·128 B for two taps of a filter row, = the row-slot pitch for the
-//             third taps of two filter rows);
-//   B = dY  : MN-major, N = 64 output channels, K = 64 pixels per stage;
-//   D_j[128 lanes = (tap pair j, ci), 64 columns = co], j = 0..4 → 320 TMEM columns.
-// Tap pairs: j=0..2: (r=j; s=0,1), j=3: (r=0,s=2 | r=1,s=2), j=4: (r=2,s=2 | junk: never stored).
+// GEMM roles (swapped with respect to wgrad_rows_kernel): the M side carries ci, the N side carries co, one accumulator
+// per tap. Consumer warpgroup r owns filter row r:
+//   A = X   : MN-major straight out of NHWC shared-memory rows (64 input channels = 128 B per pixel); tap (r, s) reads
+//             row-slot r shifted by s·dil pixel rows, so each filter row's activations are staged once for its 3 taps;
+//   B = dY  : MN-major, N = 64 output channels, K = 64 pixels per stage, staged once for all nine taps;
+//   D_(r,s)[64 ci, 64 co] in registers, 3 x 32 fp32 per thread.
 //
-// Why: the row kernel maps co to M. M = 64 costs a tcgen05.mma as many cycles as M = 128, so the K = 64 layers (layer1, the
-// stems' neighbours — the biggest wgrads of the step) ran half-empty MMAs; it also runs one CTA per filter row, reading dY
-// (and X) three times. Here every MMA is a full 128 x 64 x 16 (4.5 useful of 5 per K-step), dY is staged once for all nine
-// taps and X once per filter row.
+// Why: the row kernel maps co to M and runs one CTA per filter row, reading dY (and X) three times; here dY is staged
+// once for all nine taps and X once per filter row.
 //
 // Per stage (64 pixels = TH rows of TW): dY box {64 co, TW, TH} (8 KB) + three X boxes {64 ci, TW + 2·dil, TH} (one per
-// filter row, at rows p0 + (r-1)·dil; the zero-filled out-of-bounds halo IS the padding). 4 K-steps x 5 MMAs (N = 64: 32
-// tensor-pipe cycles each) = 640 cycles per stage against ~780 cycles of L2→SM ingest for the 33 KB at ~43 B/clk/SM.
+// filter row, at rows p0 + (r-1)·dil; the zero-filled out-of-bounds halo IS the padding).
 #include "conv_common.cuh"
 #include "conv_v2.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
-using namespace sm100;
+using namespace sm90;
 using namespace convhost;
 
 namespace {
 
-constexpr int kTpThreads = 256;   // warp 0: TMA, warp 1: MMA, warp 2: TMEM alloc, warps 4-7: epilogue
+constexpr int kTpConsumers = 3;                       // warpgroups, one per filter row
+constexpr int kTpThreads = kTpConsumers * 128 + 32;   // + one TMA producer warp
 constexpr int kTpMaxStages = 6;
 constexpr int kTpDyBytes = 64 * 128;
 
@@ -43,38 +39,34 @@ struct alignas(64) TpParams {
     int kdy[4];          // ... and inside the dY tile (always k·2048)
     int K, C;
     long long dw_row_stride;   // R·S·C
-    float* dw;
+    float* dw;                 // dW-shaped slice per split (workspace), part_stride apart; or dW itself when `add`
+    long long part_stride;
+    int add;                   // one split: add in place
+    int use_base_offset;
 };
 
 __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_constant__ TpParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* tail = smem + p.nstages * p.stage_bytes + 1024;   // 1 KB slack: the junk half of D_4 reads past the last slot
+    uint8_t* tail = smem + p.nstages * p.stage_bytes;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
     uint64_t* empty_bar = full_bar + kTpMaxStages;
-    uint64_t* tmem_full = empty_bar + kTpMaxStages;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int co0 = blockIdx.y * 64, ci0 = blockIdx.z * 64;
     const int t_begin = blockIdx.x * p.tiles_per_split;
     const int t_end = min(p.total_tiles, t_begin + p.tiles_per_split);
     const int iters = t_end - t_begin;
+    constexpr int kProducer = kTpConsumers * 4;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducer && lane == 0) {
         tma_prefetch_desc(&p.mapDy);
         tma_prefetch_desc(&p.mapX);
-        for (int s = 0; s < p.nstages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full, 1);
+        for (int s = 0; s < p.nstages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kTpConsumers * 4); }
         fence_barrier_init();
-    } else if (warp == 2) {
-        tmem_alloc<512>(tmem_ptr);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
+    if (warp == kProducer) {
         if (lane == 0) {
             int s = 0;
             uint32_t ph = 0;
@@ -95,86 +87,61 @@ __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_
                 if (++s == p.nstages) { s = 0; ph ^= 1u; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && iters > 0) {
-            constexpr uint32_t idesc = make_idesc_bf16(128, 64, true, true);
-            const uint32_t tapb = (uint32_t)p.dil * 128u;            // bytes between horizontally adjacent taps
-            // descriptor high parts (start address 0): SBO = 1024 B between 8-pixel groups; LBO = M-group distance
-            const uint64_t hi_row = make_smem_desc_sw128(0, tapb, 1024);                  // taps (r,0),(r,1)
-            const uint64_t hi_col = make_smem_desc_sw128(0, (uint32_t)p.slot_bytes, 1024);  // taps (0,2),(1,2)
-            const uint64_t hi_dy = make_smem_desc_sw128(0, 64 * 128, 1024);               // single N-group
-            const uint32_t base_lo = smem_u32(smem) >> 4;
-            const uint32_t slot16 = (uint32_t)p.slot_bytes >> 4;
-            const uint32_t tap2 = (2u * tapb) >> 4;
-            uint32_t ka[4], kb[4];
+    } else {   // every split stores its (possibly all-zero) tile: the slices are summed in split order afterwards
+        const int r = warp >> 2, wq = warp & 3;
+        const uint64_t desc_hi = desc_hi_sw128(64 * 128, 1024);   // MN-major, one 64-element atom; 8-pixel groups 1 KB apart
+        const uint32_t base_lo = smem_u32(smem) >> 4;
+        const uint32_t tap16 = (uint32_t)p.dil * 8u;             // 16-byte units between horizontally adjacent taps
+        uint32_t ka[4], kb[4];
 #pragma unroll
-            for (int k = 0; k < 4; ++k) { ka[k] = (uint32_t)p.koff[k] >> 4; kb[k] = (uint32_t)p.kdy[k] >> 4; }
-            int s = 0;
-            uint32_t ph = 0, acc = 0;
-            for (int it = 0; it < iters; ++it) {
-                mbar_wait(&full_bar[s], ph);
-                tc_fence_after();
-                const uint32_t st_lo = base_lo + (uint32_t)(s * (p.stage_bytes >> 4));
-                const uint32_t x_lo = st_lo + (kTpDyBytes >> 4);
-                const uint64_t db0 = hi_dy | (uint64_t)st_lo;
-                const uint64_t a0 = hi_row | (uint64_t)x_lo;
-                const uint64_t a1 = hi_row | (uint64_t)(x_lo + slot16);
-                const uint64_t a2 = hi_row | (uint64_t)(x_lo + 2 * slot16);
-                const uint64_t a3 = hi_col | (uint64_t)(x_lo + tap2);
-                const uint64_t a4 = hi_row | (uint64_t)(x_lo + 2 * slot16 + tap2);
+        for (int k = 0; k < 4; ++k) { ka[k] = (uint32_t)p.koff[k] >> 4; kb[k] = (uint32_t)p.kdy[k] >> 4; }
+        float acc[3][32];
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint64_t db = db0 + kb[k];
-                    umma_bf16(tmem_base + 0, a0 + ka[k], db, idesc, acc);
-                    umma_bf16(tmem_base + 64, a1 + ka[k], db, idesc, acc);
-                    umma_bf16(tmem_base + 128, a2 + ka[k], db, idesc, acc);
-                    umma_bf16(tmem_base + 192, a3 + ka[k], db, idesc, acc);
-                    umma_bf16(tmem_base + 256, a4 + ka[k], db, idesc, acc);
-                    acc = 1u;
-                }
-                umma_commit(&empty_bar[s]);
-                if (++s == p.nstages) { s = 0; ph ^= 1u; }
+        for (int t = 0; t < 3; ++t)
+#pragma unroll
+            for (int q = 0; q < 32; ++q) acc[t][q] = 0.f;
+        int s = 0;
+        uint32_t ph = 0;
+        for (int it = 0; it < iters; ++it) {
+            mbar_wait(&full_bar[s], ph);
+#pragma unroll
+            for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
+            wgmma_fence();
+            const uint32_t st_lo = base_lo + (uint32_t)(s * (p.stage_bytes >> 4));
+            const uint32_t x_lo = st_lo + (kTpDyBytes >> 4) + (uint32_t)r * ((uint32_t)p.slot_bytes >> 4);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint64_t db = desc_at(desc_hi, st_lo + kb[k], 0);
+#pragma unroll
+                for (int t = 0; t < 3; ++t)
+                    wgmma_m64n64<1, 1>(acc[t], desc_at(desc_hi, x_lo + t * tap16 + ka[k], p.use_base_offset), db, 1u);
             }
-            umma_commit(tmem_full);
-        }
-    } else if (warp >= 4 && iters > 0) {
-        // lanes 0-63 ↔ first tap of the pair, 64-127 ↔ second; column c ↔ output channel co0 + c.
-        // dW is [K][3][3][C] fp32: a warp's 32 lanes add to 32 consecutive input channels (one 128-byte line) per column.
-        const int ew = warp - 4;                 // TMEM lane quarter (== warp % 4)
-        const int half = ew >> 1;
-        const int ci = ci0 + (ew & 1) * 32 + lane;
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16);
-        const bool ci_ok = ci < p.C;
-#pragma unroll 1
-        for (int j = 0; j < 5; ++j) {
-            int tap;
-            if (j < 3) tap = j * 3 + half;
-            else if (j == 3) tap = half * 3 + 2;
-            else tap = half ? -1 : 8;
-            if (tap < 0) continue;               // junk half of D_4 (warp-uniform)
-            float* dst = p.dw + (long long)tap * p.C + ci;
-#pragma unroll 1
-            for (int hc = 0; hc < 2; ++hc) {
-                uint32_t r[32];
-                tmem_ld_32x32b_x32(taddr + j * 64 + hc * 32, r);
-                tmem_ld_wait();
-                if (ci_ok) {
+            wgmma_commit();
+            wgmma_wait<0>();
 #pragma unroll
-                    for (int c = 0; c < 32; ++c) {
-                        const int co = co0 + hc * 32 + c;
-                        if (co < p.K) atomicAdd(dst + (long long)co * p.dw_row_stride, __uint_as_float(r[c]));
+            for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
+            // wait_group covers only this warp's MMAs: every consumer warp releases the stage
+            if (lane == 0) mbar_arrive(&empty_bar[s]);
+            if (++s == p.nstages) { s = 0; ph ^= 1u; }
+        }
+        // fragment: rows = input channels ci0 + 16·wq + lane/4 (+8), columns = output channels co0 + 8j + 2(lane%4) (+1)
+        // dW is [K][3][3][C] fp32
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int ci = ci0 + wq * 16 + (lane >> 2) + 8 * h;
+            if (ci >= p.C) continue;
+#pragma unroll
+            for (int t = 0; t < 3; ++t) {
+                float* dst = p.dw + blockIdx.x * p.part_stride + (long long)(r * 3 + t) * p.C + ci;
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int co = co0 + 8 * j + 2 * (lane & 3) + e;
+                        if (co < p.K) put_f1(dst + (long long)co * p.dw_row_stride, acc[t][4 * j + 2 * h + e], p.add);
                     }
-                }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc<512>(tmem_base);
     }
 }
 
@@ -203,7 +170,7 @@ int launch_wgrad_taps(const WgradDesc& d, int R, int pad, int dil, cudaStream_t 
     }
     if (TW < 16) return TSB_ERR_UNSUPPORTED;       // a 16-pixel K-step must stay inside one tile row
     prm.stage_bytes = (kTpDyBytes + 3 * prm.slot_bytes + 1023) / 1024 * 1024;
-    int ns = (227 * 1024 - 1024 /*align*/ - 1024 /*slack*/ - 256 /*barriers*/) / prm.stage_bytes;
+    int ns = (227 * 1024 - 1024 /*align*/ - 256 /*barriers*/) / prm.stage_bytes;
     if (ns > kTpMaxStages) ns = kTpMaxStages;
     if (ns < 2) return TSB_ERR_UNSUPPORTED;
     prm.nstages = ns;
@@ -217,11 +184,12 @@ int launch_wgrad_taps(const WgradDesc& d, int R, int pad, int dil, cudaStream_t 
     prm.tiles_h = (d.P + TH - 1) / TH;
     prm.total_tiles = prm.tiles_w * prm.tiles_h * d.N;
     prm.K = d.K; prm.C = d.C; prm.dw_row_stride = d.dw_row_stride; prm.dw = d.dw;
+    prm.use_base_offset = g_use_base_offset;
     const int co_tiles = (d.K + 63) / 64, ci_tiles = d.C / 64;
     const int base = co_tiles * ci_tiles;
-    // one CTA per SM (persistent over a contiguous pixel range); at least 8 tiles per CTA so the 320-column drain
-    // (288 fp32 reductions per thread) stays small next to the main loop
-    // ... and the split count that minimises waves x tiles-per-CTA (wave quantisation: 192 CTAs cost two full waves)
+    // one CTA per SM (persistent over a contiguous pixel range); at least 8 tiles per CTA so the drain of the nine
+    // accumulators (96 fp32 reductions per thread) stays small next to the main loop, and the split count that
+    // minimises waves x tiles-per-CTA (wave quantisation)
     const int sms = tsb_num_sms();
     int max_splits = (prm.total_tiles + 7) / 8;
     if (max_splits < 1) max_splits = 1;
@@ -231,17 +199,23 @@ int launch_wgrad_taps(const WgradDesc& d, int R, int pad, int dil, cudaStream_t 
     for (int sp = 1; sp <= max_splits; ++sp) {
         const long long per = (prm.total_tiles + sp - 1) / sp;
         const long long waves = ((long long)base * sp + sms - 1) / sms;
-        const long long cost = waves * (per + 6);     // + ~6 stage-times of prologue / 320-column drain per CTA
+        const long long cost = waves * (per + 6);     // + ~6 stage-times of prologue / accumulator drain per CTA
         if (best < 0 || cost < best) { best = cost; want = sp; }
     }
+    const long long n_dw = (long long)d.K * d.dw_row_stride;
+    if (want > (d.ws ? d.ws_floats / n_dw : 0)) want = (int)(d.ws ? d.ws_floats / n_dw : 0);
+    if (want < 1) want = 1;
     prm.tiles_per_split = (prm.total_tiles + want - 1) / want;
     const int splits = (prm.total_tiles + prm.tiles_per_split - 1) / prm.tiles_per_split;
-    const size_t smem = 1024 + (size_t)ns * prm.stage_bytes + 1024 + 256;
+    prm.add = splits == 1;
+    prm.dw = prm.add ? d.dw : d.ws;
+    prm.part_stride = prm.add ? 0 : n_dw;
+    const size_t smem = 1024 + (size_t)ns * prm.stage_bytes + 256;
     rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(wgrad_taps_kernel), smem);
     if (rc) return rc;
     wgrad_taps_kernel<<<dim3(splits, co_tiles, ci_tiles), kTpThreads, smem, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("wgrad_taps");
-    return TSB_OK;
+    return prm.add ? TSB_OK : tsb_det_reduce(d.dw, prm.dw, splits, n_dw, n_dw, st);
 }
 
 }  // namespace convv2

@@ -1,8 +1,8 @@
 // Training-time input pipeline on the device (SURVEY §8 f4): random mirror → random scale (cv2.resize INTER_LINEAR for the
 // image, INTER_NEAREST for the label) → normalize → random crop + centred constant pad → HWC→CHW, fused into ONE pass
 // from the decoded uint8 image to the fp32 NCHW batch and the int64 label batch the train loop consumes.
-// Replaces TrainPre.__call__ (/root/reference/model/bisenet/cityscapes.bisenet.R18/dataloader.py:16-33) and the
-// img_utils functions it calls (/root/reference/furnace/utils/img_utils.py:24-78,118-125,140-145,181-187); the random draws
+// Replaces TrainPre.__call__ (TorchSeg model/bisenet/cityscapes.bisenet.R18/dataloader.py:16-33) and the
+// img_utils functions it calls (TorchSeg furnace/utils/img_utils.py:24-78,118-125,140-145,181-187); the random draws
 // stay on the host (torchseg_b200/utils/gpu_pipeline.py) in the reference's order.
 //
 // Bit-exact by construction: OpenCV's 8-bit INTER_LINEAR is FIXED POINT (11-bit coefficients, int32 horizontal pass,
@@ -95,7 +95,7 @@ train_preprocess_kernel(const PreSample* __restrict__ samples, int crop_h, int c
 
 
 // ------------------------------------------------------------------------------------------------
-// DFN border labels (/root/reference/model/dfn/cityscapes.dfn.R101_v1c/dataloader.py:15-29): Canny(apertureSize 7, thresholds
+// DFN border labels (TorchSeg model/dfn/cityscapes.dfn.R101_v1c/dataloader.py:15-29): Canny(apertureSize 7, thresholds
 // 5 → 0 after OpenCV's /16) of the scaled label map with 255 → 0, dilated by a 7x7 rectangle, 255 → 1, cropped / padded like
 // the label. All integer arithmetic (imgproc/src/canny.cpp restated): Sobel-7 sums are exact ints, /16 with round-half-even,
 // L1 magnitude with a ZERO border, fixed-point tangent test for the non-maximum suppression; low == high, so hysteresis adds

@@ -1,5 +1,5 @@
-// OHEM cross-entropy for sm_100a — replaces ProbOhemCrossEntropy2d.forward
-// (/root/reference/furnace/seg_opr/loss_opr.py:68-98).  HBM-bound byte work: coalesced loads,
+// OHEM cross-entropy for sm_90a — replaces ProbOhemCrossEntropy2d.forward
+// (TorchSeg furnace/seg_opr/loss_opr.py:68-98).  HBM-bound byte work: coalesced loads,
 // warp-shuffle / shared-memory histogram reductions, an exact radix *select* instead of the full sort.
 #include "tsb_common.cuh"
 #include "band.cuh"
@@ -565,8 +565,9 @@ ohem_grad_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const in
 //     thread in its own column (no synchronisation): a row costs 2 LDS + 3 flops per class instead of 4 LDS + 9;
 //   * the target class is fetched by ONE dynamic shared-memory read pair (its exp is recomputed: bit-identical, same
 //     inputs) instead of CX compare-selects;
-//   * gradient: the one-hot term goes straight to a low-resolution shared-memory accumulator (4 RED.shared per pixel) instead
-//     of CX compare-selects; the accumulators' hand-over to phase 2 re-uses the T arrays in place (thread-private
+//   * gradient: softmax minus one-hot accumulates in the thread's own registers, and the bands run in four (row parity,
+//     strip parity) launches that add to the low-res gradient without atomics: the gradient is the same on every run;
+//     the accumulators' hand-over to phase 2 re-uses the T arrays in place (thread-private
 //     columns), which leaves ~80 registers and 3 CTAs / SM.
 // Arithmetic (operation order, roundings) is unchanged: p, T and the kept set stay bit-exact against the oracle.
 // =============================================================================================
@@ -637,20 +638,23 @@ __global__ void __launch_bounds__(kThreads, 3)
 ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64_t* __restrict__ labels,
                       const float* __restrict__ p, int N, int H, int W, int ignore_label, const float* __restrict__ cw,
                       const uint32_t* __restrict__ state, const float* __restrict__ gscale, float* __restrict__ dlo,
-                      int maxcols) {
-    extern __shared__ float s_dyn_x[];   // sT0 / s_g0 [CX][kPitchX] | sT1 / s_g1 | s_lo0 | s_lo1 | s_oh[2][maxcols][CX]
+                      int maxcols, int phase) {
+    extern __shared__ float s_dyn_x[];   // sT0 / s_g0 [CX][kPitchX] | sT1 / s_g1 | s_lo0 | s_lo1
     float* sT0 = s_dyn_x;
     float* sT1 = s_dyn_x + CX * kPitchX;
     float* s_lo0 = s_dyn_x + 2 * CX * kPitchX;
     float* s_lo1 = s_lo0 + maxcols * CX;
-    float* s_oh = s_lo1 + maxcols * CX;  // one-hot part of the gradient, already at low resolution: [row][col][c]
     __shared__ float s_l0[kStrip], s_l1[kStrip];
     __shared__ short s_seg[kStrip + 8];
     const bool active = state[ST_ACTIVE] != 0;
     const float Tth = __uint_as_float(state[ST_THRESH]);
     const float scale = __uint_as_float(state[ST_INVDEN]) * (gscale ? *gscale : 1.f);
     const float ry = area_scale(h, H), rx = area_scale(w, W);
-    const int n = blockIdx.z, ci = blockIdx.y, x0 = blockIdx.x * kStrip, x1 = min(W, x0 + kStrip);
+    // launch `phase` (0..3) runs the bands of one (row parity, strip parity): bands of one launch never add to the same
+    // low-res cell, and the four launches run in a fixed order, so every cell is summed in the same order on every run
+    const int n = blockIdx.z, ci = 2 * blockIdx.y + (phase & 1), x0 = (2 * blockIdx.x + (phase >> 1)) * kStrip;
+    if (ci >= h || x0 >= W) return;
+    const int x1 = min(W, x0 + kStrip);
     const int nx = x1 - x0;
     const int i1 = ci + (ci < h - 1 ? 1 : 0);
     const BandGeom g = band_geom(ry, rx, ci, x0, x1, H, w);
@@ -658,7 +662,6 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
     for (int q = threadIdx.x; q < 2 * g.ncols * CX; q += kThreads) {
         const int c = q % CX, t2 = q / CX, col = t2 % g.ncols, row = t2 / g.ncols;
         (row ? s_lo1 : s_lo0)[col * CX + c] = __ldg(lo + (((long long)n * h + (row ? i1 : ci)) * w + g.jbase + col) * cs + c);
-        s_oh[q] = 0.f;
     }
     const int tid = threadIdx.x;
     const int x = x0 + tid;
@@ -682,10 +685,6 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
     float G0[CX], G1[CX];
 #pragma unroll
     for (int c = 0; c < CX; ++c) { G0[c] = 0.f; G1[c] = 0.f; }
-    float* oh00 = s_oh + j0 * CX;                       // (row i, col j0), (i, j1), (i1, j0), (i1, j1)
-    float* oh01 = s_oh + j1 * CX;
-    float* oh10 = s_oh + (g.ncols + j0) * CX;
-    float* oh11 = s_oh + (g.ncols + j1) * CX;
     long long lab_next = 0;
     float p_next = 0.f;
     if (xin) {
@@ -719,15 +718,12 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
         const float inv = wt / ssum;
 #pragma unroll
         for (int c = 0; c < CX; ++c) {
-            const float gg = v[c] * inv;               // softmax part; the one-hot part goes to s_oh below
+            // softmax minus one-hot, in this thread's own accumulators: the column sums of phase 2 add them in a fixed
+            // order (shared-memory atomics would make the gradient's rounding vary from run to run)
+            const float gg = v[c] * inv - (c == t ? wt : 0.f);
             G0[c] = fmaf(ly.l0, gg, G0[c]);
             G1[c] = fmaf(ly.l1, gg, G1[c]);
         }
-        const float a0 = -wt * ly.l0, a1 = -wt * ly.l1;
-        atomicAdd(oh00 + t, a0 * lx.l0);
-        atomicAdd(oh01 + t, a0 * lx.l1);
-        atomicAdd(oh10 + t, a1 * lx.l0);
-        atomicAdd(oh11 + t, a1 * lx.l1);
     }
     // hand-over to phase 2 in place: column `tid` of sT0 / sT1 was only ever read by this thread
 #pragma unroll
@@ -741,7 +737,7 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
         const float* g0 = sT0 + c * kPitchX;
         const float* g1 = sT1 + c * kPitchX;
         const int a0 = s_seg[j], a1 = s_seg[j + 1];
-        float top = s_oh[j * CX + c], bot = s_oh[(g.ncols + j) * CX + c];
+        float top = 0.f, bot = 0.f;
         for (int xx = a0; xx < a1; ++xx) {
             const float wl = s_l0[xx];
             top = fmaf(wl, g0[xx], top);
@@ -762,8 +758,8 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
                 bot = fmaf(wr, g1[xx], bot);
             }
         }
-        if (top != 0.f) atomicAdd(dlo + (((long long)n * h + ci) * w + g.jbase + j) * cs + c, top);
-        if (bot != 0.f) atomicAdd(dlo + (((long long)n * h + i1) * w + g.jbase + j) * cs + c, bot);
+        if (top != 0.f) dlo[(((long long)n * h + ci) * w + g.jbase + j) * cs + c] += top;
+        if (bot != 0.f) dlo[(((long long)n * h + i1) * w + g.jbase + j) * cs + c] += bot;
     }
 }
 
@@ -907,18 +903,20 @@ extern "C" int tsb_ohem_grad_up(const float* logits_lo, int cs, int h, int w, co
     const int maxcols = band_maxcols(w, W);
     TSB_REQUIRE(maxcols <= kStrip, "tsb_ohem_grad_up: up-scale factor W/w too small for the band kernel");
     if (g_tsb_ohem_exact && (C == 19 || C == 21)) {
-        const size_t smx = sizeof(float) * (2 * (size_t)C * kPitchX + 4 * (size_t)maxcols * C);
+        const size_t smx = sizeof(float) * (2 * (size_t)C * kPitchX + 2 * (size_t)maxcols * C);
         if (smx <= 72 * 1024) {
-            dim3 gridx((W + kStrip - 1) / kStrip, h, N);
+            dim3 gridx(((W + kStrip - 1) / kStrip + 1) / 2, (h + 1) / 2, N);
 #define GX(CX)                                                                                                      \
     do {                                                                                                            \
         int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(ohem_grad_up_x_kernel<CX>), smx);               \
         if (rc_) return rc_;                                                                                        \
-        ohem_grad_up_x_kernel<CX><<<gridx, kThreads, smx, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, p, N, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols); \
+        for (int ph = 0; ph < 4; ++ph) {                                                                            \
+            ohem_grad_up_x_kernel<CX><<<gridx, kThreads, smx, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, p, N, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols, ph); \
+            TSB_CUDA_CHECK_LAUNCH("ohem_grad_up_x");                                                               \
+        }                                                                                                           \
     } while (0)
             if (C == 19) GX(19); else GX(21);
 #undef GX
-            TSB_CUDA_CHECK_LAUNCH("ohem_grad_up_x");
             return TSB_OK;
         }
     }

@@ -1,5 +1,5 @@
 // Device-initiated all-reduce of SMALL fp32 vectors over NVLink peer memory — the SyncBatchNorm statistics exchange
-// (replaces apex SyncBatchNorm's per-layer all-reduce, /root/reference/model/bisenet/cityscapes.bisenet.R18/train.py:54-55).
+// (replaces apex SyncBatchNorm's per-layer all-reduce, TorchSeg model/bisenet/cityscapes.bisenet.R18/train.py:54-55).
 //
 // A BiSeNet step has ~70 of these exchanges ([Σx | Σx²] forward, [Σdz | Σdz·x̂] backward; 128..8192 floats each): with NCCL
 // every one costs a launch + protocol latency of 25-40 us on the compute stream, i.e. the whole weak-scaling loss of the
@@ -9,9 +9,8 @@
 //
 // Protocol ("LL": the flag travels WITH the data, no memory fences): every fp32 value is stored as an 8-byte pair
 // {value bits, seq}; 8-byte stores are single transactions over NVLink, so a reader that sees seq in a pair has the value.
-// A first version used data stores + __threadfence_system + st.release.sys / ld.acquire.sys flags: measured on 2 x B200 it
-// cost ~77 us per exchange (system-scope fences with peer writes in flight), twice an NCCL all-reduce; the fence-free
-// form needs one NVLink store latency.
+// The alternative (data stores + __threadfence_system + st.release.sys / ld.acquire.sys flags) pays system-scope fences
+// with peer writes in flight on every exchange; the fence-free form needs one NVLink store latency.
 //
 // Symmetric buffer of every rank (allocated and exchanged by the caller, e.g. torch symmetric memory):
 //   [nslots] x { uint2 pair[world][slot_floats] }

@@ -1,5 +1,5 @@
 // Layout/precision packing, elementwise glue, fused flat-buffer SGD and the sigmoid focal loss.
-// All HBM-bound streaming kernels (vectorised where the layout allows), sm_100a.
+// All HBM-bound streaming kernels (vectorised where the layout allows), sm_90a.
 #include "nhwc_vec.cuh"
 
 namespace {
@@ -177,7 +177,8 @@ cast_pad_kernel(const TS* __restrict__ src, int scs, int K, __nv_bfloat16* __res
     }
 }
 
-// db[k] += Σ_pix dy[pix,k]; one warp per pixel stripe, lanes over channels (K <= 64 typical: 19 padded)
+// db[k] += Σ_pix dy[pix,k]; one warp per pixel stripe, lanes over channels (K <= 64 typical: 19 padded). Each CTA
+// writes its partial sums to its own slot of the deterministic workspace (`db` here), summed in CTA order afterwards.
 __global__ void __launch_bounds__(kThreads)
 bias_grad_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, long long npix, int K, float* __restrict__ db) {
     __shared__ float s_acc[kThreads];
@@ -190,7 +191,7 @@ bias_grad_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, long long npix,
                 acc += __bfloat162float(dy[p * dycs + k]);
         s_acc[threadIdx.x] = acc;
         __syncthreads();
-        if (lane == 0 && k < K) atomicAdd(db + k, s_acc[kk] + s_acc[64 + kk] + s_acc[128 + kk] + s_acc[192 + kk]);
+        if (lane == 0 && k < K) db[(long long)blockIdx.x * K + k] = s_acc[kk] + s_acc[64 + kk] + s_acc[128 + kk] + s_acc[192 + kk];
         __syncthreads();
     }
 }
@@ -408,12 +409,14 @@ extern "C" int tsb_relu_bwd(const void* dy, int dycs, const void* y, int ycs, vo
     return TSB_OK;
 }
 
-extern "C" int tsb_bias_grad(const void* dy, int dycs, long long npix, int K, float* db, tsb_stream_t stream) {
+extern "C" int tsb_bias_grad(const void* dy, int dycs, long long npix, int K, float* db, float* ws, long long ws_floats,
+                             tsb_stream_t stream) {
     TSB_REQUIRE(dy && db && npix > 0 && K > 0, "tsb_bias_grad: bad args");
     int grid = tsb_grid_for(npix, 64, 4);
-    bias_grad_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)dy, dycs, npix, K, db);
+    TSB_REQUIRE(ws && (long long)grid * K <= ws_floats, "tsb_bias_grad: workspace needs %lld floats", (long long)grid * K);
+    bias_grad_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)dy, dycs, npix, K, ws);
     TSB_CUDA_CHECK_LAUNCH("bias_grad");
-    return TSB_OK;
+    return tsb_det_reduce(db, ws, grid, K, K, (cudaStream_t)stream);
 }
 
 extern "C" int tsb_sgd_flat(float* param, const float* grad, float* mom_buf, long long n, const long long* seg_end,

@@ -1,4 +1,4 @@
-// Point-wise spatial attention helpers (PSANet, /root/reference/model/psanet/ade.psanet.R101_v1c/network.py:119-138):
+// Point-wise spatial attention helpers (PSANet, TorchSeg model/psanet/ade.psanet.R101_v1c/network.py:119-138):
 //   softmax over the 3600 attention channels of every pixel (torch.softmax(att.view(b,c,-1), dim=1) — in NHWC the
 //   reduction dimension is the contiguous one), its backward, and the 2-D transposes that turn the per-image
 //   `torch.bmm(reduce_x, softmax)` into the 1x1 implicit-GEMM convolution kernels (weights = the image's own

@@ -172,7 +172,7 @@ bilinear_bwd_kernel(const TO* __restrict__ dout, int ocs, TI* __restrict__ din, 
 }
 
 // ---------------------------------------------------------------- adaptive average pool
-// grid = (N*S*S, chunks). Threads: (pixel lane, channel group of 8). fp32 atomics into out (pre-zeroed).
+// grid = (N*S*S, chunks). Threads: (pixel lane, channel group of 8). Each chunk stores its bin sums into workspace slot blockIdx.y.
 __global__ void __launch_bounds__(kThreads)
 adaptive_avgpool_fwd_kernel(const __nv_bfloat16* __restrict__ in, int ics, int N, int C, int H, int W, int S,
                             float* __restrict__ out) {
@@ -214,7 +214,8 @@ adaptive_avgpool_fwd_kernel(const __nv_bfloat16* __restrict__ in, int ics, int N
             for (int k = 0; k < 8; ++k) {
                 float s = 0.f;
                 for (int l = 0; l < lanes; ++l) s += s_acc[(l * groups_per_pass + g) * 8 + k];
-                atomicAdd(out + (long long)bin * C + cg * 8 + k, s * inv_area);
+                // slot blockIdx.y of the deterministic workspace; the chunks are summed in order afterwards
+                out[(long long)blockIdx.y * gridDim.x * C + (long long)bin * C + cg * 8 + k] = s * inv_area;
             }
         }
         __syncthreads();
@@ -460,8 +461,8 @@ extern "C" int tsb_bilinear_bwd(const void* dout, int odtype, int ocs, void* din
     return TSB_OK;
 }
 
-extern "C" int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, int H, int W, int S, float* out,
-                                        tsb_stream_t stream) {
+extern "C" int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, int H, int W, int S, float* out, float* ws,
+                                        long long ws_floats, tsb_stream_t stream) {
     TSB_REQUIRE(in && out, "tsb_adaptive_avgpool_fwd: null pointer");
     TSB_REQUIRE(C % 8 == 0 && ics % 8 == 0 && tsb_aligned16(in), "tsb_adaptive_avgpool_fwd: C, ics must be multiples of 8");
     TSB_REQUIRE(S >= 1 && S <= H && S <= W, "tsb_adaptive_avgpool_fwd: bad S");
@@ -477,9 +478,11 @@ extern "C" int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, i
     if (chunks > max_chunks) chunks = max_chunks;
     if (chunks < 1) chunks = 1;
     size_t smem = sizeof(float) * (size_t)lanes * groups * 8;
-    adaptive_avgpool_fwd_kernel<<<dim3(bins, chunks), kThreads, smem, st>>>((const __nv_bfloat16*)in, ics, N, C, H, W, S, out);
+    TSB_REQUIRE(ws && (long long)chunks * bins * C <= ws_floats, "tsb_adaptive_avgpool_fwd: workspace needs %lld floats",
+                (long long)chunks * bins * C);
+    adaptive_avgpool_fwd_kernel<<<dim3(bins, chunks), kThreads, smem, st>>>((const __nv_bfloat16*)in, ics, N, C, H, W, S, ws);
     TSB_CUDA_CHECK_LAUNCH("adaptive_avgpool_fwd");
-    return TSB_OK;
+    return tsb_det_reduce(out, ws, chunks, (long long)bins * C, (long long)bins * C, st);
 }
 
 extern "C" int tsb_adaptive_avgpool_bwd(const float* dout, int N, int C, int H, int W, int S, void* din, int ics,

@@ -19,6 +19,21 @@ void tsb_set_error(const char* fmt, ...) {
 
 void tsb_count_launch(int n) { g_tsb_launches.fetch_add(n, std::memory_order_relaxed); }
 
+__global__ void det_reduce_kernel(float* __restrict__ out, const float* __restrict__ parts, int nparts, long long n,
+                                  long long stride) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        float s = 0.f;
+        for (int b = 0; b < nparts; ++b) s += parts[(long long)b * stride + i];
+        out[i] += s;
+    }
+}
+
+int tsb_det_reduce(float* out, const float* parts, int nparts, long long n, long long stride, cudaStream_t st) {
+    det_reduce_kernel<<<tsb_grid_for(n, 256, 8), 256, 0, st>>>(out, parts, nparts, n, stride);
+    TSB_CUDA_CHECK_LAUNCH("det_reduce");
+    return TSB_OK;
+}
+
 extern "C" const char* tsb_last_error(void) { return g_err; }
 extern "C" int tsb_version(void) { return 100; }
 extern "C" long long tsb_launch_count(void) { return g_tsb_launches.load(); }

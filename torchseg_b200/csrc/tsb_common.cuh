@@ -1,4 +1,4 @@
-// Common device/host helpers for libtsb (B200 / sm_100a only).
+// Common device/host helpers for libtsb (H100 / sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -14,6 +14,12 @@
 void tsb_set_error(const char* fmt, ...);
 void tsb_count_launch(int n);
 int tsb_ensure_dyn_smem(const void* func, size_t bytes);   // per-(device, function), thread-safe
+
+// Deterministic cross-CTA sums. A kernel that would add per-CTA partials into one output with float atomics (whose
+// order, hence rounding, changes from run to run) instead stores partial b into slot b of the caller's workspace
+// (`ws`, `ws_floats` of the entry point); tsb_det_reduce then adds sum_b slot[b][i] (b in increasing order) to out[i].
+// Slot b of the partials starts at parts + b * stride.
+int tsb_det_reduce(float* out, const float* parts, int nparts, long long n, long long stride, cudaStream_t st);
 
 #define TSB_FAIL(code, ...)            \
     do {                               \
@@ -44,10 +50,10 @@ int tsb_ensure_dyn_smem(const void* func, size_t bytes);   // per-(device, funct
 static inline int tsb_num_sms() {
     static int sms[64] = {0};   // per device; a racing first call writes the same value twice
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (sms[dev] == 0) {
         int v = 0;
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         sms[dev] = v;
     }
     return sms[dev];
@@ -109,19 +115,13 @@ __device__ __forceinline__ void stg_v4(void* p, const uint4& v) {
     asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.256): a thread that owns 32 or 64 contiguous bytes fills whole 32-byte
-// sectors per instruction instead of half sectors with 16-byte accesses. `p` must be 32-byte aligned.
-__device__ __forceinline__ void stg_v8(void* p, const uint4& a, const uint4& b) {
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w),
-                 "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-                 : "memory");
+// weight-gradient epilogues: store into this split's workspace slice, or add in place when the CTA is the only writer
+__device__ __forceinline__ void put_f2(float* p, float a, float b, bool add) {
+    float2 v = make_float2(a, b);
+    if (add) { const float2 o = *reinterpret_cast<const float2*>(p); v.x += o.x; v.y += o.y; }
+    *reinterpret_cast<float2*>(p) = v;
 }
-__device__ __forceinline__ void ldg_v8(const void* p, uint4& a, uint4& b) {
-    asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-                 : "l"(p)
-                 : "memory");
-}
+__device__ __forceinline__ void put_f1(float* p, float a, bool add) { *p = add ? *p + a : a; }
 
 __device__ __forceinline__ float bf16lo(uint32_t u) { return __uint_as_float(u << 16); }
 __device__ __forceinline__ float bf16hi(uint32_t u) { return __uint_as_float(u & 0xffff0000u); }

@@ -1,4 +1,4 @@
-"""Engine / State with the reference API (/root/reference/furnace/engine/engine.py:23-163): argparse injection
+"""Engine / State with the reference API (TorchSeg furnace/engine/engine.py:23-163): argparse injection
 (-d / -c / --local_rank), WORLD_SIZE detection, process-group init, state registry, checkpoint
 save / link / restore in the reference's on-disk format.
 
@@ -55,7 +55,7 @@ class Engine(object):
 
     def __init__(self, custom_parser=None, argv=None):
         self.version = __version__
-        logger.info("PyTorch Version {}, Furnace(B200) Version {}".format(torch.__version__, self.version))
+        logger.info("PyTorch Version {}, Furnace(libtsb) Version {}".format(torch.__version__, self.version))
         self.state = State()
         self.devices, self.distributed, self.local_rank, self.world_size = None, False, 0, 1
         if custom_parser is not None and not isinstance(custom_parser, argparse.ArgumentParser):

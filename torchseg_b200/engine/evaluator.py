@@ -1,8 +1,8 @@
-"""Evaluator with the reference's surface (/root/reference/furnace/engine/evaluator.py): `whole_eval`, `sliding_eval`,
+"""Evaluator with the reference's surface (TorchSeg furnace/engine/evaluator.py): `whole_eval`, `sliding_eval`,
 `scale_process`, `val_func_process`, `process_image`, `func_per_iteration` / `compute_metric` hooks and a
 single-process `run`. SURVEY.md §8f rank 2 — the first slice of the evaluator row.
 
-What is B200-first here: all sliding-window crops of one scale go through the network in ONE batched forward (the
+What is GPU-first here: all sliding-window crops of one scale go through the network in ONE batched forward (the
 reference runs them one by one, evaluator.py:222-239) and are accumulated on the device; the eval-mode network forward
 itself is the libtsb path (BN from running statistics). What deliberately stays on the host, exactly like the
 reference, so that predictions can be compared pixel by pixel: cv2 resizing of the input per scale and of the

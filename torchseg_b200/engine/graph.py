@@ -1,6 +1,6 @@
 """Whole-step CUDA graph for the train loop (zero_grad → forward(loss) → backward → fused SGD step).
 
-The step of /root/reference/model/bisenet/cityscapes.bisenet.R18/train.py:116-142 is ~400 kernel launches of 5-200 us
+The step of TorchSeg model/bisenet/cityscapes.bisenet.R18/train.py:116-142 is ~400 kernel launches of 5-200 us
 each; captured once, a replay removes the per-launch CPU work (Python autograd, ctypes, tensor-map encoding) and the
 inter-kernel launch gaps. One process per GPU; with `ddp=` the gradient all-reduce and the SyncBN exchanges are part of the graph.
 
@@ -12,7 +12,7 @@ Usage:
 If capture is impossible (non-CUDA device, an op that cannot be captured) the object runs eager steps and keeps the
 reason in `.error`.
 
-Requirements (verified on B200, tools/diag_graph.py — each variant in its own process):
+Requirements (tools/diag_graph.py — each variant in its own process):
   * everything runs on ONE non-default stream (`torch.cuda.set_stream(torch.cuda.Stream())` at program start): work that
     touches the legacy default stream during a capture invalidates it;
   * NO autograd graph of an earlier eager step may be alive when the object is constructed — e.g. a `loss` tensor still

@@ -1,4 +1,4 @@
-"""get_logger with the reference's behaviour (/root/reference/furnace/engine/logger.py:82-99): root logger,
+"""get_logger with the reference's behaviour (TorchSeg furnace/engine/logger.py:82-99): root logger,
 level from ENGINE_LOGGING_LEVEL, optional file handler, coloured stream handler."""
 import logging
 import os

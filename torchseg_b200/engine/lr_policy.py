@@ -1,5 +1,5 @@
 """Learning-rate schedules with the reference's class names and `get_lr(step)` protocol
-(/root/reference/furnace/engine/lr_policy.py:11-49). Each schedule is a small callable table: the train loops only
+(TorchSeg furnace/engine/lr_policy.py:11-49). Each schedule is a small callable table: the train loops only
 ever call `policy.get_lr(iteration)` (train.py:133) and read nothing else, except `PolyLR.start_lr / lr_power /
 total_iters`, which stay public."""
 

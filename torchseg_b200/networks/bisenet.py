@@ -1,5 +1,5 @@
 """BiSeNet (ResNet-18 context path) with the reference's class / attribute names
-(/root/reference/model/bisenet/cityscapes.bisenet.R18/network.py:18-168) on the libtsb path.
+(TorchSeg model/bisenet/cityscapes.bisenet.R18/network.py:18-168) on the libtsb path.
 
 Training forward returns the scalar loss exactly like the reference (`loss = model(imgs, gts)`); the three
 heads end in the FUSED bilinear-upsample + OHEM loss when the criterion supports it

@@ -1,5 +1,5 @@
 """DFN (ResNet-101 v1c) with the reference's class / attribute / state_dict names
-(/root/reference/model/dfn/cityscapes.dfn.R101_v1c/network.py:15-172) on the libtsb path.
+(TorchSeg model/dfn/cityscapes.dfn.R101_v1c/network.py:15-172) on the libtsb path.
 
 Training forward returns `Σ₄ criterion(smooth head) + alpha · Σ₄ aux_criterion(border head)` (network.py:139-152).
 Smooth network (network.py:94-119): global context → per stage RRB → CAB(with the up-sampled deeper stage) → RRB →

@@ -1,4 +1,4 @@
-"""FCN-32s with the reference's class / attribute names (/root/reference/model/fcn/voc.fcn32s.R101_v1c/network.py:13-68).
+"""FCN-32s with the reference's class / attribute names (TorchSeg model/fcn/voc.fcn32s.R101_v1c/network.py:13-68).
 BASELINE configs[0] uses the ResNet-18 variant (SURVEY.md §8 a15): resnet18(deep_stem=False) with
 _FCNHead(512, .) / _FCNHead(256, .). Training forward returns `loss + aux_ratio * aux_loss` (network.py:43-47)
 through the fused bilinear-upsample + cross-entropy kernels (plain CE == OHEM with min_kept = 0)."""

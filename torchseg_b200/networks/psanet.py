@@ -1,10 +1,10 @@
 """PSANet (ResNet-101 v1c, dilated-8, point-wise spatial attention head) with the reference's class / attribute /
-state_dict names (/root/reference/model/psanet/ade.psanet.R101_v1c/network.py:14-144 — the reference class is still
+state_dict names (TorchSeg model/psanet/ade.psanet.R101_v1c/network.py:14-144 — the reference class is still
 called `PSPNet` there; both names are exported) on the libtsb path.
 
 The PSA head needs exactly h*w = 3600 positions at 1/8 resolution (480x480 or 473x473 inputs, network.py:88,101):
 the 3600-channel attention maps are soft-maxed over their channel dimension and contracted with the 512-channel
-reduced feature map by `torch.bmm`; here both contractions (and their two backward GEMMs) run on the tcgen05 1x1
+reduced feature map by `torch.bmm`; here both contractions (and their two backward GEMMs) run on the wgmma 1x1
 convolution kernels (ops.PSABmmFn). Loss: `criterion(log_softmax(x8 up-sampled logits)) + 0.4 * aux` (network.py:41-57),
 evaluated like PSPNet through the OHEM kernels with min_kept = 0."""
 from functools import partial

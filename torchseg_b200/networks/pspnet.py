@@ -1,5 +1,5 @@
 """PSPNet (ResNet-101 v1c, dilated-8) with the reference's class / attribute / state_dict names
-(/root/reference/model/pspnet/ade.pspnet.R101_v1c/network.py:14-109) on the libtsb path.
+(TorchSeg model/pspnet/ade.pspnet.R101_v1c/network.py:14-109) on the libtsb path.
 
 Training forward returns `loss + 0.4 * aux_loss` (network.py:53-57). The reference applies log_softmax and then
 nn.CrossEntropyLoss (a second, idempotent log_softmax); here each head ends in ONE fused kernel pair (bilinear up-sampling to

@@ -1,6 +1,6 @@
 """torch.autograd.Function wrappers around the libtsb C ABI (include/tsb.h).
 
-PyTorch drives only the graph, the memory and the streams; every op below runs a hand-written sm_100a
+PyTorch drives only the graph, the memory and the streams; every op below runs a hand-written sm_90a
 kernel. Activations are bf16 tensors of LOGICAL shape [N,C,H,W] stored NHWC (`nhwc_empty`), possibly a
 channel slice of a wider buffer (channel stride `cs`). There is no CPU / ATen fallback: without a GPU or
 without libtsb.so these functions raise.
@@ -8,7 +8,7 @@ without libtsb.so these functions raise.
 import torch
 
 from . import _lib
-from ._lib import BF16, F32, ConvShape, call, ptr, stream
+from ._lib import BF16, F32, ConvShape, call, det_ws, ptr, stream
 
 import ctypes
 import weakref
@@ -345,7 +345,7 @@ def conv_fprop(x, wb, K, R, stride, pad, dil, bias=None, out_dtype=_BF, out=None
         s1, s2 = stats[0], stats[1]
     ev = conv_prof.begin()
     call("tsb_conv2d_fprop", ctypes.byref(shp), ptr(x), cs_of(x), ptr(wb), ptr(bias), ptr(out), _lib.dt(out), cs_of(out),
-         ptr(s1), ptr(s2), stream())
+         ptr(s1), ptr(s2), *det_ws(), stream())
     conv_prof.end(ev, _conv_flops(shp))
     return out
 
@@ -432,7 +432,7 @@ def conv_wgrad(x, dy, K, R, stride, pad, dil, dw_krsc):
     N, C, H, W = x.shape
     shp = make_shape(N, H, W, C, K, R, stride, pad, dil)
     ev = conv_prof.begin()
-    call("tsb_conv2d_wgrad", ctypes.byref(shp), ptr(x), cs_of(x), ptr(dy), cs_of(dy), ptr(dw_krsc), stream())
+    call("tsb_conv2d_wgrad", ctypes.byref(shp), ptr(x), cs_of(x), ptr(dy), cs_of(dy), ptr(dw_krsc), *det_ws(), stream())
     conv_prof.end(ev, _conv_flops(shp))
 
 
@@ -478,8 +478,8 @@ class GradShare(object):
 class ConvBNActFn(torch.autograd.Function):
     """y = act(BN_train(conv(x, w)) + residual).
 
-    Replaces ConvBnRelu.forward (/root/reference/furnace/seg_opr/seg_oprs.py:39-46) and the conv→bn→(+res)→relu
-    groups of BasicBlock.forward (/root/reference/furnace/base_model/resnet.py:33-53). The conv epilogue emits
+    Replaces ConvBnRelu.forward (TorchSeg furnace/seg_opr/seg_oprs.py:39-46) and the conv→bn→(+res)→relu
+    groups of BasicBlock.forward (TorchSeg furnace/base_model/resnet.py:33-53). The conv epilogue emits
     the per-channel Σ/Σ² (BN statistics), tsb_bn_finalize turns them into scale/shift (and updates the
     running stats), tsb_bn_apply normalises (+residual, +ReLU) in one pass.
     """
@@ -504,7 +504,7 @@ class ConvBNActFn(torch.autograd.Function):
             wp, _ = pack_cache.get(w, False, stem=True)
             ev = conv_prof.begin()
             call("tsb_conv_stem_fprop", ptr(x), N, H, W, ptr(wp), K, ptr(raw), K, ptr(stats[0]) if training else None,
-                 ptr(stats[1]) if training else None, stream())
+                 ptr(stats[1]) if training else None, *det_ws(), stream())
             conv_prof.end(ev, 2.0 * N * P * Q * K * 147)
         else:
             wb, _ = pack_cache.get(w, False)
@@ -548,7 +548,7 @@ class ConvBNActFn(torch.autograd.Function):
         # ReLU mask: recomputed from raw*scale+shift when there is no residual (saves reading y in both passes)
         y_mask = ptr(y) if (relu and has_res) else None
         call("tsb_bn_bwd_reduce", ptr(dy), cs_of(dy), y_mask, K, ptr(raw), K, ptr(aux[0]), ptr(aux[1]), int(relu), npix, K,
-             ptr(red[0]), ptr(red[1]), ptr(aux[2]), ptr(aux[3]), stream())
+             ptr(red[0]), ptr(red[1]), ptr(aux[2]), ptr(aux[3]), *det_ws(), stream())
         # dgamma = Σ dz·x̂, dbeta = Σ dz are LOCAL sums (the DDP all-reduce averages parameter grads);
         # the dx formula needs the GLOBAL sums under SyncBN.
         beta = ctx.beta_ref
@@ -576,7 +576,7 @@ class ConvBNActFn(torch.autograd.Function):
             H, W = P * 2, Q * 2
             dwp = zero_arena.take((K, 4, 64), dev)
             ev = conv_prof.begin()
-            call("tsb_conv_stem_wgrad", ptr(x), N, H, W, ptr(draw), K, K, ptr(dwp), stream())
+            call("tsb_conv_stem_wgrad", ptr(x), N, H, W, ptr(draw), K, K, ptr(dwp), *det_ws(), stream())
             conv_prof.end(ev, 2.0 * N * P * Q * K * 147)
             call("tsb_unpack_stem_wgrad", ptr(dwp), K, R, ptr(dw), stream())
         else:
@@ -600,7 +600,7 @@ class ConvBNActFn(torch.autograd.Function):
 
 class StemPairFn(torch.autograd.Function):
     """The TWO 7x7/2 stems of BiSeNet (spatial_path.conv_7x7, bisenet network.py:118, and context_path.conv1,
-    resnet.py:126) read the same image: one tcgen05 launch computes both (K = 64 + 64 output channels, N = 128 MMA
+    resnet.py:126) read the same image: one conv launch computes both (K = 64 + 64 output channels, N = 128 MMA
     tiles), one BN-apply pass normalises both, one wgrad launch produces both weight gradients. Returns the two
     64-channel halves as channel-slice views of one NHWC buffer."""
 
@@ -621,7 +621,7 @@ class StemPairFn(torch.autograd.Function):
         for off, Kh in ((0, K1), (K1, K2)):
             ev = conv_prof.begin()
             call("tsb_conv_stem_fprop", ptr(xs), N, H, W, ptr(wp[off:]), Kh, ptr(raw[:, off:]), K, ptr(stats[0][off:]),
-                 ptr(stats[1][off:]), stream())
+                 ptr(stats[1][off:]), *det_ws(), stream())
             conv_prof.end(ev, 2.0 * N * P * Q * Kh * 147)
         _allreduce_stats(stats)
         count = float(N * P * Q) * _sync["world"]
@@ -653,7 +653,7 @@ class StemPairFn(torch.autograd.Function):
             red = zero_arena.take((2, Kh), dev)
             xr = raw[:, off:off + Kh]
             call("tsb_bn_bwd_reduce", ptr(dy), cs_of(dy), None, 0, ptr(xr), K, ptr(aux[0][off:]), ptr(aux[1][off:]), 1, npix, Kh,
-                 ptr(red[0]), ptr(red[1]), ptr(aux[2][off:]), ptr(aux[3][off:]), stream())
+                 ptr(red[0]), ptr(red[1]), ptr(aux[2][off:]), ptr(aux[3][off:]), *det_ws(), stream())
             direct = _direct_grad(w) and _direct_grad(g) and _direct_grad(b)
             fold = direct and _sync["world"] == 1
             dg, db = (None, None) if direct else (red[1].clone(), red[0].clone())
@@ -665,7 +665,7 @@ class StemPairFn(torch.autograd.Function):
         H, W = P * 2, Q * 2
         dwp = zero_arena.take((K, 4, 64), dev)
         ev = conv_prof.begin()
-        call("tsb_conv_stem_wgrad", ptr(xs), N, H, W, ptr(draw), K, K, ptr(dwp), stream())
+        call("tsb_conv_stem_wgrad", ptr(xs), N, H, W, ptr(draw), K, K, ptr(dwp), *det_ws(), stream())
         conv_prof.end(ev, 2.0 * N * P * Q * K * 147)
         outs = []
         for (off, w, g, b), (direct, dg, db) in zip(((0, w1, g1, b1), (K1, w2, g2, b2)), grads):
@@ -723,7 +723,7 @@ class ConvFn(torch.autograd.Function):
         db = None
         if has_bias:
             db = ctx.bias_ref.grad if direct else torch.zeros((K,), dtype=torch.float32, device=dev)
-            call("tsb_bias_grad", ptr(dyb), Kp, N * P * Q, K, ptr(db), stream())
+            call("tsb_bias_grad", ptr(dyb), Kp, N * P * Q, K, ptr(db), *det_ws(), stream())
             if direct:
                 db = None
         dx = None
@@ -739,7 +739,7 @@ class ConvFn(torch.autograd.Function):
 # pooling / resize / attention scale
 # --------------------------------------------------------------------------------------------------
 class MaxPool3x3S2Fn(torch.autograd.Function):
-    """nn.MaxPool2d(3, 2, 1) — /root/reference/furnace/base_model/resnet.py:132"""
+    """nn.MaxPool2d(3, 2, 1) — TorchSeg furnace/base_model/resnet.py:132"""
 
     @staticmethod
     def forward(ctx, x):
@@ -771,7 +771,7 @@ class AdaptiveAvgPoolFn(torch.autograd.Function):
     def forward(ctx, x, S):
         N, C, H, W = x.shape
         o32 = torch.empty((N, S, S, C), dtype=torch.float32, device=x.device)
-        call("tsb_adaptive_avgpool_fwd", ptr(x), cs_of(x), N, C, H, W, S, ptr(o32), stream())
+        call("tsb_adaptive_avgpool_fwd", ptr(x), cs_of(x), N, C, H, W, S, ptr(o32), *det_ws(), stream())
         out = nhwc_empty(N, C, S, S, device=x.device)
         call("tsb_cast_scale", ptr(o32), F32, C, ptr(out), BF16, C, N * S * S, C, None, stream())
         ctx.shape = (N, C, H, W, S)
@@ -823,7 +823,7 @@ class BilinearFn(torch.autograd.Function):
             # broadcast forward (1x1 → HxW, bisenet network.py:82-84) ⇒ the backward is a plain spatial sum: reuse the
             # pooling reduction (mean) and scale by H*W instead of a one-block gather
             m32 = torch.empty((N, 1, 1, C), dtype=torch.float32, device=dy.device)
-            call("tsb_adaptive_avgpool_fwd", ptr(dy), cs_of(dy), N, C, Ho, Wo, 1, ptr(m32), stream())
+            call("tsb_adaptive_avgpool_fwd", ptr(dy), cs_of(dy), N, C, Ho, Wo, 1, ptr(m32), *det_ws(), stream())
             call("tsb_cast_scale", ptr(m32), F32, C, ptr(dx), BF16, C, N, C, ptr(_const_scalar(float(Ho * Wo), dy.device)), stream())
         else:
             call("tsb_bilinear_bwd", ptr(dy), BF16, cs_of(dy), ptr(dx), BF16, C, N, C, Hi, Wi, Ho, Wo, 0, stream())
@@ -856,7 +856,7 @@ class ChanScaleFn(torch.autograd.Function):
         dx = nhwc_empty(N, C, H, W, device=x.device)
         da32 = torch.zeros((N, C), dtype=torch.float32, device=x.device)
         call("tsb_chan_scale_bwd", ptr(dy), cs_of(dy), ptr(x), cs_of(x), ptr(a32), float(base), ptr(dx), C, ptr(da32), N,
-             H * W, C, stream())
+             H * W, C, *det_ws(), stream())
         da = nhwc_empty(N, C, 1, 1, device=x.device)
         call("tsb_cast_scale", ptr(da32), F32, C, ptr(da), BF16, C, N, C, None, stream())
         return dx, da, (dy if has_add else None), None
@@ -911,7 +911,7 @@ class PSABmmFn(torch.autograd.Function):
     NHWC form per image: out[j, ch] = Σ_i S[j, i] · x[i, ch] with S = row-softmax of att[j, :]. That is a 1x1
     convolution whose "image" is S (L pixels x L channels, zero-padded to a multiple of 64 channels) and whose weight
     operand is the image's own feature map transposed ([c, L]); dS is the matching dgrad (weight operand = x itself),
-    dx the matching wgrad. All three run on the tcgen05 conv kernels, one launch per image."""
+    dx the matching wgrad. All three run on the wgmma conv kernels, one launch per image."""
 
     @staticmethod
     def forward(ctx, x, att):
@@ -990,7 +990,7 @@ def _ohem_forward(pt_call, n, labels, ignore_label, thresh, min_kept, class_weig
 
 class OhemCEFn(torch.autograd.Function):
     """ProbOhemCrossEntropy2d.forward on MATERIALISED logits [N,C,H,W] (any strides, fp32/bf16) —
-    /root/reference/furnace/seg_opr/loss_opr.py:68-98."""
+    TorchSeg furnace/seg_opr/loss_opr.py:68-98."""
 
     @staticmethod
     def forward(ctx, pred, target, ignore_label, thresh, min_kept, class_weight):

@@ -135,7 +135,7 @@ class SGD(object):
         self.pack.mark_fresh()       # ... and the flat bf16 mirror written by the kernel above is current
 
     # ---- checkpoint format: torch.optim.SGD's (what the reference stores under 'optimizer',
-    # /root/reference/furnace/engine/engine.py:103,142-146): {'state': {i: {'momentum_buffer': [K,C,R,S] fp32}},
+    # TorchSeg furnace/engine/engine.py:103,142-146): {'state': {i: {'momentum_buffer': [K,C,R,S] fp32}},
     # 'param_groups': [{'lr','momentum','dampening','weight_decay','nesterov',..., 'params': [indices]}]}
     def state_dict(self):
         groups, idx = [], 0

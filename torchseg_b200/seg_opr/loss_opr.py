@@ -1,4 +1,4 @@
-"""Losses with the reference API (/root/reference/furnace/seg_opr/loss_opr.py)."""
+"""Losses with the reference API (TorchSeg furnace/seg_opr/loss_opr.py)."""
 import torch
 import torch.nn as nn
 
@@ -7,7 +7,7 @@ from .. import ops
 
 class ProbOhemCrossEntropy2d(nn.Module):
     """loss_opr.py:48-98 — same constructor; forward(pred, target) takes MATERIALISED [b,c,h,w] logits exactly like
-    the reference. `forward_lowres` is the fused-upsample form used by the B200 networks: it consumes the
+    the reference. `forward_lowres` is the fused-upsample form used by the libtsb networks: it consumes the
     low-resolution head output and never writes the full-resolution logits."""
 
     CITYSCAPES_WEIGHT = [1.4297, 1.4805, 1.4363, 3.365, 2.6635, 1.4311, 2.1943, 1.4817, 1.4513, 2.1984, 1.5295,

@@ -1,5 +1,5 @@
 """Segmentation metrics with the reference's function names and return conventions
-(/root/reference/furnace/seg_opr/metric.py) — the host-side half of the Evaluator row (SURVEY.md §8f rank 2).
+(TorchSeg furnace/seg_opr/metric.py) — the host-side half of the Evaluator row (SURVEY.md §8f rank 2).
 
 VOC / Cityscapes protocol: a confusion matrix over the labelled pixels (`hist_info`) reduced to per-class IoU, mean IoU
 (with and without class 0) and pixel accuracy (`compute_score`). ADE protocol: per-image intersection / union areas with

@@ -1,5 +1,5 @@
-"""B200-native building blocks with the reference's names, constructor signatures and child-module names
-(/root/reference/furnace/seg_opr/seg_oprs.py). Parameters live in genuine nn.Conv2d / norm_layer children —
+"""H100-native building blocks with the reference's names, constructor signatures and child-module names
+(TorchSeg furnace/seg_opr/seg_oprs.py). Parameters live in genuine nn.Conv2d / norm_layer children —
 `group_weight`'s completeness assert (furnace/utils/init_func.py:52-53) and the checkpoint keys (SURVEY.md
 App. D) depend on that — only `forward` is replaced by the fused libtsb path.
 """

@@ -1,6 +1,6 @@
 """Device-side training input pipeline (SURVEY §8 f4) behind the reference's TrainPre protocol.
 
-`TrainPreGPU` restates TrainPre.__call__ (/root/reference/model/bisenet/cityscapes.bisenet.R18/dataloader.py:11-33): the
+`TrainPreGPU` restates TrainPre.__call__ (TorchSeg model/bisenet/cityscapes.bisenet.R18/dataloader.py:11-33): the
 random draws (mirror, scale, crop position) are made on the host with Python's `random` module in the reference's order
 (furnace/utils/img_utils.py:141, :119, :54-58 — same seed ⇒ same augmentation), everything that touches pixels —
 cv2.flip, cv2.resize (INTER_LINEAR image / INTER_NEAREST label), normalize, crop + centred pad, HWC→CHW — runs as ONE

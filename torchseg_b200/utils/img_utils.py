@@ -1,4 +1,4 @@
-"""Host-side image helpers used by the evaluator (/root/reference/furnace/utils/img_utils.py:8-21,60-74,181-187):
+"""Host-side image helpers used by the evaluator (TorchSeg furnace/utils/img_utils.py:8-21,60-74,181-187):
 shape canonicalisation, centred constant padding up to a crop size, 0-1 scaling + mean / std normalisation.
 cv2 is only needed by pad_image_to_shape (and is imported lazily)."""
 from collections.abc import Iterable

@@ -1,4 +1,4 @@
-"""init_weight / group_weight with the reference semantics (/root/reference/furnace/utils/init_func.py:11-57)."""
+"""init_weight / group_weight with the reference semantics (TorchSeg furnace/utils/init_func.py:11-57)."""
 import torch.nn as nn
 
 _CONV = (nn.Conv2d, nn.Conv3d, nn.ConvTranspose2d)

@@ -1,5 +1,5 @@
 """Host→device input prefetcher for the train loop (the `minibatch = dataloader.next(); imgs.cuda(non_blocking=True)`
-step of /root/reference/model/bisenet/cityscapes.bisenet.R18/train.py:119-124).
+step of TorchSeg model/bisenet/cityscapes.bisenet.R18/train.py:119-124).
 
 Copies batch i+1 from pinned host memory on a side stream into one of TWO persistent device buffers while step i
 computes (no per-step device allocation), and hands out the device tensors with the correct stream dependencies.

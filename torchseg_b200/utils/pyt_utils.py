@@ -1,4 +1,4 @@
-"""API-compatible helpers (/root/reference/furnace/utils/pyt_utils.py): all_reduce_tensor, load_model,
+"""API-compatible helpers (TorchSeg furnace/utils/pyt_utils.py): all_reduce_tensor, load_model,
 parse_devices, link_file, ensure_dir, extant_file."""
 import argparse
 import logging
