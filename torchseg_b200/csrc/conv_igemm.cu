@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __gr
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kWgBarOff);
     uint64_t* empty_bar = full_bar + kWgStages;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = warp_uniform_idx(), lane = threadIdx.x & 31;
     const int split = blockIdx.x;
     const int co0 = blockIdx.y * 128;
     const int box0 = blockIdx.z * p.nb;
@@ -103,12 +103,14 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __gr
         for (int j = 0; j < 4; ++j)
 #pragma unroll
             for (int q = 0; q < 32; ++q) acc[j][q] = 0.f;
-        int s = 0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) fence_operands(acc[j]);
+        // a stage is released one stage late: wait_group<1> after issuing stage s retires the MMAs of stage s-1, so the
+        // tensor pipe never drains between stages
+        int s = 0, prev = -1;
         uint32_t ph = 0;
         for (int it = 0; it < total_iters; ++it) {
             mbar_wait(&full_bar[s], ph);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) fence_operands(acc[j]);
             wgmma_fence();
             const uint32_t a_lo = base_lo + (uint32_t)(s * (kWgStageBytes >> 4)) + (uint32_t)c * (kWgBoxBytes >> 4);
             const uint32_t b_lo = base_lo + (uint32_t)(s * (kWgStageBytes >> 4)) + ((2 * kWgBoxBytes) >> 4);
@@ -122,13 +124,18 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __gr
                 }
             }
             wgmma_commit();
-            wgmma_wait<0>();
-#pragma unroll
-            for (int j = 0; j < 4; ++j) fence_operands(acc[j]);
-            // wait_group covers only this warp's MMAs: every consumer warp releases the stage
-            if (lane == 0) mbar_arrive(&empty_bar[s]);
+            if (prev >= 0) {
+                wgmma_wait<1>();
+                // wait_group covers only this warp's MMAs: every consumer warp releases the stage
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            }
+            prev = s;
             if (++s == kWgStages) { s = 0; ph ^= 1u; }
         }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int j = 0; j < 4; ++j) fence_operands(acc[j]);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int co = co0 + c * 64 + wq * 16 + (lane >> 2) + 8 * h;

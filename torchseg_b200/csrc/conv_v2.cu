@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
     uint64_t* b_ready = empty_bar + kMaxStages;
     float* s_stats = reinterpret_cast<float*>(tail + 256);  // [consumer warp][2*BN]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = warp_uniform_idx(), lane = threadIdx.x & 31;
     const int n0 = blockIdx.y * BN;
     const int my_tiles = (p.m_tiles > (int)blockIdx.x) ? (p.m_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     constexpr int kBTile = BN * 128;
@@ -140,33 +140,38 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
             float acc[BN / 2];
 #pragma unroll
             for (int q = 0; q < BN / 2; ++q) acc[q] = 0.f;
+            fence_operands(acc);
+            // a stage is released one stage late: wait_group<1> after issuing stage s retires the MMAs of stage s-1, so
+            // the tensor pipe never drains between stages of a tile (wait_group covers only this warp's MMAs: every
+            // consumer warp releases the stage)
+            int prev = -1;
             for (int g = 0; g < p.ngroups; ++g) {
                 const int ntaps = p.groups[g].ntaps;
                 for (int kc = 0; kc < p.kchunks; ++kc) {
                     mbar_wait(&full_bar[sl], ph);
-                    fence_operands(acc);
                     wgmma_fence();
                     const uint32_t st_lo = stages_lo + (uint32_t)(sl * p.stage_bytes >> 4);
+                    for (int t = 0; t < ntaps; ++t) {
+                        const uint32_t a_lo = st_lo + (uint32_t)c * 512u + (uint32_t)p.groups[g].row_off[t] * 8u;
+                        const uint32_t b_lo = RES ? res_lo + (uint32_t)((p.groups[g].tap_idx[t] * p.kchunks + kc) * kBTile >> 4)
+                                                  : st_lo + (uint32_t)((kAStageBytes + t * kBTile) >> 4);
 #pragma unroll
-                    for (int t = 0; t < 3; ++t) {
-                        if (t < ntaps) {
-                            const uint32_t a_lo = st_lo + (uint32_t)c * 512u + (uint32_t)p.groups[g].row_off[t] * 8u;
-                            const uint32_t b_lo = RES ? res_lo + (uint32_t)((p.groups[g].tap_idx[t] * p.kchunks + kc) * kBTile >> 4)
-                                                      : st_lo + (uint32_t)((kAStageBytes + t * kBTile) >> 4);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k)   // 16 bf16 = 32 B = 2 descriptor units inside the swizzle atom
-                                wgmma_kmajor<BN>(acc, desc_at(desc_hi, a_lo + 2 * k, p.use_base_offset),
-                                                 desc_at(desc_hi, b_lo + 2 * k, 0));
-                        }
+                        for (int k = 0; k < 4; ++k)   // 16 bf16 = 32 B = 2 descriptor units inside the swizzle atom
+                            wgmma_kmajor<BN>(acc, desc_at(desc_hi, a_lo + 2 * k, p.use_base_offset),
+                                             desc_at(desc_hi, b_lo + 2 * k, 0));
                     }
                     wgmma_commit();
-                    wgmma_wait<0>();
-                    fence_operands(acc);
-                    // wait_group covers only this warp's MMAs: every consumer warp releases the stage
-                    if (lane == 0) mbar_arrive(&empty_bar[sl]);
+                    if (prev >= 0) {
+                        wgmma_wait<1>();
+                        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                    }
+                    prev = sl;
                     if (++sl == p.nstages) { sl = 0; ph ^= 1u; }
                 }
             }
+            wgmma_wait<0>();
+            fence_operands(acc);
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
             const int tile = blockIdx.x + i * gridDim.x;
             const int tw_i = tile % p.tiles_w;
             const int th_i = (tile / p.tiles_w) % p.tiles_h;
@@ -228,7 +233,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
             // fixed summation order everywhere (no float atomics): per-warp slots, summed in warp order; the CTA's
             // totals go to its workspace slot and tsb_det_reduce adds the slots in CTA order
             if (lane < 4) {
-                float* sw = s_stats + warp * 2 * BN;
+                float* sw = s_stats + (threadIdx.x >> 5) * 2 * BN;   // re-derived: keeping `warp` live spills at BN = 128
 #pragma unroll
                 for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
@@ -286,7 +291,7 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_co
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kWrStages * kWrStageBytes);
     uint64_t* empty_bar = full_bar + kWrStages;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = warp_uniform_idx(), lane = threadIdx.x & 31;
     const int co0 = blockIdx.y * 128;
     const int g = blockIdx.z / p.cchunks, cc = blockIdx.z - g * p.cchunks;
     const WrGroup G = p.groups[g];
@@ -330,12 +335,13 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_co
         for (int t = 0; t < 3; ++t)
 #pragma unroll
             for (int q = 0; q < 32; ++q) acc[t][q] = 0.f;
-        int s = 0;
+#pragma unroll
+        for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
+        // a stage is released one stage late (wait_group<1> retires the previous stage's MMAs), as in igemm_v2_kernel
+        int s = 0, prev = -1;
         uint32_t ph = 0;
         for (int it = 0; it < total_iters; ++it) {
             mbar_wait(&full_bar[s], ph);
-#pragma unroll
-            for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
             wgmma_fence();
             const uint32_t a_lo = base_lo + (uint32_t)(s * (kWrStageBytes >> 4)) + (uint32_t)c * 512u;
             const uint32_t b_lo = base_lo + (uint32_t)(s * (kWrStageBytes >> 4)) + (kWrABytes >> 4);
@@ -349,13 +355,17 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_co
                 }
             }
             wgmma_commit();
-            wgmma_wait<0>();
-#pragma unroll
-            for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
-            // wait_group covers only this warp's MMAs: every consumer warp releases the stage
-            if (lane == 0) mbar_arrive(&empty_bar[s]);
+            if (prev >= 0) {
+                wgmma_wait<1>();
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            }
+            prev = s;
             if (++s == kWrStages) { s = 0; ph ^= 1u; }
         }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int co = co0 + c * 64 + wq * 16 + (lane >> 2) + 8 * h;

@@ -51,7 +51,7 @@ __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_
     uint8_t* tail = smem + p.nstages * p.stage_bytes;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
     uint64_t* empty_bar = full_bar + kTpMaxStages;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = warp_uniform_idx(), lane = threadIdx.x & 31;
     const int co0 = blockIdx.y * 64, ci0 = blockIdx.z * 64;
     const int t_begin = blockIdx.x * p.tiles_per_split;
     const int t_end = min(p.total_tiles, t_begin + p.tiles_per_split);
@@ -100,12 +100,14 @@ __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_
         for (int t = 0; t < 3; ++t)
 #pragma unroll
             for (int q = 0; q < 32; ++q) acc[t][q] = 0.f;
-        int s = 0;
+#pragma unroll
+        for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
+        // a stage is released one stage late: wait_group<1> after issuing stage s retires the MMAs of stage s-1, so the
+        // tensor pipe never drains between stages
+        int s = 0, prev = -1;
         uint32_t ph = 0;
         for (int it = 0; it < iters; ++it) {
             mbar_wait(&full_bar[s], ph);
-#pragma unroll
-            for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
             wgmma_fence();
             const uint32_t st_lo = base_lo + (uint32_t)(s * (p.stage_bytes >> 4));
             const uint32_t x_lo = st_lo + (kTpDyBytes >> 4) + (uint32_t)r * ((uint32_t)p.slot_bytes >> 4);
@@ -117,13 +119,18 @@ __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_
                     wgmma_m64n64<1, 1>(acc[t], desc_at(desc_hi, x_lo + t * tap16 + ka[k], p.use_base_offset), db, 1u);
             }
             wgmma_commit();
-            wgmma_wait<0>();
-#pragma unroll
-            for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
-            // wait_group covers only this warp's MMAs: every consumer warp releases the stage
-            if (lane == 0) mbar_arrive(&empty_bar[s]);
+            if (prev >= 0) {
+                wgmma_wait<1>();
+                // wait_group covers only this warp's MMAs: every consumer warp releases the stage
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            }
+            prev = s;
             if (++s == p.nstages) { s = 0; ph ^= 1u; }
         }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
         // fragment: rows = input channels ci0 + 16·wq + lane/4 (+8), columns = output channels co0 + 8j + 2(lane%4) (+1)
         // dW is [K][3][3][C] fp32
 #pragma unroll

@@ -7,6 +7,10 @@ namespace sm90 {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// Warp index broadcast from lane 0. ptxas cannot prove threadIdx.x / 32 warp-uniform; a warp-role branch on it makes
+// every wgmma behind it a "divergent path", and ptxas then waits for each wgmma before issuing the next (C7520).
+__device__ __forceinline__ int warp_uniform_idx() { return __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0); }
+
 // ------------------------------------------------------------------ mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
