@@ -30,7 +30,7 @@ def install_as_furnace():
     (`from seg_opr.loss_opr import ...`, `from engine.engine import Engine`, `from apex.parallel import ...`)."""
     import importlib
     import sys
-    for name in ("seg_opr", "seg_opr.seg_oprs", "seg_opr.loss_opr", "seg_opr.metric", "base_model", "base_model.resnet", "engine",
+    for name in ("seg_opr", "seg_opr.seg_oprs", "seg_opr.loss_opr", "seg_opr.metric", "base_model", "base_model.resnet", "base_model.xception", "engine",
                  "engine.engine", "engine.lr_policy", "engine.logger", "engine.evaluator", "utils", "utils.init_func", "utils.pyt_utils", "utils.img_utils",
                  "apex", "apex.parallel"):
         sys.modules[name] = importlib.import_module("torchseg_b200." + name)

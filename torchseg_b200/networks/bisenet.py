@@ -134,9 +134,9 @@ class SpatialPath(nn.Module):
 class BiSeNetHead(nn.Module):
     """network.py:140-168"""
 
-    def __init__(self, in_planes, out_planes, scale, is_aux=False, norm_layer=nn.BatchNorm2d):
+    def __init__(self, in_planes, out_planes, scale, is_aux=False, norm_layer=nn.BatchNorm2d, aux_mid=256):
         super(BiSeNetHead, self).__init__()
-        mid = 256 if is_aux else 64
+        mid = aux_mid if is_aux else 64   # aux_mid: 256 in the R18 network, 128 in X39 (X39 network.py:147-152)
         self.conv_3x3 = ConvBnRelu(in_planes, mid, 3, 1, 1, has_bn=True, norm_layer=norm_layer, has_relu=True,
                                    has_bias=False)
         self.conv_1x1 = nn.Conv2d(mid, out_planes, kernel_size=1, stride=1, padding=0)

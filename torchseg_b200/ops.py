@@ -735,6 +735,61 @@ class ConvFn(torch.autograd.Function):
         return dx, dw_view, db, None, None, None, None, None
 
 
+class DWConvFn(torch.autograd.Function):
+    """depthwise 3x3 convolution, padding 1, stride 1 or 2, no bias: the `groups=in_channels` conv of
+    SeparableConvBnRelu (TorchSeg furnace/base_model/xception.py:14-16), on tsb_dwconv_{fprop,dgrad,wgrad}.
+
+    x may carry more logical channels than the conv has (a 64-padded buffer whose channels [C, Cx) are zero): the
+    kernels read its first C channels in place. The output has `ocs` >= C logical channels whose pads are exact zeros,
+    so it can feed the 64-padded pointwise conv that follows without a copy. `share` (ops.GradShare): x has other
+    consumers in the same block and their input gradients are chained through one buffer (dgrad accumulate)."""
+
+    @staticmethod
+    def forward(ctx, x, w, stride, ocs, share=None):
+        C = w.shape[0]
+        assert w.shape[1:] == (1, 3, 3), "depthwise 3x3 weight [C,1,3,3] expected"
+        N, Cx, H, W = x.shape
+        assert Cx >= C
+        P, Q = conv_out_size(H, 3, stride, 1, 1), conv_out_size(W, 3, stride, 1, 1)
+        ocs = C if ocs is None else ocs
+        y = (nhwc_zeros if ocs > C else nhwc_empty)(N, ocs, P, Q, device=x.device)
+        call("tsb_dwconv_fprop", ptr(x), cs_of(x), ptr(w.detach().reshape(C, 9)), ptr(y), cs_of(y), N, H, W, C, stride,
+             stream())
+        ctx.save_for_backward(x, w)
+        ctx.stride, ctx.share = stride, share
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w = ctx.saved_tensors
+        stride, share = ctx.stride, ctx.share
+        C = w.shape[0]
+        N, Cx, H, W = x.shape
+        if dy.dtype != _BF or dy.stride(1) != 1:
+            dy = to_nhwc(dy)
+        w9 = w.detach().reshape(C, 9)
+        direct = _direct_grad(w)
+        if direct:
+            dw_view, dw = None, w.grad
+        else:
+            dw_view = dw = torch.zeros_like(w, memory_format=torch.contiguous_format)
+        call("tsb_dwconv_wgrad", ptr(x), cs_of(x), ptr(dy), cs_of(dy), ptr(dw), N, H, W, C, stride, *det_ws(), stream())
+        dx = None
+        if ctx.needs_input_grad[0]:
+            if share is not None and share.stash is not None:
+                dx = share.stash
+                call("tsb_dwconv_dgrad", ptr(dy), cs_of(dy), ptr(w9), ptr(dx), cs_of(dx), N, H, W, C, stride, 1, stream())
+                dx = share.contribute(dx, accumulated=True)
+            else:
+                dx = (nhwc_zeros if Cx > C else nhwc_empty)(N, Cx, H, W, device=dy.device)
+                call("tsb_dwconv_dgrad", ptr(dy), cs_of(dy), ptr(w9), ptr(dx), cs_of(dx), N, H, W, C, stride, 0, stream())
+                if share is not None:
+                    dx = share.contribute(dx)
+        if direct:
+            _notify(w)
+        return dx, dw_view, None, None, None
+
+
 # --------------------------------------------------------------------------------------------------
 # pooling / resize / attention scale
 # --------------------------------------------------------------------------------------------------

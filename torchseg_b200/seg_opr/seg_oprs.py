@@ -100,8 +100,14 @@ def conv_bn_act(x, conv, bn, relu, residual=None, in_share=None, res_share=None)
         gamma, beta = _pad_vec(gamma, Kp, 1.0), _pad_vec(beta, Kp)
         with torch.no_grad():
             rm, rv = _pad_vec(rm, Kp), _pad_vec(rv, Kp, 1.0)
-    if padded or stem or not bn.training:
+    if stem or not bn.training:
         in_share = res_share = None
+    elif padded:
+        # the padded conv may read a zero-padded copy of x, whose gradient is not x's; the residual is used as it
+        # comes whenever K itself needs no padding (Xception's 16/32-channel pointwise convs into 64/128 channels)
+        in_share = None
+        if Kp != K:
+            res_share = None
     if (not bn.training) and EVAL_FOLD_BN and not padded and not torch.is_grad_enabled():
         # inference (evaluator.py:255-275): w' = w·γ/σ, b' = β − μ·γ/σ, epilogue = + b' (+ shortcut) → ReLU
         wb, bias = ops.fold_cache.get(conv.weight, bn, stem)
