@@ -47,10 +47,6 @@ const char* tsb_last_error(void);
 int tsb_version(void);          /* 10000*major + 100*minor + patch */
 /* number of kernels launched by this library from the calling process since load (all threads) */
 long long tsb_launch_count(void);
-/* debug / A-B switches: key 1 = wgmma descriptor base_offset for row-shifted taps, 2 = allow row tiles,
- * 3 = allow resident weights, 5 = wgrad waves, 6 = OHEM register hoisting, 8 = nine-tap wgrad kernel,
- * 10 = exact-class-count OHEM band kernels */
-int tsb_debug_set(int key, int value);
 
 /* ================================================================================================
  * OHEM cross-entropy — replaces ProbOhemCrossEntropy2d.forward, furnace/seg_opr/loss_opr.py:68-98

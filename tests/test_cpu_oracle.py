@@ -206,6 +206,35 @@ def test_bilinear_oracle_matches_aten():
     assert np.max(np.abs(out - ref.numpy())) < 1e-5
 
 
+@pytest.mark.parametrize("weighted", [False, True], ids=["unweighted", "weighted"])
+def test_ohem_extra_masked_class_changes_nothing(weighted):
+    """An extra class whose low-res logit is -1e4 and that no label names leaves the fused-upsample OHEM bit-identical:
+    its exp flushes to exactly 0 and adding +0 leaves every class-order sum unchanged, so p, T, the kept set, the loss
+    and the gradient of the real classes are the same, and the extra class's gradient is 0. test_gpu_kernels.py relies
+    on this to run the same 19-class input through the generic band kernels (as C = 20)."""
+    from oracle import c_oracle
+    N, C, h, w, s = 2, 19, 12, 16, 8
+    H, W = h * s, w * s
+    g = torch.Generator().manual_seed(31)
+    lo = torch.randn(N, h, w, 32, generator=g) * 3
+    lo[..., C] = -1e4
+    labels = torch.randint(0, C, (N, H, W), generator=g)
+    labels[:, :10] = 255
+    cw = (torch.rand(C + 1, generator=g) + 0.5).numpy() if weighted else None
+    min_kept = N * H * W // 16
+    res = []
+    for c in (C, C + 1):
+        up = c_oracle.bilinear_nhwc_to_nchw(lo.numpy(), c, H, W)
+        res.append(c_oracle.ohem(up, labels.numpy(), 255, 0.7, min_kept, class_weight=None if cw is None else cw[:c],
+                                 want_grad=True))
+    a, b = res
+    assert np.array_equal(a["p"].view(np.uint32), b["p"].view(np.uint32))
+    assert np.array_equal(a["kept"], b["kept"])
+    assert a["T"] == b["T"] and a["active"] == b["active"] and a["loss"] == b["loss"]
+    assert np.array_equal(a["dlogits"].view(np.uint32), np.ascontiguousarray(b["dlogits"][:, :C]).view(np.uint32))
+    assert np.all(b["dlogits"][:, C] == 0)
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # the reference modules' own outputs, stored by tools/make_live_golden.py (tests/golden/live_reference.npz)
 # ---------------------------------------------------------------------------------------------------------------

@@ -215,25 +215,6 @@ def test_conv_full_size_vs_cudnn(cuda, case):
         torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
 
 
-def test_wgrad_taps_matches_row_kernel(cuda):
-    """the nine-tap wgrad kernel (tsb_debug_set key 8) against the row-tile kernel on the same operands, dilation 2"""
-    from torchseg_b200 import ops
-    g = torch.Generator(device="cuda").manual_seed(12)
-    N, C, H, W, K, dil = 4, 128, 60, 60, 192, 2
-    x = ops.to_nhwc(torch.randn(N, C, H, W, device=cuda, generator=g))
-    gy = ops.to_nhwc(torch.randn(N, K, H, W, device=cuda, generator=g))
-    outs = []
-    try:
-        for flag in (1, 0):
-            ops.call("tsb_debug_set", 8, flag)
-            dw = torch.zeros((K, 3, 3, C), dtype=torch.float32, device=cuda)
-            ops.conv_wgrad(x, gy, K, 3, 1, dil, dil, dw)
-            outs.append(dw)
-    finally:
-        ops.call("tsb_debug_set", 8, 1)
-    assert rel_err(outs[0], outs[1]) < 1e-4
-
-
 @pytest.mark.parametrize("HW,R", [((57, 75), 3), ((45, 34), 7)])
 def test_stem_odd_image_size(cuda, HW, R):
     """odd input sizes (BASELINE configs[2] 713, configs[4] 473): the space-to-depth pack pads one zero row / column, which

@@ -16,6 +16,8 @@ pytestmark = pytest.mark.gpu
 EXTRA = [
     (1, 64, 8, 128, 64, 3, 1, 1, 1),     # 8 row tiles: one tile per CTA
     (3, 64, 132, 128, 64, 3, 1, 1, 1),   # 396 row tiles over 132 CTAs: three (odd) tiles per CTA
+    (4, 128, 60, 60, 192, 3, 1, 2, 2),   # dilated 3x3, Q = 60: the nine-tap wgrad kernel
+    (2, 64, 8, 8, 64, 3, 1, 2, 2),       # dilated 3x3, Q = 8: too narrow for the nine-tap and row kernels, generic wgrad
 ]
 
 

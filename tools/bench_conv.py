@@ -5,7 +5,7 @@ D = dgrad; W = wgrad). CUDA events around single launches, L2 flushed before eac
 Prints µs and TF/s per (shape, pass) and the step-weighted total, comparable with bench.py's
 roofline.kernel_ms_per_step. With --out DIR the table is also written to DIR/bench_conv.json.
 
-Usage: python tools/bench_conv.py [--out DIR] [key=value ...]   (key=value: tsb_debug_set switches)
+Usage: python tools/bench_conv.py [--out DIR]
 """
 import json
 import os
@@ -13,7 +13,7 @@ import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
-from torchseg_b200 import ops, _lib
+from torchseg_b200 import ops
 
 N = 16
 # (name, C, H, W, K, R, stride, pad, count in the step, passes, BN statistics in the forward)
@@ -131,8 +131,6 @@ def main():
     out_dir = None
     if "--out" in args:
         out_dir = args[args.index("--out") + 1]
-    for k, v in [a.split("=") for a in args if "=" in a]:
-        _lib.call("tsb_debug_set", int(k), int(v))
     rows = []
     fl, t = stem_pair()
     rows.append(("stem pair 7x7/2 3->2x64 @1024", 1, fl, t))

@@ -28,7 +28,6 @@ D = c_double
 
 # name -> argtypes (the trailing stream argument is included)
 _SIGS = {
-    "tsb_debug_set": [I, I],
     "tsb_ohem_begin": [P, P],
     "tsb_ohem_ptarget": [P, I, L, L, L, L, P, I, I, I, I, I, F, P, P, P, P],
     "tsb_ohem_ptarget_up": [P, I, I, I, P, I, I, I, I, I, F, P, P, P, P],
@@ -109,10 +108,6 @@ def lib():
         h.tsb_p2p_buffer_bytes.argtypes = [I, I, I]
         h.tsb_edge_labels_workspace_bytes.restype = c_size_t
         h.tsb_edge_labels_workspace_bytes.argtypes = [I, I, I]
-        # developer A/B switches (include/tsb.h tsb_debug_set): TSB_DEBUG_SET="6=0,5=2"
-        for kv in filter(None, os.environ.get("TSB_DEBUG_SET", "").split(",")):
-            k, v = kv.split("=")
-            h.tsb_debug_set(int(k), int(v))
         _lib = h
     return _lib
 

@@ -94,21 +94,82 @@ static inline void pick_tile(int Q, int npx, int* TW, int* TH) {
 
 // A-operand maps over an NHWC bf16 tensor [N,H,W,Cs] (channel count Cc, channel stride cs), for a conv of
 // stride `st`: st==1 → 1 map; st==2 → 4 parity views (ph,pw) of dims ceil((H-ph)/2) x ceil((W-pw)/2).
-static inline int encode_act_maps(CUtensorMap* maps, const void* base, int N, int H, int W, int Cc, int cs, int st, int TW, int TH) {
+// Map m loads boxes of 64 channels x box_w[m] pixels x TH rows.
+static inline int encode_act_maps(CUtensorMap* maps, const void* base, int N, int H, int W, int Cc, int cs, int st,
+                                  const int box_w[4], int TH) {
     const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(base);
     if (st == 1) {
-        return encode_4d(&maps[0], b, Cc, W, H, N, (uint64_t)cs * 2, (uint64_t)W * cs * 2, (uint64_t)H * W * cs * 2, 64, TW,
-                         TH, 1);
+        return encode_4d(&maps[0], b, Cc, W, H, N, (uint64_t)cs * 2, (uint64_t)W * cs * 2, (uint64_t)H * W * cs * 2, 64,
+                         box_w[0], TH, 1);
     }
     for (int ph = 0; ph < 2; ++ph)
         for (int pw = 0; pw < 2; ++pw) {
             int Hh = (H - ph + 1) / 2, Ww = (W - pw + 1) / 2;
             if (Hh <= 0 || Ww <= 0) { Hh = Hh > 0 ? Hh : 1; Ww = Ww > 0 ? Ww : 1; }
             int rc = encode_4d(&maps[ph * 2 + pw], b + ((long long)ph * W + pw) * cs, Cc, Ww, Hh, N, (uint64_t)2 * cs * 2,
-                               (uint64_t)2 * W * cs * 2, (uint64_t)H * W * cs * 2, 64, TW, TH, 1);
+                               (uint64_t)2 * W * cs * 2, (uint64_t)H * W * cs * 2, 64, box_w[ph * 2 + pw], TH, 1);
             if (rc) return rc;
         }
     return TSB_OK;
+}
+
+// Overlapped-window view of the 7x7/2 stem's s2d image: coordinate (e, ow, oh, n) → xs2d[n][oh][ow .. ow+3][0..15]
+static inline int encode_stem_map(CUtensorMap* m, const void* xs2d, int N, int H2, int W2, int box_w, int TH) {
+    const uint64_t row = (uint64_t)(W2 + 4) * 16 * 2;
+    return encode_4d(m, xs2d, 64, (uint64_t)W2, (uint64_t)H2, (uint64_t)N, 32, row, row * H2, 64, box_w, TH, 1);
+}
+
+// Forward taps of a conv in (r, s) order: the box origin relative to the output-tile origin, in the coordinates of the
+// tap's map (a stride-2 parity view), and the tap's K offset in the packed [K][R][S][C] weights. Returns the count.
+static inline int forward_taps(const tsb_conv_shape* s, Tap* taps) {
+    int nt = 0;
+    for (int r = 0; r < s->R; ++r)
+        for (int ss = 0; ss < s->S; ++ss) {
+            Tap& T = taps[nt++];
+            int th = r * s->dil - s->pad, tw = ss * s->dil - s->pad;
+            if (s->stride == 1) { T.dh = th; T.dw = tw; T.map = 0; }
+            else {
+                int ph = posmod(th, 2), pw = posmod(tw, 2);
+                T.dh = (th - ph) / 2; T.dw = (tw - pw) / 2; T.map = ph * 2 + pw;
+            }
+            T.bk = (r * s->S + ss) * s->C;
+        }
+    return nt;
+}
+
+// How a weight-gradient launch splits its pixel tiles over CTAs (blockIdx.x). Every split stores a dW-shaped slice into
+// the workspace and finish_splits adds the slices in split order; one split adds into dW in place, as does a workspace
+// too small for two slices. The split count sets the fp32 summation order, so each kernel keeps its own policy for
+// `want`, the split count it asks for.
+struct SplitPlan {
+    int tiles_per_split, splits;
+    int add;                 // one split: the kernel adds into dW
+    float* dst;              // dW (add) or the workspace slices
+    long long part_stride;   // elements between the slices of consecutive splits (0 when add)
+    long long n_dw;          // elements of dW
+};
+static inline SplitPlan plan_splits(int want, int total_tiles, long long n_dw, float* dw, float* ws, long long ws_floats) {
+    const long long fit = ws ? ws_floats / n_dw : 0;
+    if (want > fit) want = (int)fit;
+    if (want < 1) want = 1;
+    SplitPlan sp;
+    sp.tiles_per_split = (total_tiles + want - 1) / want;
+    sp.splits = (total_tiles + sp.tiles_per_split - 1) / sp.tiles_per_split;
+    sp.add = sp.splits == 1;
+    sp.dst = sp.add ? dw : ws;
+    sp.part_stride = sp.add ? 0 : n_dw;
+    sp.n_dw = n_dw;
+    return sp;
+}
+static inline int finish_splits(const SplitPlan& sp, float* dw, cudaStream_t st) {
+    return sp.add ? TSB_OK : tsb_det_reduce(dw, sp.dst, sp.splits, sp.n_dw, sp.n_dw, st);
+}
+// Split count for about kWgradWaves waves of `ctas_per_split` CTAs, keeping at least `min_tiles` tiles per split.
+constexpr int kWgradWaves = 2;
+static inline int wave_splits(int ctas_per_split, int total_tiles, int min_tiles) {
+    const int want = (kWgradWaves * tsb_num_sms() + ctas_per_split - 1) / ctas_per_split;
+    const int max_splits = (total_tiles + min_tiles - 1) / min_tiles;
+    return want < max_splits ? want : max_splits;
 }
 
 

@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __gr
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kWgBarOff);
-    uint64_t* empty_bar = full_bar + kWgStages;
+    StageRing ring(full_bar, full_bar + kWgStages, kWgStages);
 
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31;
     const int split = blockIdx.x;
@@ -63,7 +63,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __gr
     if (warp == kProducer && lane == 0) {
         tma_prefetch_desc(&p.mapA);
         tma_prefetch_desc(&p.mapB[0]);
-        for (int s = 0; s < kWgStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kWgConsumers * 4); }
+        ring.init(kWgConsumers * 4);
         fence_barrier_init();
     }
     __syncthreads();
@@ -71,25 +71,24 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __gr
     if (warp == kProducer) {
         if (lane == 0) {
             for (int it = 0; it < total_iters; ++it) {
-                const int s = it % kWgStages;
-                const uint32_t ph = (uint32_t)(it / kWgStages) & 1u;
-                mbar_wait(&empty_bar[s], ph ^ 1u);
+                ring.acquire();
                 const int t = t_begin + it;
                 const int tw_i = t % p.tiles_w;
                 const int th_i = (t / p.tiles_w) % p.tiles_h;
                 const int n_img = t / (p.tiles_w * p.tiles_h);
                 const int q0 = tw_i * p.TW, p0 = th_i * p.TH;
-                uint8_t* a_s = smem + s * kWgStageBytes;
+                uint8_t* a_s = smem + ring.slot * kWgStageBytes;
                 uint8_t* b_s = a_s + 2 * kWgBoxBytes;
-                mbar_arrive_expect_tx(&full_bar[s], (uint32_t)((2 + nb) * kWgBoxBytes));
-                tma_load_4d(a_s, &p.mapA, &full_bar[s], co0, q0, p0, n_img);
-                tma_load_4d(a_s + kWgBoxBytes, &p.mapA, &full_bar[s], co0 + 64, q0, p0, n_img);  // OOB → zeros
+                mbar_arrive_expect_tx(ring.full_bar(), (uint32_t)((2 + nb) * kWgBoxBytes));
+                tma_load_4d(a_s, &p.mapA, ring.full_bar(), co0, q0, p0, n_img);
+                tma_load_4d(a_s + kWgBoxBytes, &p.mapA, ring.full_bar(), co0 + 64, q0, p0, n_img);  // OOB → zeros
                 for (int j = 0; j < nb; ++j) {
                     const int b = box0 + j;
                     const int tap = b / p.cchunks, cc = b - tap * p.cchunks;
                     const Tap T = p.taps[tap];
-                    tma_load_4d(b_s + j * kWgBoxBytes, &p.mapB[T.map], &full_bar[s], cc * 64, q0 + T.dw, p0 + T.dh, n_img);
+                    tma_load_4d(b_s + j * kWgBoxBytes, &p.mapB[T.map], ring.full_bar(), cc * 64, q0 + T.dw, p0 + T.dh, n_img);
                 }
+                ring.advance();
             }
         }
     } else {   // every split stores its (possibly all-zero) tile: the slices are summed in split order afterwards
@@ -105,37 +104,24 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __gr
             for (int q = 0; q < 32; ++q) acc[j][q] = 0.f;
 #pragma unroll
         for (int j = 0; j < 4; ++j) fence_operands(acc[j]);
-        // a stage is released one stage late: wait_group<1> after issuing stage s retires the MMAs of stage s-1, so the
-        // tensor pipe never drains between stages
-        int s = 0, prev = -1;
-        uint32_t ph = 0;
         for (int it = 0; it < total_iters; ++it) {
-            mbar_wait(&full_bar[s], ph);
-            wgmma_fence();
-            const uint32_t a_lo = base_lo + (uint32_t)(s * (kWgStageBytes >> 4)) + (uint32_t)c * (kWgBoxBytes >> 4);
-            const uint32_t b_lo = base_lo + (uint32_t)(s * (kWgStageBytes >> 4)) + ((2 * kWgBoxBytes) >> 4);
+            ring.wait_full();
+            const uint32_t a_lo = base_lo + (uint32_t)(ring.slot * (kWgStageBytes >> 4)) + (uint32_t)c * (kWgBoxBytes >> 4);
+            const uint32_t b_lo = base_lo + (uint32_t)(ring.slot * (kWgStageBytes >> 4)) + ((2 * kWgBoxBytes) >> 4);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 if (j < nb) {
 #pragma unroll
                     for (int k = 0; k < 4; ++k)
-                        wgmma_m64n64<1, 1>(acc[j], desc_at(desc_hi, a_lo + 128 * k, 0),
-                                           desc_at(desc_hi, b_lo + (uint32_t)j * (kWgBoxBytes >> 4) + 128 * k, 0), 1u);
+                        wgmma_m64n64<1, 1>(acc[j], desc_at(desc_hi, a_lo + 128 * k),
+                                           desc_at(desc_hi, b_lo + (uint32_t)j * (kWgBoxBytes >> 4) + 128 * k), 1u);
                 }
             }
-            wgmma_commit();
-            if (prev >= 0) {
-                wgmma_wait<1>();
-                // wait_group covers only this warp's MMAs: every consumer warp releases the stage
-                if (lane == 0) mbar_arrive(&empty_bar[prev]);
-            }
-            prev = s;
-            if (++s == kWgStages) { s = 0; ph ^= 1u; }
+            ring.commit_release_prev();
         }
-        wgmma_wait<0>();
+        ring.drain();
 #pragma unroll
         for (int j = 0; j < 4; ++j) fence_operands(acc[j]);
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int co = co0 + c * 64 + wq * 16 + (lane >> 2) + 8 * h;
@@ -188,18 +174,7 @@ static int fprop_impl(const tsb_conv_shape* s, const void* x, int xcs, const voi
     }
     convv2::Desc d;
     memset(&d, 0, sizeof(d));
-    int nt = 0;
-    for (int r = 0; r < s->R; ++r)
-        for (int ss = 0; ss < s->S; ++ss) {
-            Tap& T = d.taps[nt++];
-            int th = r * s->dil - s->pad, tw = ss * s->dil - s->pad;
-            if (s->stride == 1) { T.dh = th; T.dw = tw; T.map = 0; }
-            else {
-                int ph = posmod(th, 2), pw = posmod(tw, 2);
-                T.dh = (th - ph) / 2; T.dw = (tw - pw) / 2; T.map = ph * 2 + pw;
-            }
-            T.bk = (r * s->S + ss) * s->C;
-        }
+    const int nt = forward_taps(s, d.taps);
     int kst = (s->K + 7) / 8 * 8;
     if (kst > ycs) kst = ycs;
     d.act = x; d.aN = N; d.aH = H; d.aW = W; d.aC = s->C; d.acs = xcs; d.act_stride = s->stride; d.flat = flat;
@@ -300,6 +275,7 @@ int pick_nb(int nboxes) {
     if (nboxes % 2 == 0) return 2;
     return 1;
 }
+// the generic kernel; prm comes with its maps, taps, tiling, K, C, dw_row_stride, and dw = dW
 int wgrad_common(WgParams& prm, int N, int P, int Q, int K, float* ws, long long ws_floats, cudaStream_t st) {
     prm.tiles_w = (Q + prm.TW - 1) / prm.TW;
     prm.tiles_h = (P + prm.TH - 1) / prm.TH;
@@ -308,21 +284,14 @@ int wgrad_common(WgParams& prm, int N, int P, int Q, int K, float* ws, long long
     prm.nb = pick_nb(prm.nboxes);
     const int groups = prm.nboxes / prm.nb;
     const int co_tiles = (K + 127) / 128;
-    // split the pixel range so the grid covers ~2 waves of SMs, at least 8 tiles per CTA
-    int base = groups * co_tiles;
-    int want = (convv2::g_wgrad_waves * tsb_num_sms() + base - 1) / base;
-    int max_splits = (prm.total_tiles + 7) / 8;
-    if (want > max_splits) want = max_splits;
-    const long long n_dw = (long long)K * prm.dw_row_stride;
-    if (want > (ws ? ws_floats / n_dw : 0)) want = (int)(ws ? ws_floats / n_dw : 0);
-    if (want < 1) want = 1;
-    prm.tiles_per_split = (prm.total_tiles + want - 1) / want;
-    int splits = (prm.total_tiles + prm.tiles_per_split - 1) / prm.tiles_per_split;
+    // about two waves of CTAs, at least 8 tiles per split
     float* dw = prm.dw;
-    prm.add = splits == 1;
-    if (!prm.add) { prm.dw = ws; prm.part_stride = n_dw; }
-    int rc = launch_wg(prm, splits, co_tiles, groups, st);
-    return (rc || prm.add) ? rc : tsb_det_reduce(dw, prm.dw, splits, n_dw, n_dw, st);
+    const SplitPlan sp = plan_splits(wave_splits(groups * co_tiles, prm.total_tiles, 8), prm.total_tiles,
+                                     (long long)K * prm.dw_row_stride, dw, ws, ws_floats);
+    prm.tiles_per_split = sp.tiles_per_split;
+    prm.add = sp.add; prm.dw = sp.dst; prm.part_stride = sp.part_stride;
+    int rc = launch_wg(prm, sp.splits, co_tiles, groups, st);
+    return rc ? rc : finish_splits(sp, dw, st);
 }
 }  // namespace
 
@@ -335,8 +304,6 @@ extern "C" int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs,
     TSB_REQUIRE(xcs % 8 == 0 && dycs % 8 == 0 && dycs >= s->K && tsb_aligned16(x) && tsb_aligned16(dy) && tsb_aligned16(dw),
                 "tsb_conv2d_wgrad: alignment");
     cudaStream_t st = (cudaStream_t)stream;
-    WgParams prm;
-    memset(&prm, 0, sizeof(prm));
     int N = s->N, H = s->H, W = s->W, P = s->P, Q = s->Q;
     const bool flat = (s->R == 1 && s->stride == 1 && s->pad == 0);
     if (flat) {
@@ -344,56 +311,40 @@ extern "C" int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs,
         TSB_REQUIRE(npix < (1ll << 31), "tsb_conv2d_wgrad: too many pixels");
         W = (int)npix; H = 1; N = 1; P = 1; Q = W;
     }
-    int TW, TH;
-    if (flat) { TW = 64; TH = 1; } else pick_tile(Q, 64, &TW, &TH);
-    prm.TW = TW; prm.TH = TH; prm.tw_shift = ilog2(TW);
-    rc = encode_4d(&prm.mapA, dy, s->K, Q, P, N, (uint64_t)dycs * 2, (uint64_t)Q * dycs * 2, (uint64_t)P * Q * dycs * 2, 64, TW, TH, 1);
-    if (rc) return rc;
-    rc = encode_act_maps(prm.mapB, x, N, H, W, s->C, xcs, s->stride, TW, TH);
-    if (rc) return rc;
-    int nt = 0;
-    for (int r = 0; r < s->R; ++r)
-        for (int ss = 0; ss < s->S; ++ss) {
-            Tap& T = prm.taps[nt++];
-            int th = r * s->dil - s->pad, tw = ss * s->dil - s->pad;
-            if (s->stride == 1) { T.dh = th; T.dw = tw; T.map = 0; }
-            else {
-                int ph = posmod(th, 2), pw = posmod(tw, 2);
-                T.dh = (th - ph) / 2; T.dw = (tw - pw) / 2; T.map = ph * 2 + pw;
-            }
-            T.bk = 0;
-        }
-    prm.ntaps = nt;
-    prm.cchunks = s->C / 64;
-    prm.K = s->K;
-    prm.C = s->C;
-    prm.dw_row_stride = (long long)s->R * s->S * s->C;
-    prm.dw = dw;
+    const long long dw_row_stride = (long long)s->R * s->S * s->C;
     if (!flat && s->R > 1) {
         convv2::WgradDesc d;
         memset(&d, 0, sizeof(d));
         d.x = x; d.dy = dy; d.N = N; d.H = H; d.W = W; d.C = s->C; d.xcs = xcs; d.P = P; d.Q = Q; d.K = s->K; d.dycs = dycs;
         d.stride = s->stride;
-        for (int t = 0; t < nt; ++t) d.taps[t] = prm.taps[t];
-        d.ntaps = nt; d.dw_row_stride = prm.dw_row_stride; d.dw = dw;
+        d.ntaps = forward_taps(s, d.taps);
+        d.dw_row_stride = dw_row_stride; d.dw = dw;
         d.ws = ws; d.ws_floats = ws_floats;
         rc = convv2::launch_wgrad_taps(d, s->R, s->pad, s->dil, st);   // 3x3 stride 1: all nine taps in one CTA
         if (rc != TSB_ERR_UNSUPPORTED) return rc;
         rc = convv2::launch_wgrad_rows(d, st);
         if (rc != TSB_ERR_UNSUPPORTED) return rc;
     }
+    WgParams prm;
+    memset(&prm, 0, sizeof(prm));
+    int TW, TH;
+    if (flat) { TW = 64; TH = 1; } else pick_tile(Q, 64, &TW, &TH);
+    prm.TW = TW; prm.TH = TH; prm.tw_shift = ilog2(TW);
+    rc = encode_4d(&prm.mapA, dy, s->K, Q, P, N, (uint64_t)dycs * 2, (uint64_t)Q * dycs * 2, (uint64_t)P * Q * dycs * 2, 64, TW, TH, 1);
+    if (rc) return rc;
+    const int box_w[4] = {TW, TW, TW, TW};
+    rc = encode_act_maps(prm.mapB, x, N, H, W, s->C, xcs, s->stride, box_w, TH);
+    if (rc) return rc;
+    prm.ntaps = forward_taps(s, prm.taps);
+    prm.cchunks = s->C / 64;
+    prm.K = s->K;
+    prm.C = s->C;
+    prm.dw_row_stride = dw_row_stride;
+    prm.dw = dw;
     return wgrad_common(prm, N, P, Q, s->K, ws, ws_floats, st);
 }
 
 // ---------------------------------------------------------------------------------- 7x7/2 stem
-namespace {
-// overlapped-window view of the s2d image: coordinate (e, ow, oh, n) → xs2d[n][oh][ow .. ow+3][0..15]
-int encode_stem_map(CUtensorMap* m, const void* xs2d, int N, int H2, int W2, int TW, int TH) {
-    const uint64_t row = (uint64_t)(W2 + 4) * 16 * 2;
-    return encode_4d(m, xs2d, 64, (uint64_t)W2, (uint64_t)H2, (uint64_t)N, 32, row, row * H2, 64, TW, TH, 1);
-}
-}  // namespace
-
 static int stem_fprop_impl(const void* xs2d, int N, int H, int W, const void* wp, int K, void* y, int ycs, float* sum,
                            float* sumsq, float* ws, long long ws_floats, const float* bias, int relu, tsb_stream_t stream) {
     TSB_REQUIRE(xs2d && wp && y && N > 0 && H > 0 && W > 0 && K > 0, "tsb_conv_stem_fprop: bad args");

@@ -49,7 +49,7 @@ struct alignas(64) V2Params {
     float* part;   // [gridDim.x][2][k_real] per-CTA statistics, summed in CTA order by tsb_det_reduce
     void* out;
     // shared-memory plan
-    int nstages, stage_bytes, res_bytes, use_base_offset;
+    int nstages, stage_bytes, res_bytes;
 };
 
 template <int BN>
@@ -66,9 +66,9 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
     uint8_t* stages = smem + p.res_bytes;        // ring of A (+B) stages
     uint8_t* tail = stages + p.nstages * p.stage_bytes;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
-    uint64_t* empty_bar = full_bar + kMaxStages;
-    uint64_t* b_ready = empty_bar + kMaxStages;
+    uint64_t* b_ready = full_bar + 2 * kMaxStages;
     float* s_stats = reinterpret_cast<float*>(tail + 256);  // [consumer warp][2*BN]
+    StageRing ring(full_bar, full_bar + kMaxStages, p.nstages);
 
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31;
     const int n0 = blockIdx.y * BN;
@@ -79,7 +79,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
     if (warp == kProducer && lane == 0) {
         tma_prefetch_desc(&p.mapB);
         tma_prefetch_desc(&p.mapA[0]);
-        for (int s = 0; s < p.nstages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumers * 4); }
+        ring.init(kConsumers * 4);
         mbar_init(b_ready, 1);
         fence_barrier_init();
     }
@@ -95,8 +95,6 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
                             tma_load_2d(res_b + (p.groups[g].tap_idx[t] * p.kchunks + kc) * kBTile, &p.mapB, b_ready,
                                         p.groups[g].bk[t] + kc * 64, n0);
             }
-            int sl = 0;
-            uint32_t ph = 0;
             for (int i = 0; i < my_tiles; ++i) {
                 const int tile = blockIdx.x + i * gridDim.x;
                 const int tw_i = tile % p.tiles_w;
@@ -108,15 +106,15 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
                     const int cw = q0 + p.groups[g].dw0, chh = p0 + p.groups[g].dh;
                     const uint32_t bytes = (uint32_t)p.a_bytes[gmap] + (RES ? 0u : (uint32_t)(ntaps * kBTile));
                     for (int kc = 0; kc < p.kchunks; ++kc) {
-                        mbar_wait(&empty_bar[sl], ph ^ 1u);
-                        uint8_t* a_s = stages + sl * p.stage_bytes;
-                        mbar_arrive_expect_tx(&full_bar[sl], bytes);
-                        tma_load_4d(a_s, &p.mapA[gmap], &full_bar[sl], kc * 64, cw, chh, n_img);
+                        ring.acquire();
+                        uint8_t* a_s = stages + ring.slot * p.stage_bytes;
+                        mbar_arrive_expect_tx(ring.full_bar(), bytes);
+                        tma_load_4d(a_s, &p.mapA[gmap], ring.full_bar(), kc * 64, cw, chh, n_img);
                         if (!RES) {
                             for (int t = 0; t < ntaps; ++t)
-                                tma_load_2d(a_s + kAStageBytes + t * kBTile, &p.mapB, &full_bar[sl], p.groups[g].bk[t] + kc * 64, n0);
+                                tma_load_2d(a_s + kAStageBytes + t * kBTile, &p.mapB, ring.full_bar(), p.groups[g].bk[t] + kc * 64, n0);
                         }
-                        if (++sl == p.nstages) { sl = 0; ph ^= 1u; }
+                        ring.advance();
                     }
                 }
             }
@@ -134,44 +132,32 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
 #pragma unroll
         for (int q = 0; q < BN / 4; ++q) { run1[q] = 0.f; run2[q] = 0.f; }
         if (RES && my_tiles > 0) mbar_wait(b_ready, 0);
-        int sl = 0;
-        uint32_t ph = 0;
-        for (int i = 0; i < my_tiles; ++i) {
+        for (int i = 0; i < my_tiles; ++i) {   // the ring's slot and phase run on across tiles; each tile drains
             float acc[BN / 2];
 #pragma unroll
             for (int q = 0; q < BN / 2; ++q) acc[q] = 0.f;
             fence_operands(acc);
-            // a stage is released one stage late: wait_group<1> after issuing stage s retires the MMAs of stage s-1, so
-            // the tensor pipe never drains between stages of a tile (wait_group covers only this warp's MMAs: every
-            // consumer warp releases the stage)
-            int prev = -1;
             for (int g = 0; g < p.ngroups; ++g) {
                 const int ntaps = p.groups[g].ntaps;
                 for (int kc = 0; kc < p.kchunks; ++kc) {
-                    mbar_wait(&full_bar[sl], ph);
-                    wgmma_fence();
-                    const uint32_t st_lo = stages_lo + (uint32_t)(sl * p.stage_bytes >> 4);
+                    ring.wait_full();
+                    const uint32_t st_lo = stages_lo + (uint32_t)(ring.slot * p.stage_bytes >> 4);
+                    // a group has at most 3 taps: unrolled by 2, the issue code holds 12 HGMMA (by default ptxas unrolls
+                    // the streamed-weights variant by 4)
+#pragma unroll 2
                     for (int t = 0; t < ntaps; ++t) {
                         const uint32_t a_lo = st_lo + (uint32_t)c * 512u + (uint32_t)p.groups[g].row_off[t] * 8u;
                         const uint32_t b_lo = RES ? res_lo + (uint32_t)((p.groups[g].tap_idx[t] * p.kchunks + kc) * kBTile >> 4)
                                                   : st_lo + (uint32_t)((kAStageBytes + t * kBTile) >> 4);
 #pragma unroll
                         for (int k = 0; k < 4; ++k)   // 16 bf16 = 32 B = 2 descriptor units inside the swizzle atom
-                            wgmma_kmajor<BN>(acc, desc_at(desc_hi, a_lo + 2 * k, p.use_base_offset),
-                                             desc_at(desc_hi, b_lo + 2 * k, 0));
+                            wgmma_kmajor<BN>(acc, desc_at(desc_hi, a_lo + 2 * k), desc_at(desc_hi, b_lo + 2 * k));
                     }
-                    wgmma_commit();
-                    if (prev >= 0) {
-                        wgmma_wait<1>();
-                        if (lane == 0) mbar_arrive(&empty_bar[prev]);
-                    }
-                    prev = sl;
-                    if (++sl == p.nstages) { sl = 0; ph ^= 1u; }
+                    ring.commit_release_prev();
                 }
             }
-            wgmma_wait<0>();
+            ring.drain();
             fence_operands(acc);
-            if (lane == 0) mbar_arrive(&empty_bar[prev]);
             const int tile = blockIdx.x + i * gridDim.x;
             const int tw_i = tile % p.tiles_w;
             const int th_i = (tile / p.tiles_w) % p.tiles_h;
@@ -283,14 +269,13 @@ struct alignas(64) WrParams {
     float* dw;                // dW-shaped slice per split (workspace), part_stride apart; or dW itself when `add`
     long long part_stride;
     int add;                  // one split: add in place
-    int use_base_offset;
 };
 
 __global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_constant__ WrParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kWrStages * kWrStageBytes);
-    uint64_t* empty_bar = full_bar + kWrStages;
+    StageRing ring(full_bar, full_bar + kWrStages, kWrStages);
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31;
     const int co0 = blockIdx.y * 128;
     const int g = blockIdx.z / p.cchunks, cc = blockIdx.z - g * p.cchunks;
@@ -303,7 +288,7 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_co
     if (warp == kProducer && lane == 0) {
         tma_prefetch_desc(&p.mapA);
         tma_prefetch_desc(&p.mapB[G.map]);
-        for (int s = 0; s < kWrStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumers * 4); }
+        ring.init(kConsumers * 4);
         fence_barrier_init();
     }
     __syncthreads();
@@ -311,19 +296,18 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_co
     if (warp == kProducer) {
         if (lane == 0) {
             for (int it = 0; it < total_iters; ++it) {
-                const int s = it % kWrStages;
-                const uint32_t ph = (uint32_t)(it / kWrStages) & 1u;
-                mbar_wait(&empty_bar[s], ph ^ 1u);
+                ring.acquire();
                 const int t = t_begin + it;
                 const int tw_i = t % p.tiles_w;
                 const int row = (t / p.tiles_w) % p.tiles_h;
                 const int n_img = t / (p.tiles_w * p.tiles_h);
                 const int q0 = tw_i * p.TW;
-                uint8_t* a_s = smem + s * kWrStageBytes;
-                mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(kWrABytes + p.b_bytes[G.map]));
-                tma_load_4d(a_s, &p.mapA, &full_bar[s], co0, q0, row, n_img);
-                tma_load_4d(a_s + 64 * 128, &p.mapA, &full_bar[s], co0 + 64, q0, row, n_img);  // OOB → zeros
-                tma_load_4d(a_s + kWrABytes, &p.mapB[G.map], &full_bar[s], cc * 64, q0 + G.dw0, row + G.dh, n_img);
+                uint8_t* a_s = smem + ring.slot * kWrStageBytes;
+                mbar_arrive_expect_tx(ring.full_bar(), (uint32_t)(kWrABytes + p.b_bytes[G.map]));
+                tma_load_4d(a_s, &p.mapA, ring.full_bar(), co0, q0, row, n_img);
+                tma_load_4d(a_s + 64 * 128, &p.mapA, ring.full_bar(), co0 + 64, q0, row, n_img);  // OOB → zeros
+                tma_load_4d(a_s + kWrABytes, &p.mapB[G.map], ring.full_bar(), cc * 64, q0 + G.dw0, row + G.dh, n_img);
+                ring.advance();
             }
         }
     } else {   // every split stores its (possibly all-zero) tile: the slices are summed in split order afterwards
@@ -337,35 +321,24 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_co
             for (int q = 0; q < 32; ++q) acc[t][q] = 0.f;
 #pragma unroll
         for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
-        // a stage is released one stage late (wait_group<1> retires the previous stage's MMAs), as in igemm_v2_kernel
-        int s = 0, prev = -1;
-        uint32_t ph = 0;
         for (int it = 0; it < total_iters; ++it) {
-            mbar_wait(&full_bar[s], ph);
-            wgmma_fence();
-            const uint32_t a_lo = base_lo + (uint32_t)(s * (kWrStageBytes >> 4)) + (uint32_t)c * 512u;
-            const uint32_t b_lo = base_lo + (uint32_t)(s * (kWrStageBytes >> 4)) + (kWrABytes >> 4);
+            ring.wait_full();
+            const uint32_t a_lo = base_lo + (uint32_t)(ring.slot * (kWrStageBytes >> 4)) + (uint32_t)c * 512u;
+            const uint32_t b_lo = base_lo + (uint32_t)(ring.slot * (kWrStageBytes >> 4)) + (kWrABytes >> 4);
 #pragma unroll
             for (int t = 0; t < 3; ++t) {
                 if (t < G.ntaps) {
 #pragma unroll
                     for (int k = 0; k < 4; ++k)   // one MMA consumes 16 pixels = 2048 B = 128 descriptor units
-                        wgmma_m64n64<1, 1>(acc[t], desc_at(desc_hi, a_lo + 128 * k, 0),
-                                           desc_at(desc_hi, b_lo + (uint32_t)(t * G.step * 8) + 128 * k, p.use_base_offset), 1u);
+                        wgmma_m64n64<1, 1>(acc[t], desc_at(desc_hi, a_lo + 128 * k),
+                                           desc_at(desc_hi, b_lo + (uint32_t)(t * G.step * 8) + 128 * k), 1u);
                 }
             }
-            wgmma_commit();
-            if (prev >= 0) {
-                wgmma_wait<1>();
-                if (lane == 0) mbar_arrive(&empty_bar[prev]);
-            }
-            prev = s;
-            if (++s == kWrStages) { s = 0; ph ^= 1u; }
+            ring.commit_release_prev();
         }
-        wgmma_wait<0>();
+        ring.drain();
 #pragma unroll
         for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int co = co0 + c * 64 + wq * 16 + (lane >> 2) + 8 * h;
@@ -382,9 +355,6 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_co
     }
 }
 
-int g_allow_rows = 1;
-int g_allow_resident = 1;
-
 template <int BN, bool RES>
 int launch_v2(const V2Params& prm, int grid_x, int n_tiles, size_t smem, cudaStream_t st) {
     { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(igemm_v2_kernel<BN, RES>), smem); if (rc_) return rc_; }
@@ -395,24 +365,7 @@ int launch_v2(const V2Params& prm, int grid_x, int n_tiles, size_t smem, cudaStr
 
 }  // namespace
 
-extern int g_tsb_ohem_hoist;
-extern int g_tsb_ohem_exact;
-extern "C" int tsb_debug_set(int key, int value) {
-    if (key == 1) convv2::g_use_base_offset = value;
-    else if (key == 2) g_allow_rows = value;
-    else if (key == 3) g_allow_resident = value;
-    else if (key == 5) convv2::g_wgrad_waves = value;
-    else if (key == 6) g_tsb_ohem_hoist = value;
-    else if (key == 8) convv2::g_allow_taps = value;
-    else if (key == 10) g_tsb_ohem_exact = value;
-    else return TSB_ERR_ARG;
-    return TSB_OK;
-}
-
 namespace convv2 {
-
-int g_wgrad_waves = 2;
-int g_use_base_offset = 0;  // H100 takes the 128B-swizzle phase from the absolute shared address: row-shifted starts need no base_offset
 
 int launch(const Desc& d, cudaStream_t st) {
     V2Params prm;
@@ -421,7 +374,7 @@ int launch(const Desc& d, cudaStream_t st) {
     const int n_tiles = (d.ncols + BN - 1) / BN;
     // ---- spatial tiling: row tiles when the output rows are long enough
     int TW, TH;
-    const bool rows = g_allow_rows && !d.flat && d.Ql >= 96;
+    const bool rows = !d.flat && d.Ql >= 96;
     if (d.flat || rows) { TW = 128; TH = 1; }
     else pick_tile(d.Ql, 128, &TW, &TH);
     // ---- group the taps: same (map, dh) → one box, taps addressed by a row offset (row tiles only)
@@ -453,36 +406,18 @@ int launch(const Desc& d, cudaStream_t st) {
     for (int g = 0; g < ng; ++g)
         for (int k = 0; k < prm.groups[g].ntaps; ++k)
             if (prm.groups[g].row_off[k] > span_map[prm.groups[g].map]) span_map[prm.groups[g].map] = prm.groups[g].row_off[k];
+    int box_w[4];   // A box width of each map: TW + span of the map
     for (int m = 0; m < 4; ++m) {
         TSB_REQUIRE(span_map[m] <= 8, "conv_v2: tap span too large");
-        prm.a_bytes[m] = (TW + span_map[m]) * TH * 128;
+        box_w[m] = TW + span_map[m];
+        prm.a_bytes[m] = box_w[m] * TH * 128;
     }
     prm.ngroups = ng;
     prm.ntaps_total = d.ntaps;
     prm.kchunks = d.kchunks;
-    // ---- A tensor maps (box width = TW + span of the map)
-    const __nv_bfloat16* base = reinterpret_cast<const __nv_bfloat16*>(d.act);
-    int rc;
-    if (d.stem) {
-        const uint64_t row = (uint64_t)(d.aW + 4) * 16 * 2;
-        rc = encode_4d(&prm.mapA[0], base, 64, (uint64_t)d.aW, (uint64_t)d.aH, (uint64_t)d.aN, 32, row, row * d.aH, 64, TW + span_map[0], TH, 1);
-        if (rc) return rc;
-    } else if (d.act_stride == 1) {
-        rc = encode_4d(&prm.mapA[0], base, d.aC, d.aW, d.aH, d.aN, (uint64_t)d.acs * 2, (uint64_t)d.aW * d.acs * 2,
-                       (uint64_t)d.aH * d.aW * d.acs * 2, 64, TW + span_map[0], TH, 1);
-        if (rc) return rc;
-    } else {
-        for (int ph = 0; ph < 2; ++ph)
-            for (int pw = 0; pw < 2; ++pw) {
-                int Hh = (d.aH - ph + 1) / 2, Ww = (d.aW - pw + 1) / 2;
-                if (Hh <= 0) Hh = 1;
-                if (Ww <= 0) Ww = 1;
-                rc = encode_4d(&prm.mapA[ph * 2 + pw], base + ((long long)ph * d.aW + pw) * d.acs, d.aC, Ww, Hh, d.aN,
-                               (uint64_t)2 * d.acs * 2, (uint64_t)2 * d.aW * d.acs * 2, (uint64_t)d.aH * d.aW * d.acs * 2, 64,
-                               TW + span_map[ph * 2 + pw], TH, 1);
-                if (rc) return rc;
-            }
-    }
+    int rc = d.stem ? encode_stem_map(&prm.mapA[0], d.act, d.aN, d.aH, d.aW, box_w[0], TH)
+                    : encode_act_maps(prm.mapA, d.act, d.aN, d.aH, d.aW, d.aC, d.acs, d.act_stride, box_w, TH);
+    if (rc) return rc;
     rc = encode_2d(&prm.mapB, d.w, (uint64_t)d.w_k, (uint64_t)d.w_rows, (uint64_t)d.w_k * 2, 64, BN);
     if (rc) return rc;
     // ---- geometry / epilogue
@@ -496,11 +431,10 @@ int launch(const Desc& d, cudaStream_t st) {
     prm.k_real = d.k_real; prm.k_store = d.k_store; prm.out_f32 = d.out_f32; prm.accumulate = d.accumulate;
     prm.bias = d.bias; prm.sum = d.sum; prm.sumsq = d.sumsq; prm.out = d.out;
     prm.relu = d.relu; prm.res = d.res;
-    prm.use_base_offset = g_use_base_offset;
     // ---- shared-memory plan
     const int kBTile = BN * 128;
     const long long res_need = (long long)d.ntaps * d.kchunks * kBTile;
-    const bool resident = g_allow_resident && res_need <= 112 * 1024 && prm.m_tiles > 0;
+    const bool resident = res_need <= 112 * 1024 && prm.m_tiles > 0;
     const int tail = 256 + kConsumers * 4 * 2 * BN * 4;
     const int budget = 227 * 1024 - 1024 /*align*/ - tail;
     int max_group_taps = 1;
@@ -533,7 +467,7 @@ int launch(const Desc& d, cudaStream_t st) {
 
 // row-tile wgrad: returns TSB_ERR_UNSUPPORTED when the shape is not eligible (caller falls back to the patch kernel)
 int launch_wgrad_rows(const WgradDesc& d, cudaStream_t st) {
-    if (!g_allow_rows || d.Q < 64) return TSB_ERR_UNSUPPORTED;
+    if (d.Q < 64) return TSB_ERR_UNSUPPORTED;
     WrParams prm;
     memset(&prm, 0, sizeof(prm));
     const int TW = 64;
@@ -566,51 +500,32 @@ int launch_wgrad_rows(const WgradDesc& d, cudaStream_t st) {
     }
     prm.ngroups = ng;
     prm.cchunks = d.C / 64;
-    for (int m = 0; m < 4; ++m) prm.b_bytes[m] = (TW + span_map[m]) * 128;
+    int box_w[4];
+    for (int m = 0; m < 4; ++m) {
+        box_w[m] = TW + span_map[m];
+        prm.b_bytes[m] = box_w[m] * 128;
+    }
     int rc = encode_4d(&prm.mapA, d.dy, d.K, d.Q, d.P, d.N, (uint64_t)d.dycs * 2, (uint64_t)d.Q * d.dycs * 2,
                        (uint64_t)d.P * d.Q * d.dycs * 2, 64, TW, 1, 1);
     if (rc) return rc;
-    const __nv_bfloat16* xb = reinterpret_cast<const __nv_bfloat16*>(d.x);
-    if (d.stride == 1) {
-        rc = encode_4d(&prm.mapB[0], xb, d.C, d.W, d.H, d.N, (uint64_t)d.xcs * 2, (uint64_t)d.W * d.xcs * 2,
-                       (uint64_t)d.H * d.W * d.xcs * 2, 64, TW + span_map[0], 1, 1);
-        if (rc) return rc;
-    } else {
-        for (int ph = 0; ph < 2; ++ph)
-            for (int pw = 0; pw < 2; ++pw) {
-                int Hh = (d.H - ph + 1) / 2, Ww = (d.W - pw + 1) / 2;
-                if (Hh <= 0) Hh = 1;
-                if (Ww <= 0) Ww = 1;
-                rc = encode_4d(&prm.mapB[ph * 2 + pw], xb + ((long long)ph * d.W + pw) * d.xcs, d.C, Ww, Hh, d.N,
-                               (uint64_t)2 * d.xcs * 2, (uint64_t)2 * d.W * d.xcs * 2, (uint64_t)d.H * d.W * d.xcs * 2, 64,
-                               TW + span_map[ph * 2 + pw], 1, 1);
-                if (rc) return rc;
-            }
-    }
+    rc = encode_act_maps(prm.mapB, d.x, d.N, d.H, d.W, d.C, d.xcs, d.stride, box_w, 1);
+    if (rc) return rc;
     prm.TW = TW;
     prm.tiles_w = (d.Q + TW - 1) / TW;
     prm.tiles_h = d.P;
     prm.total_tiles = prm.tiles_w * prm.tiles_h * d.N;
-    prm.K = d.K; prm.C = d.C; prm.dw_row_stride = d.dw_row_stride; prm.dw = d.dw;
-    prm.use_base_offset = g_use_base_offset;
+    prm.K = d.K; prm.C = d.C; prm.dw_row_stride = d.dw_row_stride;
     const int co_tiles = (d.K + 127) / 128;
     const int zdim = ng * prm.cchunks;
-    int base = zdim * co_tiles;
-    int want = (g_wgrad_waves * tsb_num_sms() + base - 1) / base;
-    int max_splits = (prm.total_tiles + 15) / 16;
-    if (want > max_splits) want = max_splits;
-    const long long n_dw = (long long)d.K * d.dw_row_stride;
-    if (want > (d.ws ? d.ws_floats / n_dw : 0)) want = (int)(d.ws ? d.ws_floats / n_dw : 0);
-    if (want < 1) want = 1;
-    prm.tiles_per_split = (prm.total_tiles + want - 1) / want;
-    int splits = (prm.total_tiles + prm.tiles_per_split - 1) / prm.tiles_per_split;
-    prm.add = splits == 1;
-    prm.dw = prm.add ? d.dw : d.ws;
-    prm.part_stride = prm.add ? 0 : n_dw;
+    // about two waves of CTAs, at least 16 tiles per split
+    const SplitPlan sp = plan_splits(wave_splits(zdim * co_tiles, prm.total_tiles, 16), prm.total_tiles,
+                                     (long long)d.K * d.dw_row_stride, d.dw, d.ws, d.ws_floats);
+    prm.tiles_per_split = sp.tiles_per_split;
+    prm.add = sp.add; prm.dw = sp.dst; prm.part_stride = sp.part_stride;
     { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(wgrad_rows_kernel), kWrSmem); if (rc_) return rc_; }
-    wgrad_rows_kernel<<<dim3(splits, co_tiles, zdim), kThreads, kWrSmem, st>>>(prm);
+    wgrad_rows_kernel<<<dim3(sp.splits, co_tiles, zdim), kThreads, kWrSmem, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("wgrad_rows");
-    return prm.add ? TSB_OK : tsb_det_reduce(d.dw, prm.dw, splits, n_dw, n_dw, st);
+    return finish_splits(sp, d.dw, st);
 }
 
 }  // namespace convv2

@@ -47,9 +47,6 @@ struct WgradDesc {
     long long ws_floats;
 };
 
-extern int g_wgrad_waves;
-extern int g_use_base_offset;   // tsb_debug_set key 1
-extern int g_allow_taps;
 int launch(const Desc& d, cudaStream_t st);
 int launch_wgrad_rows(const WgradDesc& d, cudaStream_t st);
 int launch_wgrad_taps(const WgradDesc& d, int R, int pad, int dil, cudaStream_t st);   // conv_wgrad_taps.cu

@@ -42,7 +42,6 @@ struct alignas(64) TpParams {
     float* dw;                 // dW-shaped slice per split (workspace), part_stride apart; or dW itself when `add`
     long long part_stride;
     int add;                   // one split: add in place
-    int use_base_offset;
 };
 
 __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_constant__ TpParams p) {
@@ -50,7 +49,7 @@ __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* tail = smem + p.nstages * p.stage_bytes;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
-    uint64_t* empty_bar = full_bar + kTpMaxStages;
+    StageRing ring(full_bar, full_bar + kTpMaxStages, p.nstages);
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31;
     const int co0 = blockIdx.y * 64, ci0 = blockIdx.z * 64;
     const int t_begin = blockIdx.x * p.tiles_per_split;
@@ -61,30 +60,28 @@ __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_
     if (warp == kProducer && lane == 0) {
         tma_prefetch_desc(&p.mapDy);
         tma_prefetch_desc(&p.mapX);
-        for (int s = 0; s < p.nstages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kTpConsumers * 4); }
+        ring.init(kTpConsumers * 4);
         fence_barrier_init();
     }
     __syncthreads();
 
     if (warp == kProducer) {
         if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
             const uint32_t bytes = (uint32_t)(kTpDyBytes + 3 * p.slot_bytes);
             for (int it = 0; it < iters; ++it) {
-                mbar_wait(&empty_bar[s], ph ^ 1u);
+                ring.acquire();
                 const int t = t_begin + it;
                 const int q0 = (t % p.tiles_w) * p.TW;
                 const int p0 = ((t / p.tiles_w) % p.tiles_h) * p.TH;
                 const int n_img = t / (p.tiles_w * p.tiles_h);
-                uint8_t* st = smem + s * p.stage_bytes;
-                mbar_arrive_expect_tx(&full_bar[s], bytes);
-                tma_load_4d(st, &p.mapDy, &full_bar[s], co0, q0, p0, n_img);
+                uint8_t* st = smem + ring.slot * p.stage_bytes;
+                mbar_arrive_expect_tx(ring.full_bar(), bytes);
+                tma_load_4d(st, &p.mapDy, ring.full_bar(), co0, q0, p0, n_img);
 #pragma unroll
                 for (int r = 0; r < 3; ++r)
-                    tma_load_4d(st + kTpDyBytes + r * p.slot_bytes, &p.mapX, &full_bar[s], ci0, q0 - p.dil,
+                    tma_load_4d(st + kTpDyBytes + r * p.slot_bytes, &p.mapX, ring.full_bar(), ci0, q0 - p.dil,
                                 p0 + (r - 1) * p.dil, n_img);
-                if (++s == p.nstages) { s = 0; ph ^= 1u; }
+                ring.advance();
             }
         }
     } else {   // every split stores its (possibly all-zero) tile: the slices are summed in split order afterwards
@@ -102,35 +99,22 @@ __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_
             for (int q = 0; q < 32; ++q) acc[t][q] = 0.f;
 #pragma unroll
         for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
-        // a stage is released one stage late: wait_group<1> after issuing stage s retires the MMAs of stage s-1, so the
-        // tensor pipe never drains between stages
-        int s = 0, prev = -1;
-        uint32_t ph = 0;
         for (int it = 0; it < iters; ++it) {
-            mbar_wait(&full_bar[s], ph);
-            wgmma_fence();
-            const uint32_t st_lo = base_lo + (uint32_t)(s * (p.stage_bytes >> 4));
+            ring.wait_full();
+            const uint32_t st_lo = base_lo + (uint32_t)(ring.slot * (p.stage_bytes >> 4));
             const uint32_t x_lo = st_lo + (kTpDyBytes >> 4) + (uint32_t)r * ((uint32_t)p.slot_bytes >> 4);
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                const uint64_t db = desc_at(desc_hi, st_lo + kb[k], 0);
+                const uint64_t db = desc_at(desc_hi, st_lo + kb[k]);
 #pragma unroll
                 for (int t = 0; t < 3; ++t)
-                    wgmma_m64n64<1, 1>(acc[t], desc_at(desc_hi, x_lo + t * tap16 + ka[k], p.use_base_offset), db, 1u);
+                    wgmma_m64n64<1, 1>(acc[t], desc_at(desc_hi, x_lo + t * tap16 + ka[k]), db, 1u);
             }
-            wgmma_commit();
-            if (prev >= 0) {
-                wgmma_wait<1>();
-                // wait_group covers only this warp's MMAs: every consumer warp releases the stage
-                if (lane == 0) mbar_arrive(&empty_bar[prev]);
-            }
-            prev = s;
-            if (++s == p.nstages) { s = 0; ph ^= 1u; }
+            ring.commit_release_prev();
         }
-        wgmma_wait<0>();
+        ring.drain();
 #pragma unroll
         for (int t = 0; t < 3; ++t) fence_operands(acc[t]);
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
         // fragment: rows = input channels ci0 + 16·wq + lane/4 (+8), columns = output channels co0 + 8j + 2(lane%4) (+1)
         // dW is [K][3][3][C] fp32
 #pragma unroll
@@ -156,11 +140,9 @@ __global__ void __launch_bounds__(kTpThreads, 1) wgrad_taps_kernel(const __grid_
 
 namespace convv2 {
 
-int g_allow_taps = 1;   // tsb_debug_set key 8
-
 // returns TSB_ERR_UNSUPPORTED when the shape is not eligible (caller falls back to the row / patch kernels)
 int launch_wgrad_taps(const WgradDesc& d, int R, int pad, int dil, cudaStream_t st) {
-    if (!g_allow_taps || R != 3 || d.stride != 1 || pad != dil || dil < 1 || dil > 8) return TSB_ERR_UNSUPPORTED;
+    if (R != 3 || d.stride != 1 || pad != dil || dil < 1 || dil > 8) return TSB_ERR_UNSUPPORTED;
     if (d.C % 64 != 0 || d.K % 8 != 0 || d.P != d.H || d.Q != d.W) return TSB_ERR_UNSUPPORTED;
     TpParams prm;
     memset(&prm, 0, sizeof(prm));
@@ -190,8 +172,7 @@ int launch_wgrad_taps(const WgradDesc& d, int R, int pad, int dil, cudaStream_t 
     prm.tiles_w = (d.Q + TW - 1) / TW;
     prm.tiles_h = (d.P + TH - 1) / TH;
     prm.total_tiles = prm.tiles_w * prm.tiles_h * d.N;
-    prm.K = d.K; prm.C = d.C; prm.dw_row_stride = d.dw_row_stride; prm.dw = d.dw;
-    prm.use_base_offset = g_use_base_offset;
+    prm.K = d.K; prm.C = d.C; prm.dw_row_stride = d.dw_row_stride;
     const int co_tiles = (d.K + 63) / 64, ci_tiles = d.C / 64;
     const int base = co_tiles * ci_tiles;
     // one CTA per SM (persistent over a contiguous pixel range); at least 8 tiles per CTA so the drain of the nine
@@ -209,20 +190,15 @@ int launch_wgrad_taps(const WgradDesc& d, int R, int pad, int dil, cudaStream_t 
         const long long cost = waves * (per + 6);     // + ~6 stage-times of prologue / accumulator drain per CTA
         if (best < 0 || cost < best) { best = cost; want = sp; }
     }
-    const long long n_dw = (long long)d.K * d.dw_row_stride;
-    if (want > (d.ws ? d.ws_floats / n_dw : 0)) want = (int)(d.ws ? d.ws_floats / n_dw : 0);
-    if (want < 1) want = 1;
-    prm.tiles_per_split = (prm.total_tiles + want - 1) / want;
-    const int splits = (prm.total_tiles + prm.tiles_per_split - 1) / prm.tiles_per_split;
-    prm.add = splits == 1;
-    prm.dw = prm.add ? d.dw : d.ws;
-    prm.part_stride = prm.add ? 0 : n_dw;
+    const SplitPlan sp = plan_splits(want, prm.total_tiles, (long long)d.K * d.dw_row_stride, d.dw, d.ws, d.ws_floats);
+    prm.tiles_per_split = sp.tiles_per_split;
+    prm.add = sp.add; prm.dw = sp.dst; prm.part_stride = sp.part_stride;
     const size_t smem = 1024 + (size_t)ns * prm.stage_bytes + 256;
     rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(wgrad_taps_kernel), smem);
     if (rc) return rc;
-    wgrad_taps_kernel<<<dim3(splits, co_tiles, ci_tiles), kTpThreads, smem, st>>>(prm);
+    wgrad_taps_kernel<<<dim3(sp.splits, co_tiles, ci_tiles), kTpThreads, smem, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("wgrad_taps");
-    return prm.add ? TSB_OK : tsb_det_reduce(d.dw, prm.dw, splits, n_dw, n_dw, st);
+    return finish_splits(sp, d.dw, st);
 }
 
 }  // namespace convv2

@@ -138,8 +138,8 @@ constexpr int kStrip = 256;          // hi-res columns per CTA (== kThreads)
 // low-res columns a strip can touch: kStrip*w/W + 3; the two staged source rows live in DYNAMIC shared memory
 // sized by the host from the actual scale (s_lo[2][maxcols][CMAX])
 
-template <int CMAX, bool kHoist>
-__global__ void __launch_bounds__(kThreads, kHoist ? 2 : 1)
+template <int CMAX>
+__global__ void __launch_bounds__(kThreads, 1)
 ohem_ptarget_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64_t* __restrict__ labels, int N,
                        int C, int H, int W, int ignore_label, float thresh, float* __restrict__ p,
                        float* __restrict__ nll, uint32_t* state, int maxcols) {
@@ -162,15 +162,6 @@ ohem_ptarget_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const
     const bool xin = x < x1;
     const Lerp lx = make_lerp(rx, xin ? x : x0, w);
     const int j0 = lx.i0 - g.jbase, j1 = lx.i1 - g.jbase;
-    float t0[CMAX], t1[CMAX];   // horizontally blended source rows of this thread's column (row-invariant)
-#pragma unroll
-    for (int c = 0; c < CMAX; ++c) {
-        t0[c] = 0.f; t1[c] = 0.f;
-        if (kHoist && c < C) {
-            t0[c] = lerp_h(lx, s_lo0[j0 * CMAX + c], s_lo0[j1 * CMAX + c]);
-            t1[c] = lerp_h(lx, s_lo1[j0 * CMAX + c], s_lo1[j1 * CMAX + c]);
-        }
-    }
     // software pipeline: the label of row y+1 is requested before row y is evaluated (the row body is ~900 issue
     // slots, enough to cover the global-load latency at 8-16 resident warps)
     long long lab_next = xin ? labels[((long long)n * H + g.y_lo) * W + x] : 0;
@@ -186,9 +177,8 @@ ohem_ptarget_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const
 #pragma unroll
         for (int c = 0; c < CMAX; ++c)
             if (c < C)
-                v[c] = kHoist ? lerp_v(ly, t0[c], t1[c])
-                              : lerp_v(ly, lerp_h(lx, s_lo0[j0 * CMAX + c], s_lo0[j1 * CMAX + c]),
-                                       lerp_h(lx, s_lo1[j0 * CMAX + c], s_lo1[j1 * CMAX + c]));
+                v[c] = lerp_v(ly, lerp_h(lx, s_lo0[j0 * CMAX + c], s_lo0[j1 * CMAX + c]),
+                              lerp_h(lx, s_lo1[j0 * CMAX + c], s_lo1[j1 * CMAX + c]));
         float p_t, nl;
         softmax_target<CMAX>(v, C, t, p_t, nl);
         pt_emit(i, valid, p_t, nl, thresh, p, nll, acc);
@@ -423,8 +413,8 @@ ohem_grad_kernel(const T* __restrict__ logits, long long sn, long long sc, long 
 //            column j and accumulates top += l0(y)*s, bot += l1(y)*s in registers.
 // After the band: red.global.add of top → row i, bot → row i1.  No shuffles, no per-pixel atomics.
 // ---------------------------------------------------------------------------------------------
-template <int CMAX, bool kHoist>
-__global__ void __launch_bounds__(kThreads, kHoist ? 2 : 1)
+template <int CMAX>
+__global__ void __launch_bounds__(kThreads, 2)
 ohem_grad_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64_t* __restrict__ labels,
                     const float* __restrict__ p, int N, int C, int H, int W, int ignore_label,
                     const float* __restrict__ cw, const uint32_t* __restrict__ state,
@@ -468,7 +458,7 @@ ohem_grad_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const in
 #pragma unroll
     for (int c = 0; c < CMAX; ++c) {
         G0[c] = 0.f; G1[c] = 0.f; t0[c] = 0.f; t1[c] = 0.f;
-        if (kHoist && c < C && xin) {   // horizontally blended source rows: row-invariant, formed once per band
+        if (c < C && xin) {   // horizontally blended source rows: row-invariant, formed once per band
             t0[c] = lerp_h(lx, s_lo0[j0 * CMAX + c], s_lo0[j1 * CMAX + c]);
             t1[c] = lerp_h(lx, s_lo1[j0 * CMAX + c], s_lo1[j1 * CMAX + c]);
         }
@@ -500,9 +490,7 @@ ohem_grad_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const in
 #pragma unroll
         for (int c = 0; c < CMAX; ++c)
             if (c < C) {
-                v[c] = kHoist ? lerp_v(ly, t0[c], t1[c])
-                              : lerp_v(ly, lerp_h(lx, s_lo0[j0 * CMAX + c], s_lo0[j1 * CMAX + c]),
-                                       lerp_h(lx, s_lo1[j0 * CMAX + c], s_lo1[j1 * CMAX + c]));
+                v[c] = lerp_v(ly, t0[c], t1[c]);
                 m = fmaxf(m, v[c]);
             }
         float ssum = 0.f;
@@ -765,11 +753,10 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
 
 }  // namespace
 
-// A/B switch (tsb_debug_set key 6): band kernels keep the horizontally blended source rows in registers; bit 0 =
-// gradient kernel (measured 2.16 -> 1.85 ms/step), bit 1 = p_target kernel (measured slower: 111 registers halve the
-// occupancy of an issue-bound kernel, 1.72 -> 1.85 ms) — default 1.
-int g_tsb_ohem_hoist = 1;
-int g_tsb_ohem_exact = 1;   // tsb_debug_set key 10: exact-class-count band kernels (C = 19 / 21)
+// Generic band kernels (class counts other than 19 / 21): the gradient kernel forms the horizontally blended source
+// rows once per band and keeps them in registers (measured 2.16 -> 1.85 ms/step); the p_target kernel blends them again
+// for every row, because keeping them costs it 111 registers, which halves the occupancy of an issue-bound kernel
+// (measured 1.72 -> 1.85 ms when kept).
 
 // =============================================================================================
 // C ABI
@@ -818,7 +805,7 @@ extern "C" int tsb_ohem_ptarget_up(const float* logits_lo, int cs, int h, int w,
     TSB_REQUIRE(N <= 65535 && h <= 65535, "tsb_ohem_ptarget_up: N and h must fit a grid dimension");
     const int maxcols = band_maxcols(w, W);
     dim3 grid((W + kStrip - 1) / kStrip, h, N);
-    if (g_tsb_ohem_exact && (C == 19 || C == 21)) {      // exact-class-count kernels (Cityscapes / VOC)
+    if (C == 19 || C == 21) {      // exact-class-count kernels (Cityscapes / VOC)
         const size_t smx = sizeof(float) * (2 * (size_t)C * kPitchX + 2 * (size_t)maxcols * C);
         if (smx <= 100 * 1024) {
 #define LX(CX)                                                                                                      \
@@ -836,9 +823,8 @@ extern "C" int tsb_ohem_ptarget_up(const float* logits_lo, int cs, int h, int w,
     const int cmax = C <= 20 ? 20 : 32;
     const size_t smem = sizeof(float) * 2 * (size_t)maxcols * cmax;
     TSB_REQUIRE(smem <= 28 * 1024, "tsb_ohem_ptarget_up: up-scale factor W/w too small for the band kernel");
-#define L(CM, HO) ohem_ptarget_up_kernel<CM, HO><<<grid, kThreads, smem, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, N, C, H, W, ignore_label, thresh, p, nll, state, maxcols)
-    if (C <= 20) { if (g_tsb_ohem_hoist & 2) L(20, true); else L(20, false); }
-    else { if (g_tsb_ohem_hoist & 2) L(32, true); else L(32, false); }
+#define L(CM) ohem_ptarget_up_kernel<CM><<<grid, kThreads, smem, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, N, C, H, W, ignore_label, thresh, p, nll, state, maxcols)
+    if (C <= 20) L(20); else L(32);
 #undef L
     TSB_CUDA_CHECK_LAUNCH("ohem_ptarget_up");
     return TSB_OK;
@@ -902,7 +888,7 @@ extern "C" int tsb_ohem_grad_up(const float* logits_lo, int cs, int h, int w, co
     TSB_REQUIRE(N <= 65535 && h <= 65535, "tsb_ohem_grad_up: N and h must fit a grid dimension");
     const int maxcols = band_maxcols(w, W);
     TSB_REQUIRE(maxcols <= kStrip, "tsb_ohem_grad_up: up-scale factor W/w too small for the band kernel");
-    if (g_tsb_ohem_exact && (C == 19 || C == 21)) {
+    if (C == 19 || C == 21) {
         const size_t smx = sizeof(float) * (2 * (size_t)C * kPitchX + 2 * (size_t)maxcols * C);
         if (smx <= 72 * 1024) {
             dim3 gridx(((W + kStrip - 1) / kStrip + 1) / 2, (h + 1) / 2, N);
@@ -925,13 +911,12 @@ extern "C" int tsb_ohem_grad_up(const float* logits_lo, int cs, int h, int w, co
     TSB_REQUIRE(smem <= 96 * 1024, "tsb_ohem_grad_up: shared memory budget exceeded");
     dim3 grid((W + kStrip - 1) / kStrip, h, N);
     cudaStream_t st = (cudaStream_t)stream;
-#define L(CM, HO)                                                                                                       \
+#define L(CM)                                                                                                           \
     do {                                                                                                                \
-        { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(ohem_grad_up_kernel<CM, HO>), smem); if (rc_) return rc_; } \
-        ohem_grad_up_kernel<CM, HO><<<grid, kThreads, smem, st>>>(logits_lo, cs, h, w, labels, p, N, C, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols); \
+        { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(ohem_grad_up_kernel<CM>), smem); if (rc_) return rc_; } \
+        ohem_grad_up_kernel<CM><<<grid, kThreads, smem, st>>>(logits_lo, cs, h, w, labels, p, N, C, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols); \
     } while (0)
-    if (C <= 20) { if (g_tsb_ohem_hoist & 1) L(20, true); else L(20, false); }
-    else { if (g_tsb_ohem_hoist & 1) L(32, true); else L(32, false); }
+    if (C <= 20) L(20); else L(32);
 #undef L
     TSB_CUDA_CHECK_LAUNCH("ohem_grad_up");
     return TSB_OK;

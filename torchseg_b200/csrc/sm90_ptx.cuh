@@ -97,6 +97,58 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t desc_a, u
         : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
+// ------------------------------------------------------------------ stage ring
+// The shared-memory stage ring between one TMA producer thread and the consumer warps of a wgmma kernel. full[s]
+// completes when the TMA bytes of stage s have landed, empty[s] when every consumer warp has retired the MMAs that read
+// it. Both sides walk the stages in the same order and flip the parity on every wrap.
+//
+// A consumer releases a stage one stage late: after issuing stage s it commits and waits until at most one group is
+// pending, which retires the MMAs of stage s-1, so the tensor pipe never drains between stages. wait_group covers only
+// the calling warp's MMAs, so every consumer warp releases the stage (lane 0 arrives). The ring touches no
+// accumulator: the kernel pins its accumulators (fence_operands) where ordinary instructions read or write them.
+struct StageRing {
+    uint64_t* full;
+    uint64_t* empty;
+    int stages;
+    int slot = 0;
+    uint32_t phase = 0;
+    int prev = -1;   // consumer: the stage whose MMAs may still be in flight
+
+    __device__ __forceinline__ StageRing(uint64_t* full_bar, uint64_t* empty_bar, int n)
+        : full(full_bar), empty(empty_bar), stages(n) {}
+    // one thread, before fence_barrier_init()
+    __device__ __forceinline__ void init(uint32_t consumer_warps) {
+        for (int s = 0; s < stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], consumer_warps); }
+    }
+    __device__ __forceinline__ void advance() {
+        if (++slot == stages) { slot = 0; phase ^= 1u; }
+    }
+    // producer: wait until the consumers have released the current stage; fill it through full_bar(), then advance()
+    __device__ __forceinline__ void acquire() { mbar_wait(&empty[slot], phase ^ 1u); }
+    __device__ __forceinline__ uint64_t* full_bar() { return &full[slot]; }
+    // consumer: wait for the current stage's data; the MMAs of the stage follow
+    __device__ __forceinline__ void wait_full() {
+        mbar_wait(&full[slot], phase);
+        wgmma_fence();
+    }
+    // consumer, after issuing the current stage: commit it, release the previous one, advance
+    __device__ __forceinline__ void commit_release_prev() {
+        wgmma_commit();
+        if (prev >= 0) {
+            wgmma_wait<1>();
+            if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[prev]);
+        }
+        prev = slot;
+        advance();
+    }
+    // consumer, after the last stage: retire every MMA and release the last stage
+    __device__ __forceinline__ void drain() {
+        wgmma_wait<0>();
+        if (prev >= 0 && (threadIdx.x & 31) == 0) mbar_arrive(&empty[prev]);
+        prev = -1;
+    }
+};
+
 // ------------------------------------------------------------------ descriptors
 // Shared-memory matrix descriptor (sm_90 GMMA layout): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
 // base_offset [49,52), layout_type [62,64) (1 = SWIZZLE_128B). The start address is OR-ed into bits [0,14) by the caller.
@@ -104,12 +156,11 @@ __host__ __device__ constexpr uint64_t desc_hi_sw128(uint32_t lbo_bytes, uint32_
     return ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) |
            ((uint64_t)1 << 62);
 }
-// Descriptor of an operand starting at shared address `lo` (in 16-byte units). With `base_off` the 128-byte row phase
-// of the start inside the 1024-byte swizzle pattern goes into base_offset (a start shifted by whole rows, as the taps
-// of a row tile are).
-__device__ __forceinline__ uint64_t desc_at(uint64_t hi, uint32_t lo, int base_off) {
-    return hi | (uint64_t)(lo & 0x3FFFu) | (base_off ? (uint64_t)((lo >> 3) & 7u) << 49 : 0ull);
-}
+// Descriptor of an operand starting at shared address `lo` (in 16-byte units), base_offset 0. This holds also for a
+// start shifted by whole 128-byte rows inside the 1024-byte swizzle pattern (the taps of a row tile): H100 takes the
+// swizzle phase from the absolute shared address, and putting the row phase (lo >> 3) & 7 into base_offset was measured
+// to give wrong results.
+__device__ __forceinline__ uint64_t desc_at(uint64_t hi, uint32_t lo) { return hi | (uint64_t)(lo & 0x3FFFu); }
 
 
 }  // namespace sm90
