@@ -110,7 +110,9 @@ int tsb_ohem_grad_up(const float* logits_lo, int cs, int h, int w, const int64_t
 /* ================================================================================================
  * Bilinear resize, align_corners=True — replaces F.interpolate(mode='bilinear', align_corners=True)
  * call sites model/bisenet/cityscapes.bisenet.R18/network.py:82-84,93-94,164-166 (SURVEY §8 a10).
- * NHWC, C channels, channel strides ics/ocs. Backward is the deterministic gather-form transpose.
+ * NHWC, C channels, channel strides ics/ocs >= C. Backward is the deterministic gather-form transpose.
+ * The forward takes 16-byte vectors when C, ics and ocs are multiples of 8 and both pointers are 16-byte aligned, and
+ * a scalar path otherwise; the backward requires exactly that (C, ics, ocs multiples of 8; dout, din 16-byte aligned).
  * ============================================================================================== */
 int tsb_bilinear_fwd(const void* in, int idtype, int ics, void* out, int odtype, int ocs, int N, int C, int Hi,
                      int Wi, int Ho, int Wo, tsb_stream_t stream);
@@ -122,7 +124,8 @@ int tsb_bilinear_fwd_nhwc_to_nchw(const void* in, int idtype, int ics, float* ou
 
 /* ================================================================================================
  * Pooling — nn.AdaptiveAvgPool2d (furnace/seg_opr/seg_oprs.py:113,200,223; pspnet network.py:83)
- * and nn.MaxPool2d(3,2,1) (furnace/base_model/resnet.py:132). NHWC bf16.
+ * and nn.MaxPool2d(3,2,1) (furnace/base_model/resnet.py:132). NHWC bf16; C and every channel stride are multiples of
+ * 8 with stride >= C; activations and the fp32 adaptive-pool gradient dout are 16-byte aligned, argmax 8-byte aligned.
  * ============================================================================================== */
 /* out fp32 [N, S, S, C] (bins [floor(i*H/S), ceil((i+1)*H/S)) ), S==1 is the global pool */
 int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, int H, int W, int S, float* out, float* ws,
@@ -142,6 +145,8 @@ int tsb_maxpool3x3s2_bwd(const void* argmax, const void* dout, int ocs, void* di
  * bn1/bn2 (resnet.py:24-51) and apex SyncBatchNorm (train.py:54-55). Statistics come from the conv
  * epilogue (tsb_conv2d sum/sumsq) or tsb_bn_stats; cross-GPU reduction of {sum,sumsq} happens between
  * stats and finalize (NCCL, outside this library).
+ * x, y, dy, dx, residual, dres: bf16 NHWC, C and channel strides multiples of 8, strides >= C, 16-byte aligned. The fp32
+ * per-channel vectors (scale, shift, mean, invstd, gamma, sum_dz, sum_dz_xhat) and the workspace are 16-byte aligned.
  * ============================================================================================== */
 /* per-channel sum and sum of squares of x (bf16 NHWC), accumulated into fp32 sum[C], sumsq[C] (caller zeroes) */
 int tsb_bn_stats(const void* x, int cs, long long npix, int C, float* sum, float* sumsq, float* ws, long long ws_floats,
@@ -174,6 +179,7 @@ int tsb_bn_bwd_apply(const void* dy, int dycs, const void* y, int ycs, const voi
  * caller's `fm += last_fm`, bisenet network.py:91-92) and FeatureFusion.forward seg_oprs.py:233-238
  * (fm + fm*sigmoid(se)).  a[n,c] is the PRE-sigmoid attention logit (fp32 [N,C]).
  *   y = x * (base + sigmoid(a[n,c])) + add          base=0 (ARM) / 1 (FFM); add may be NULL
+ * bf16 NHWC operands: C and channel strides multiples of 8, strides >= C, 16-byte aligned; a is 16-byte aligned.
  * ============================================================================================== */
 int tsb_chan_scale_fwd(const void* x, int xcs, const float* a, float base, const void* add, int acs, void* y,
                        int ycs, int N, int HW, int C, tsb_stream_t stream);
@@ -196,7 +202,8 @@ int tsb_pack_weight(const float* w, int K, int R, int S, int C, void* w_bf16, vo
  * (dW[K,R,R,3] += unpack(dWp[K,4,4,16] fp32)) */
 int tsb_pack_stem_weight(const float* w, int K, int R, void* wp_bf16, tsb_stream_t stream);
 int tsb_unpack_stem_wgrad(const float* dwp, int K, int R, float* dw, tsb_stream_t stream);
-/* elementwise: dst = (dtype)src * (*scale_dev or 1) ; strided NHWC channel slices, C multiple of 8 */
+/* elementwise: dst = (dtype)src * (*scale_dev or 1) ; strided NHWC channel slices, C multiple of 8.
+ * For cast_scale, add, add_relu and relu_bwd: C and channel strides multiples of 8, strides >= C, 16-byte aligned. */
 int tsb_cast_scale(const void* src, int sdtype, int scs, void* dst, int ddtype, int dcs, long long npix, int C,
                    const float* scale_dev, tsb_stream_t stream);
 /* dst[pix, 0..Kp) = (bf16) src[pix, 0..K) zero-extended (any K, any source channel stride): the gradient of a K-class
@@ -269,7 +276,7 @@ int tsb_conv_stem_fprop_fused(const void* xs2d, int N, int H, int W, const void*
                               void* y, int ycs, tsb_stream_t stream);
 int tsb_conv_stem_wgrad(const void* xs2d, int N, int H, int W, const void* dy, int dycs, int K, float* dwp, float* ws,
                         long long ws_floats, tsb_stream_t stream);
-/* column sums: db[k] += Σ_pixels dy[pix,k] (bias gradient of the 1x1 classifier heads) */
+/* column sums: db[k] += Σ_pixels dy[pix,k] (bias gradient of the 1x1 classifier heads); any K, dycs >= K */
 int tsb_bias_grad(const void* dy, int dycs, long long npix, int K, float* db, float* ws, long long ws_floats,
                   tsb_stream_t stream);
 

@@ -52,6 +52,50 @@ def test_argument_validation_without_gpu(lib):
                               ctypes.addressof(buf), 1, 64, None, None, None, 0, None)
     assert rc == -1 and b"multiple of 64" in lib.tsb_last_error()
 
+    # The streaming NHWC kernels move 16-byte vectors (fp32 per-channel vectors as float4, the max-pool argmax as
+    # 8 bytes) and address pixel p at p * cs: a misaligned pointer or a channel stride below C must come back as
+    # TSB_ERR_ARG with a message, before any CUDA call, instead of launching a kernel that faults or writes into the
+    # next pixel. A = 256-byte aligned host memory, M = 2 bytes past it (bf16-aligned only), M4 = 4 bytes past it.
+    mem = (ctypes.c_uint8 * 4096)()
+    A = (ctypes.addressof(mem) + 255) & ~255
+    M, M4 = A + 2, A + 4
+    C, npix, WS = 16, 4, 1 << 20
+    cases = [
+        ("tsb_bilinear_bwd", (A, 1, 8, A, 1, C, 1, C, 2, 2, 4, 4, 0, None), b">= C"),
+        ("tsb_adaptive_avgpool_fwd", (A, 8, 1, C, 4, 4, 2, A, A, WS, None), b">= C"),
+        ("tsb_adaptive_avgpool_bwd", (A, 1, C, 4, 4, 2, A, 8, 0, None), b">= C"),
+        ("tsb_maxpool3x3s2_fwd", (M, C, A, C, A, 1, C, 4, 4, None), b"aligned"),
+        ("tsb_maxpool3x3s2_fwd", (A, C, A, C, M4, 1, C, 4, 4, None), b"argmax 8B aligned"),
+        ("tsb_maxpool3x3s2_fwd", (A, C, A, 8, A, 1, C, 4, 4, None), b">= C"),
+        ("tsb_maxpool3x3s2_bwd", (A, M, C, A, C, 1, C, 4, 4, None), b"aligned"),
+        ("tsb_maxpool3x3s2_bwd", (A, A, C, A, 8, 1, C, 4, 4, None), b">= C"),
+        ("tsb_bn_stats", (A, 8, npix, C, A, A, A, WS, None), b">= C"),
+        ("tsb_bn_stats", (A, C, npix, C, A, A, M4, WS, None), b"ws must be 16B aligned"),
+        ("tsb_bn_apply", (A, C, M4, A, None, 0, 1, A, C, npix, C, None), b"scale and shift must be 16B aligned"),
+        ("tsb_bn_apply", (A, C, A, A, A, 8, 1, A, C, npix, C, None), b">= C"),
+        ("tsb_bn_bwd_reduce", (A, C, None, 0, A, C, M4, A, 0, npix, C, A, A, None, None, A, WS, None),
+         b"per-channel vectors must be 16B aligned"),
+        ("tsb_bn_bwd_reduce", (A, C, None, 0, A, C, A, A, 1, npix, C, A, A, A, M4, A, WS, None),
+         b"per-channel vectors must be 16B aligned"),
+        ("tsb_bn_bwd_reduce", (A, C, None, 0, A, 8, A, A, 0, npix, C, A, A, None, None, A, WS, None), b">= C"),
+        ("tsb_bn_bwd_apply", (A, C, None, 0, A, C, A, A, M4, A, A, 4.0, 0, A, C, None, 0, npix, C, None, None, None,
+                              None, None), b"per-channel vectors must be 16B aligned"),
+        ("tsb_bn_bwd_apply", (A, C, None, 0, A, C, A, A, A, A, A, 4.0, 0, A, C, A, 8, npix, C, None, None, None, None,
+                              None), b">= C"),
+        ("tsb_chan_scale_fwd", (A, C, A, 0.0, None, 0, A, 8, 1, npix, C, None), b">= C"),
+        ("tsb_chan_scale_bwd", (A, C, A, 8, A, 1.0, A, C, A, 1, npix, C, A, WS, None), b">= C"),
+        ("tsb_cast_scale", (A, 1, C, A, 1, 8, npix, C, None, None), b">= C"),
+        ("tsb_bias_grad", (A, 16, npix, 19, A, A, WS, None), b">= K"),
+    ]
+    for name in ("tsb_add", "tsb_add_relu", "tsb_relu_bwd"):
+        cases += [(name, (A, C, M, C, A, C, npix, C, None), b"16B aligned"),
+                  (name, (A, C, A, C, M, C, npix, C, None), b"16B aligned"),
+                  (name, (A, C, A, C, A, 8, npix, C, None), b">= C")]
+    for name, args, msg in cases:
+        rc = getattr(lib, name)(*args)
+        err = lib.tsb_last_error()
+        assert rc == -1 and msg in err and name.encode() in err, (name, args, rc, err)
+
 
 def test_product_path_fails_loudly_without_cuda():
     import torch

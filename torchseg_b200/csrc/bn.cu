@@ -439,15 +439,17 @@ static inline int colred_grid(long long npix, int C8) {
 }
 }  // namespace
 
-#define TSB_VEC_OK(C, cs, ptr) ((C) % 8 == 0 && (cs) % 8 == 0 && tsb_aligned16(ptr))
+// an NHWC bf16 operand read or written with 16-byte vectors: C and its channel stride multiples of 8, cs >= C, aligned
+#define TSB_VEC_OK(C, cs, ptr) ((C) % 8 == 0 && (cs) % 8 == 0 && (cs) >= (C) && tsb_aligned16(ptr))
 
 extern "C" int tsb_bn_stats(const void* x, int cs, long long npix, int C, float* sum, float* sumsq, float* ws,
                             long long ws_floats, tsb_stream_t stream) {
     TSB_REQUIRE(x && sum && sumsq && npix > 0, "tsb_bn_stats: bad args");
-    TSB_REQUIRE(TSB_VEC_OK(C, cs, x), "tsb_bn_stats: C and cs must be multiples of 8");
+    TSB_REQUIRE(TSB_VEC_OK(C, cs, x), "tsb_bn_stats: C and cs must be multiples of 8, cs >= C, x 16B aligned");
     int C8 = C / 8;
     const int grid = colred_grid(npix, C8);
     TSB_REQUIRE(ws && (long long)grid * 2 * C <= ws_floats, "tsb_bn_stats: workspace needs %lld floats", (long long)grid * 2 * C);
+    TSB_REQUIRE(tsb_aligned16(ws), "tsb_bn_stats: ws must be 16B aligned");
     bn_stats_kernel<<<grid, kThreads, colred_smem(C8, 2), (cudaStream_t)stream>>>((const __nv_bfloat16*)x, cs, npix, C8, ws, ws + C, 2LL * C);
     TSB_CUDA_CHECK_LAUNCH("bn_stats");
     int rc = tsb_det_reduce(sum, ws, grid, C, 2LL * C, (cudaStream_t)stream);
@@ -467,7 +469,8 @@ extern "C" int tsb_bn_apply(const void* x, int xcs, const float* scale, const fl
                             int rcs, int relu, void* y, int ycs, long long npix, int C, tsb_stream_t stream) {
     TSB_REQUIRE(x && scale && shift && y && npix > 0, "tsb_bn_apply: bad args");
     TSB_REQUIRE(TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, ycs, y) && (!residual || TSB_VEC_OK(C, rcs, residual)),
-                "tsb_bn_apply: C and channel strides must be multiples of 8");
+                "tsb_bn_apply: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned");
+    TSB_REQUIRE(tsb_aligned16(scale) && tsb_aligned16(shift), "tsb_bn_apply: scale and shift must be 16B aligned");
     int C8 = C / 8;
     int grid = tsb_grid_for(npix * C8, kThreads, 8);
     cudaStream_t st = (cudaStream_t)stream;
@@ -486,11 +489,14 @@ extern "C" int tsb_bn_bwd_reduce(const void* dy, int dycs, const void* y, int yc
     TSB_REQUIRE(dy && x && mean && invstd && sum_dz && sum_dz_xhat && npix > 0, "tsb_bn_bwd_reduce: bad args");
     const int mode = !relu ? 0 : (y ? 1 : 2);
     TSB_REQUIRE(mode != 2 || (scale && shift), "tsb_bn_bwd_reduce: relu without y needs scale and shift");
-    TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && (mode != 1 || TSB_VEC_OK(C, ycs, y)), "tsb_bn_bwd_reduce: alignment");
+    TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && (mode != 1 || TSB_VEC_OK(C, ycs, y)), "tsb_bn_bwd_reduce: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned");
+    TSB_REQUIRE(tsb_aligned16(mean) && tsb_aligned16(invstd) && (mode != 2 || (tsb_aligned16(scale) && tsb_aligned16(shift))),
+                "tsb_bn_bwd_reduce: per-channel vectors must be 16B aligned");
     int C8 = C / 8;
     cudaStream_t st = (cudaStream_t)stream;
     const int grid = colred_grid(npix, C8);
     TSB_REQUIRE(ws && (long long)grid * 2 * C <= ws_floats, "tsb_bn_bwd_reduce: workspace needs %lld floats", (long long)grid * 2 * C);
+    TSB_REQUIRE(tsb_aligned16(ws), "tsb_bn_bwd_reduce: ws must be 16B aligned");
 #define L(M) bn_bwd_reduce_kernel<M><<<grid, kThreads, colred_smem(C8, 2), st>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)y, ycs, (const __nv_bfloat16*)x, xcs, mean, invstd, scale, shift, npix, C8, ws, ws + C, 2LL * C)
     if (mode == 0) L(0); else if (mode == 1) L(1); else L(2);
 #undef L
@@ -509,7 +515,10 @@ extern "C" int tsb_bn_bwd_apply(const void* dy, int dycs, const void* y, int ycs
     const int mode = !relu ? 0 : (y ? 1 : 2);
     TSB_REQUIRE(mode != 2 || (scale && shift), "tsb_bn_bwd_apply: relu without y needs scale and shift");
     TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, dxcs, dx) &&
-                (mode != 1 || TSB_VEC_OK(C, ycs, y)) && (!dres || TSB_VEC_OK(C, drcs, dres)), "tsb_bn_bwd_apply: alignment");
+                (mode != 1 || TSB_VEC_OK(C, ycs, y)) && (!dres || TSB_VEC_OK(C, drcs, dres)), "tsb_bn_bwd_apply: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned");
+    TSB_REQUIRE(tsb_aligned16(mean) && tsb_aligned16(invstd) && tsb_aligned16(gamma) && tsb_aligned16(sum_dz) &&
+                tsb_aligned16(sum_dz_xhat) && (mode != 2 || (tsb_aligned16(scale) && tsb_aligned16(shift))),
+                "tsb_bn_bwd_apply: per-channel vectors must be 16B aligned");
     int C8 = C / 8;
     int grid = tsb_grid_for(npix * C8, kThreads, 8);
     cudaStream_t st = (cudaStream_t)stream;
@@ -526,7 +535,7 @@ extern "C" int tsb_bn_bwd_apply(const void* dy, int dycs, const void* y, int ycs
 extern "C" int tsb_chan_scale_fwd(const void* x, int xcs, const float* a, float base, const void* add, int acs, void* y,
                                   int ycs, int N, int HW, int C, tsb_stream_t stream) {
     TSB_REQUIRE(x && a && y && N > 0 && HW > 0, "tsb_chan_scale_fwd: bad args");
-    TSB_REQUIRE(TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, ycs, y) && (!add || TSB_VEC_OK(C, acs, add)) && tsb_aligned16(a), "tsb_chan_scale_fwd: alignment");
+    TSB_REQUIRE(TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, ycs, y) && (!add || TSB_VEC_OK(C, acs, add)) && tsb_aligned16(a), "tsb_chan_scale_fwd: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned");
     int C8 = C / 8;
     long long total = (long long)N * HW * C8;
     int grid = tsb_grid_for(total, kThreads, 8);
@@ -543,7 +552,7 @@ extern "C" int tsb_chan_scale_bwd(const void* dy, int dycs, const void* x, int x
                                   int dxcs, float* da, int N, int HW, int C, float* ws, long long ws_floats,
                                   tsb_stream_t stream) {
     TSB_REQUIRE(dy && x && a && dx && da && N > 0 && HW > 0, "tsb_chan_scale_bwd: bad args");
-    TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, dxcs, dx) && tsb_aligned16(a), "tsb_chan_scale_bwd: alignment");
+    TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, dxcs, dx) && tsb_aligned16(a), "tsb_chan_scale_bwd: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned");
     int C8 = C / 8;
     int groups = C8 < kThreads ? C8 : kThreads;
     int lanes = kThreads / groups;

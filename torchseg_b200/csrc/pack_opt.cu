@@ -347,7 +347,9 @@ extern "C" int tsb_unpack_stem_wgrad(const float* dwp, int K, int R, float* dw, 
 extern "C" int tsb_cast_scale(const void* src, int sdtype, int scs, void* dst, int ddtype, int dcs, long long npix, int C,
                               const float* scale_dev, tsb_stream_t stream) {
     TSB_REQUIRE(src && dst && npix > 0 && C > 0, "tsb_cast_scale: bad args");
-    TSB_REQUIRE(C % 8 == 0 && scs % 8 == 0 && dcs % 8 == 0 && tsb_aligned16(src) && tsb_aligned16(dst), "tsb_cast_scale: alignment");
+    TSB_REQUIRE(scs >= C && dcs >= C, "tsb_cast_scale: channel strides must be >= C");
+    TSB_REQUIRE(C % 8 == 0 && scs % 8 == 0 && dcs % 8 == 0 && tsb_aligned16(src) && tsb_aligned16(dst),
+                "tsb_cast_scale: C and channel strides must be multiples of 8, pointers 16B aligned");
     int C8 = C / 8;
     int grid = tsb_grid_for(npix * C8, kThreads, 8);
     cudaStream_t st = (cudaStream_t)stream;
@@ -379,7 +381,9 @@ extern "C" int tsb_cast_pad(const void* src, int sdtype, int scs, int K, void* d
 extern "C" int tsb_add(const void* a, int acs, const void* b, int bcs, void* y, int ycs, long long npix, int C,
                        tsb_stream_t stream) {
     TSB_REQUIRE(a && b && y && npix > 0, "tsb_add: bad args");
-    TSB_REQUIRE(C % 8 == 0 && acs % 8 == 0 && bcs % 8 == 0 && ycs % 8 == 0, "tsb_add: alignment");
+    TSB_REQUIRE(acs >= C && bcs >= C && ycs >= C, "tsb_add: channel strides must be >= C");
+    TSB_REQUIRE(C % 8 == 0 && acs % 8 == 0 && bcs % 8 == 0 && ycs % 8 == 0 && tsb_aligned16(a) && tsb_aligned16(b) && tsb_aligned16(y),
+                "tsb_add: C and channel strides must be multiples of 8, pointers 16B aligned");
     int C8 = C / 8;
     int grid = tsb_grid_for(npix * C8, kThreads, 8);
     add_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)a, acs, (const __nv_bfloat16*)b, bcs, (__nv_bfloat16*)y, ycs, npix, C8);
@@ -390,7 +394,9 @@ extern "C" int tsb_add(const void* a, int acs, const void* b, int bcs, void* y, 
 extern "C" int tsb_add_relu(const void* a, int acs, const void* b, int bcs, void* y, int ycs, long long npix, int C,
                             tsb_stream_t stream) {
     TSB_REQUIRE(a && b && y && npix > 0, "tsb_add_relu: bad args");
-    TSB_REQUIRE(C % 8 == 0 && acs % 8 == 0 && bcs % 8 == 0 && ycs % 8 == 0, "tsb_add_relu: alignment");
+    TSB_REQUIRE(acs >= C && bcs >= C && ycs >= C, "tsb_add_relu: channel strides must be >= C");
+    TSB_REQUIRE(C % 8 == 0 && acs % 8 == 0 && bcs % 8 == 0 && ycs % 8 == 0 && tsb_aligned16(a) && tsb_aligned16(b) && tsb_aligned16(y),
+                "tsb_add_relu: C and channel strides must be multiples of 8, pointers 16B aligned");
     int C8 = C / 8;
     int grid = tsb_grid_for(npix * C8, kThreads, 8);
     add_relu_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)a, acs, (const __nv_bfloat16*)b, bcs, (__nv_bfloat16*)y, ycs, npix, C8);
@@ -401,7 +407,9 @@ extern "C" int tsb_add_relu(const void* a, int acs, const void* b, int bcs, void
 extern "C" int tsb_relu_bwd(const void* dy, int dycs, const void* y, int ycs, void* dx, int dxcs, long long npix, int C,
                             tsb_stream_t stream) {
     TSB_REQUIRE(dy && y && dx && npix > 0, "tsb_relu_bwd: bad args");
-    TSB_REQUIRE(C % 8 == 0 && dycs % 8 == 0 && ycs % 8 == 0 && dxcs % 8 == 0, "tsb_relu_bwd: alignment");
+    TSB_REQUIRE(dycs >= C && ycs >= C && dxcs >= C, "tsb_relu_bwd: channel strides must be >= C");
+    TSB_REQUIRE(C % 8 == 0 && dycs % 8 == 0 && ycs % 8 == 0 && dxcs % 8 == 0 && tsb_aligned16(dy) && tsb_aligned16(y) && tsb_aligned16(dx),
+                "tsb_relu_bwd: C and channel strides must be multiples of 8, pointers 16B aligned");
     int C8 = C / 8;
     int grid = tsb_grid_for(npix * C8, kThreads, 8);
     relu_bwd_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)y, ycs, (__nv_bfloat16*)dx, dxcs, npix, C8);
@@ -412,6 +420,7 @@ extern "C" int tsb_relu_bwd(const void* dy, int dycs, const void* y, int ycs, vo
 extern "C" int tsb_bias_grad(const void* dy, int dycs, long long npix, int K, float* db, float* ws, long long ws_floats,
                              tsb_stream_t stream) {
     TSB_REQUIRE(dy && db && npix > 0 && K > 0, "tsb_bias_grad: bad args");
+    TSB_REQUIRE(dycs >= K, "tsb_bias_grad: dycs must be >= K");
     int grid = tsb_grid_for(npix, 64, 4);
     TSB_REQUIRE(ws && (long long)grid * K <= ws_floats, "tsb_bias_grad: workspace needs %lld floats", (long long)grid * K);
     bias_grad_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)dy, dycs, npix, K, ws);

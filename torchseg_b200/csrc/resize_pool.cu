@@ -446,6 +446,7 @@ extern "C" int tsb_bilinear_fwd_nhwc_to_nchw(const void* in, int idtype, int ics
 extern "C" int tsb_bilinear_bwd(const void* dout, int odtype, int ocs, void* din, int idtype, int ics, int N, int C,
                                 int Hi, int Wi, int Ho, int Wo, int accumulate, tsb_stream_t stream) {
     TSB_REQUIRE(dout && din && TSB_DT_OK(idtype) && TSB_DT_OK(odtype), "tsb_bilinear_bwd: bad args");
+    TSB_REQUIRE(ics >= C && ocs >= C, "tsb_bilinear_bwd: channel strides must be >= C");
     TSB_REQUIRE((C % 8 == 0) && (ics % 8 == 0) && (ocs % 8 == 0) && tsb_aligned16(dout) && tsb_aligned16(din),
                 "tsb_bilinear_bwd: C and channel strides must be multiples of 8, pointers 16B aligned");
     long long total = (long long)N * Hi * Wi * (C / 8);
@@ -464,7 +465,8 @@ extern "C" int tsb_bilinear_bwd(const void* dout, int odtype, int ocs, void* din
 extern "C" int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, int H, int W, int S, float* out, float* ws,
                                         long long ws_floats, tsb_stream_t stream) {
     TSB_REQUIRE(in && out, "tsb_adaptive_avgpool_fwd: null pointer");
-    TSB_REQUIRE(C % 8 == 0 && ics % 8 == 0 && tsb_aligned16(in), "tsb_adaptive_avgpool_fwd: C, ics must be multiples of 8");
+    TSB_REQUIRE(ics >= C, "tsb_adaptive_avgpool_fwd: ics must be >= C");
+    TSB_REQUIRE(C % 8 == 0 && ics % 8 == 0 && tsb_aligned16(in), "tsb_adaptive_avgpool_fwd: C, ics must be multiples of 8, in 16B aligned");
     TSB_REQUIRE(S >= 1 && S <= H && S <= W, "tsb_adaptive_avgpool_fwd: bad S");
     cudaStream_t st = (cudaStream_t)stream;
     TSB_CUDA_CALL(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)N * S * S * C, st));
@@ -488,7 +490,9 @@ extern "C" int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, i
 extern "C" int tsb_adaptive_avgpool_bwd(const float* dout, int N, int C, int H, int W, int S, void* din, int ics,
                                         int accumulate, tsb_stream_t stream) {
     TSB_REQUIRE(dout && din, "tsb_adaptive_avgpool_bwd: null pointer");
-    TSB_REQUIRE(C % 8 == 0 && ics % 8 == 0 && tsb_aligned16(din) && tsb_aligned16(dout), "tsb_adaptive_avgpool_bwd: C, ics multiples of 8");
+    TSB_REQUIRE(ics >= C, "tsb_adaptive_avgpool_bwd: ics must be >= C");
+    TSB_REQUIRE(C % 8 == 0 && ics % 8 == 0 && tsb_aligned16(din) && tsb_aligned16(dout),
+                "tsb_adaptive_avgpool_bwd: C, ics must be multiples of 8, pointers 16B aligned");
     long long total = (long long)N * H * W * (C / 8);
     int grid = tsb_grid_for(total, kThreads, 8);
     if (S == 1) {
@@ -504,7 +508,10 @@ extern "C" int tsb_adaptive_avgpool_bwd(const float* dout, int N, int C, int H, 
 
 extern "C" int tsb_maxpool3x3s2_fwd(const void* in, int ics, void* out, int ocs, void* argmax, int N, int C, int H,
                                     int W, tsb_stream_t stream) {
-    TSB_REQUIRE(in && out && C % 8 == 0 && ics % 8 == 0 && ocs % 8 == 0, "tsb_maxpool3x3s2_fwd: bad args");
+    TSB_REQUIRE(in && out, "tsb_maxpool3x3s2_fwd: null pointer");
+    TSB_REQUIRE(ics >= C && ocs >= C, "tsb_maxpool3x3s2_fwd: channel strides must be >= C");
+    TSB_REQUIRE(C % 8 == 0 && ics % 8 == 0 && ocs % 8 == 0 && tsb_aligned16(in) && tsb_aligned16(out) && tsb_aligned8(argmax),
+                "tsb_maxpool3x3s2_fwd: C, strides must be multiples of 8, in/out 16B and argmax 8B aligned");
     const int P = (H + 2 - 3) / 2 + 1, Q = (W + 2 - 3) / 2 + 1;
     long long total = (long long)N * P * Q * (C / 8);
     int grid = tsb_grid_for(total, kThreads, 8);
@@ -515,7 +522,10 @@ extern "C" int tsb_maxpool3x3s2_fwd(const void* in, int ics, void* out, int ocs,
 
 extern "C" int tsb_maxpool3x3s2_bwd(const void* argmax, const void* dout, int ocs, void* din, int dcs, int N, int C,
                                     int H, int W, tsb_stream_t stream) {
-    TSB_REQUIRE(argmax && dout && din && C % 8 == 0 && ocs % 8 == 0 && dcs % 8 == 0, "tsb_maxpool3x3s2_bwd: bad args");
+    TSB_REQUIRE(argmax && dout && din, "tsb_maxpool3x3s2_bwd: null pointer");
+    TSB_REQUIRE(ocs >= C && dcs >= C, "tsb_maxpool3x3s2_bwd: channel strides must be >= C");
+    TSB_REQUIRE(C % 8 == 0 && ocs % 8 == 0 && dcs % 8 == 0 && tsb_aligned16(dout) && tsb_aligned16(din) && tsb_aligned8(argmax),
+                "tsb_maxpool3x3s2_bwd: C, strides must be multiples of 8, dout/din 16B and argmax 8B aligned");
     const int P = (H + 2 - 3) / 2 + 1, Q = (W + 2 - 3) / 2 + 1;
     long long total = (long long)N * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
     int grid = tsb_grid_for(total, kThreads, 8);

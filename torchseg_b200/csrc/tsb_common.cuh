@@ -60,6 +60,7 @@ static inline int tsb_num_sms() {
 }
 
 static inline bool tsb_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+static inline bool tsb_aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 
 // grid sized as a multiple of the SM count (grid-stride kernels)
 static inline int tsb_grid_for(long long work_items, int per_block, int blocks_per_sm) {
