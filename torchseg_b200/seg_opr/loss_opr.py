@@ -37,6 +37,10 @@ class ProbOhemCrossEntropy2d(nn.Module):
 
     def forward_lowres(self, logits_lo, target, num_classes):
         H, W = target.shape[-2:]
+        if tuple(logits_lo.shape[-2:]) == (H, W):
+            # head already at label resolution (the .speed lines): nothing to interpolate, so the strided pair reads
+            # the classifier's fp32 NHWC buffer in place
+            return self.forward(logits_lo, target)
         return self._record(ops.OhemUpCEFn.apply(logits_lo, target, H, W, num_classes, self.ignore_label, self.thresh,
                                                  self.min_kept, self.weight))
 
