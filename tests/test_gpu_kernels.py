@@ -340,20 +340,23 @@ def test_cuda_prefetcher_delivers_batches_in_order(cuda):
     assert seen == 7
 
 
-@pytest.mark.parametrize("cfg", [(19, 16, False), (21, 8, True), (20, 8, False), (19, 4, True)],
-                         ids=["c19_x16", "c21_x8_weighted", "c20_generic", "c19_x4_weighted"])
+@pytest.mark.parametrize("cfg", [(19, 16, False), (21, 8, True), (20, 8, False), (19, 4, True), (19, (89, 301), False),
+                                 (20, (89, 301), False)],
+                         ids=["c19_x16", "c21_x8_weighted", "c20_generic", "c19_x4_weighted", "c19_89x301",
+                              "c20_generic_89x301"])
 def test_ohem_fused_upsample_variants(cuda, cfg):
-    """exact-class-count band kernels (C = 19 / 21) and the generic fallback (C = 20), scales x4 / x8 / x16, class
-    weights: p bits and kept set vs the C oracle, gradient vs autograd through F.interpolate + the torch restatement"""
+    """exact-class-count band kernels (C = 19 / 21) and the generic fallback (C = 20), scales x4 / x8 / x16 and a
+    non-integer one (12 x 40 -> 89 x 301: uneven column segments), class weights: p bits and kept set vs the C oracle,
+    gradient vs autograd through F.interpolate + the torch restatement"""
     ops = _ops()
     from oracle import c_oracle, torch_ref
-    C, s, weighted = cfg
+    C, size, weighted = cfg
     N, h, w = 2, 12, 40
-    H, W = h * s, w * s
-    g = torch.Generator().manual_seed(100 + C + s)
+    H, W = (h * size, w * size) if isinstance(size, int) else size
+    g = torch.Generator().manual_seed(100 + C + H // h)
     labels = make_labels(N, H, W, C, 255, g)
     lo = torch.randn(N, h, w, 32, generator=g) * 2
-    lab_lo = labels[:, ::s, ::s].clamp(max=C - 1)
+    lab_lo = labels[:, torch.arange(h) * H // h][:, :, torch.arange(w) * W // w].clamp(max=C - 1)
     lo[..., :C] += 3 * F.one_hot(lab_lo, C).float()
     cwt = (torch.rand(C, generator=g) + 0.5) if weighted else None
     min_kept = N * H * W // 16
@@ -370,7 +373,7 @@ def test_ohem_fused_upsample_variants(cuda, cfg):
     assert np.array_equal(kept, ref["kept"])
     assert abs(loss.item() - ref["loss"]) <= 1e-5 * abs(ref["loss"])
     lo_t = lo[..., :C].permute(0, 3, 1, 2).clone().requires_grad_(True)
-    l2 = torch_ref.ohem_ce(F.interpolate(lo_t, scale_factor=s, mode="bilinear", align_corners=True), labels, 255, 0.7,
+    l2 = torch_ref.ohem_ce(F.interpolate(lo_t, size=(H, W), mode="bilinear", align_corners=True), labels, 255, 0.7,
                            min_kept, weight=cwt)
     l2.backward()
     assert rel_err(lo_dev.grad, lo_t.grad) < 1e-3

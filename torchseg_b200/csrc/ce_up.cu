@@ -10,8 +10,9 @@
 // + 3 flops per class for the value, and the 4 lanes of a pixel combine max / sum with two shuffles.
 //   forward : lse[pixel] = logsumexp_c v_c (kept for the backward), loss = mean over valid pixels of lse − v_target
 //   backward: d lo[i, j, c] += Σ_pixels w_y·w_x·(exp(v_c − lse) − [c = target])·g/count — the softmax part through per-thread
-//             register accumulators reduced per band in shared memory (phase 2, as in the OHEM gradient kernel), the one-hot part
-//             through a low-resolution shared-memory tile (4 RED.shared per pixel)
+//             register accumulators reduced per band in shared memory (phase 2: band.cuh col_sums, shared with the OHEM
+//             gradient kernels), the one-hot part through a low-resolution shared-memory tile (4 RED.shared per pixel) that
+//             phase 2 starts from
 #include "band.cuh"
 
 namespace {
@@ -40,26 +41,16 @@ ce_up_fwd_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64
     float* s_lo1 = s_lo0 + maxcols * C;
     const float ry = area_scale(h, H), rx = area_scale(w, W);
     const int n = blockIdx.z, ci = blockIdx.y, x0 = blockIdx.x * kXS, x1 = min(W, x0 + kXS);
-    const int i1 = ci + (ci < h - 1 ? 1 : 0);
-    const BandGeom g = band_geom(ry, rx, ci, x0, x1, H, w);
+    const BandGeom g = band_geom(ry, rx, ci, x0, x1, h, H, w);
     if (g.ncols > maxcols) __trap();
-    for (int q = threadIdx.x; q < 2 * g.ncols * C; q += kT) {
-        const int c = q % C, t2 = q / C, col = t2 % g.ncols, row = t2 / g.ncols;
-        (row ? s_lo1 : s_lo0)[col * C + c] = __ldg(lo + (((long long)n * h + (row ? i1 : ci)) * w + g.jbase + col) * cs + c);
-    }
+    stage_rows<kT>(lo, cs, h, w, n, ci, g, C, C, s_lo0, s_lo1);
     __syncthreads();
     const int xloc = threadIdx.x >> 2, qd = threadIdx.x & 3;
     const int x = x0 + xloc;
     const bool xin = x < x1;
     const Lerp lx = make_lerp(rx, xin ? x : x0, w);
     const int j0 = lx.i0 - g.jbase, j1 = lx.i1 - g.jbase;
-    for (int j = 0; j < J; ++j) {
-        const int c = 4 * j + qd;
-        if (c < C) {
-            sT0[t_index(c, xloc)] = lerp_h(lx, s_lo0[j0 * C + c], s_lo0[j1 * C + c]);
-            sT1[t_index(c, xloc)] = lerp_h(lx, s_lo1[j0 * C + c], s_lo1[j1 * C + c]);
-        }
-    }
+    blend_rows(lx, j0, j1, s_lo0, s_lo1, C, J, qd, 4, C, sT0, sT1, [&](int c) { return t_index(c, xloc); });
     // (thread-private entries: no barrier needed before the row loop; lanes of one pixel only read each other's entries for
     //  the TARGET class, so make the quad's writes visible to the quad)
     __syncwarp();
@@ -136,36 +127,18 @@ ce_up_bwd_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64
     const float ry = area_scale(h, H), rx = area_scale(w, W);
     const int n = blockIdx.z, ci = blockIdx.y, x0 = blockIdx.x * kXS, x1 = min(W, x0 + kXS);
     const int nx = x1 - x0;
-    const int i1 = ci + (ci < h - 1 ? 1 : 0);
-    const BandGeom g = band_geom(ry, rx, ci, x0, x1, H, w);
+    const BandGeom g = band_geom(ry, rx, ci, x0, x1, h, H, w);
     if (g.ncols > maxcols) __trap();
-    for (int q = threadIdx.x; q < 2 * g.ncols * C; q += kT) {
-        const int c = q % C, t2 = q / C, col = t2 % g.ncols, row = t2 / g.ncols;
-        (row ? s_lo1 : s_lo0)[col * C + c] = __ldg(lo + (((long long)n * h + (row ? i1 : ci)) * w + g.jbase + col) * cs + c);
-        s_oh[q] = 0.f;
-    }
+    stage_rows<kT, true>(lo, cs, h, w, n, ci, g, C, C, s_lo0, s_lo1, s_oh);   // and clear the one-hot tile
     const int xloc = threadIdx.x >> 2, qd = threadIdx.x & 3;
     const int x = x0 + xloc;
     const bool xin = x < x1;
     const Lerp lx = make_lerp(rx, xin ? x : x0, w);
     const int j0 = lx.i0 - g.jbase, j1 = lx.i1 - g.jbase;
-    if (qd == 0) {
-        s_l0[xloc] = xin ? lx.l0 : 0.f;
-        s_l1[xloc] = xin ? lx.l1 : 0.f;
-    }
-    for (int q = threadIdx.x; q < g.ncols + 2; q += kT) s_seg[q] = (short)nx;
+    seg_init<kT>(s_l0, s_l1, s_seg, xloc, qd == 0, xin, lx, g.ncols, nx);
     __syncthreads();
-    if (xin && qd == 0) {      // s_seg[j] = first strip column whose left stencil column is >= j
-        const int jprev = (xloc == 0) ? -1 : (make_lerp(rx, x - 1, w).i0 - g.jbase);
-        for (int jj = jprev + 1; jj <= j0; ++jj) s_seg[jj] = (short)xloc;
-    }
-    for (int j = 0; j < J; ++j) {
-        const int c = 4 * j + qd;
-        if (c < C) {
-            sT0[t_index(c, xloc)] = lerp_h(lx, s_lo0[j0 * C + c], s_lo0[j1 * C + c]);
-            sT1[t_index(c, xloc)] = lerp_h(lx, s_lo1[j0 * C + c], s_lo1[j1 * C + c]);
-        }
-    }
+    seg_fill(s_seg, xloc, qd == 0, xin, rx, x, w, g.jbase, j0);
+    blend_rows(lx, j0, j1, s_lo0, s_lo1, C, J, qd, 4, C, sT0, sT1, [&](int c) { return t_index(c, xloc); });
     float G0[kJMax], G1[kJMax];
 #pragma unroll
     for (int j = 0; j < kJMax; ++j) { G0[j] = 0.f; G1[j] = 0.f; }
@@ -214,39 +187,16 @@ ce_up_bwd_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64
         if (c < C) { sT0[t_index(c, xloc)] = G0[j]; sT1[t_index(c, xloc)] = G1[j]; }
     }
     __syncthreads();
-    // phase 2: low-res column j receives the l0x-weighted sum of its own segment of strip columns and the l1x-weighted sum of
-    // the previous segment (or of its own when the stencil is clamped at the last column)
+    // phase 2, starting from the one-hot tile
     const int npairs = g.ncols * C;
     for (int q = threadIdx.x; q < npairs; q += kT) {
         const int j = q / C, c = q - j * C;
-        const int a0 = s_seg[j], a1 = s_seg[j + 1];
-        float top = s_oh[j * C + c], bot = s_oh[(g.ncols + j) * C + c];
-        for (int xx = a0; xx < a1; ++xx) {
-            const float wl = s_l0[xx];
-            top = fmaf(wl, sT0[t_index(c, xx)], top);
-            bot = fmaf(wl, sT1[t_index(c, xx)], bot);
-        }
-        const bool clamped = (g.jbase + j == w - 1);
-        const int b0 = clamped ? a0 : (j > 0 ? (int)s_seg[j - 1] : 0);
-        const int b1 = clamped ? a1 : (j > 0 ? a0 : 0);
-        for (int xx = b0; xx < b1; ++xx) {
-            const float wr = s_l1[xx];
-            top = fmaf(wr, sT0[t_index(c, xx)], top);
-            bot = fmaf(wr, sT1[t_index(c, xx)], bot);
-        }
-        if (clamped && j > 0) {
-            for (int xx = s_seg[j - 1]; xx < a0; ++xx) {
-                const float wr = s_l1[xx];
-                top = fmaf(wr, sT0[t_index(c, xx)], top);
-                bot = fmaf(wr, sT1[t_index(c, xx)], bot);
-            }
-        }
-        if (top != 0.f) atomicAdd(dlo + (((long long)n * h + ci) * w + g.jbase + j) * cs + c, top);
-        if (bot != 0.f) atomicAdd(dlo + (((long long)n * h + i1) * w + g.jbase + j) * cs + c, bot);
+        const float2 s = col_sums(sT0, sT1, [&](int xx) { return t_index(c, xx); }, s_seg, s_l0, s_l1, g, w, j,
+                                  s_oh[j * C + c], s_oh[(g.ncols + j) * C + c]);
+        if (s.x != 0.f) atomicAdd(dlo + (((long long)n * h + ci) * w + g.jbase + j) * cs + c, s.x);
+        if (s.y != 0.f) atomicAdd(dlo + (((long long)n * h + g.i1) * w + g.jbase + j) * cs + c, s.y);
     }
 }
-
-inline int ce_maxcols(int w, int W) { return (int)(((long long)kXS * w + W - 1) / W) + 3; }
 
 }  // namespace
 
@@ -255,7 +205,7 @@ extern "C" int tsb_ce_up_fwd(const float* logits_lo, int cs, int h, int w, const
     TSB_REQUIRE(logits_lo && labels && lse && state, "tsb_ce_up_fwd: null pointer");
     TSB_REQUIRE(N > 0 && N <= 65535 && h > 0 && h <= 65535 && w > 0 && H > 0 && W > 0, "tsb_ce_up_fwd: bad shape");
     TSB_REQUIRE(C >= 1 && C <= 4 * kJMax && cs >= C, "tsb_ce_up_fwd: 1 <= C <= %d", 4 * kJMax);
-    const int maxcols = ce_maxcols(w, W);
+    const int maxcols = band_maxcols(kXS, w, W);
     const int J = (C + 3) / 4;
     const size_t smem = sizeof(float) * (2 * (size_t)J * kTQ + 2 * (size_t)maxcols * C);
     TSB_REQUIRE(smem <= 110 * 1024, "tsb_ce_up_fwd: up-scale factor W/w too small for the band kernel");
@@ -276,7 +226,7 @@ extern "C" int tsb_ce_up_bwd(const float* logits_lo, int cs, int h, int w, const
     TSB_REQUIRE(logits_lo && labels && lse && state && dlogits_lo, "tsb_ce_up_bwd: null pointer");
     TSB_REQUIRE(N > 0 && N <= 65535 && h > 0 && h <= 65535 && w > 0 && H > 0 && W > 0, "tsb_ce_up_bwd: bad shape");
     TSB_REQUIRE(C >= 1 && C <= 4 * kJMax && cs >= C, "tsb_ce_up_bwd: 1 <= C <= %d", 4 * kJMax);
-    const int maxcols = ce_maxcols(w, W);
+    const int maxcols = band_maxcols(kXS, w, W);
     TSB_REQUIRE(maxcols <= kXS, "tsb_ce_up_bwd: up-scale factor W/w too small for the band kernel");
     const int J = (C + 3) / 4;
     const size_t smem = sizeof(float) * (2 * (size_t)J * kTQ + 4 * (size_t)maxcols * C);

@@ -67,6 +67,8 @@ __device__ __forceinline__ void pt_flush(const PtAccum& acc, uint32_t* state, fl
     }
 }
 
+// CMAX > 0: the C <= CMAX logits of a pixel in registers; CMAX == 0: any C (e.g. ADE 150 classes), two passes over the
+// pixel's logits
 template <typename T, int CMAX>
 __global__ void __launch_bounds__(kThreads)
 ohem_ptarget_kernel(const T* __restrict__ logits, long long sn, long long sc, long long sy, long long sx,
@@ -84,59 +86,44 @@ ohem_ptarget_kernel(const T* __restrict__ logits, long long sn, long long sc, lo
         bool valid = lab != (long long)ignore_label;
         int t = valid ? (int)lab : 0;
         const T* base = logits + n * sn + y * sy + x * sx;
-        float v[CMAX];
-#pragma unroll
-        for (int c = 0; c < CMAX; ++c)
-            if (c < C) v[c] = ld_as_float<T>(base + c * sc);
         float p_t, nl;
-        softmax_target<CMAX>(v, C, t, p_t, nl);
-        pt_emit(i, valid, p_t, nl, thresh, p, nll, acc);
-    }
-    pt_flush(acc, state, s_red);
-}
-
-// generic-C variant (C > 32, e.g. ADE 150 classes): two passes over the pixel's logits
-template <typename T>
-__global__ void __launch_bounds__(kThreads)
-ohem_ptarget_kernel_anyc(const T* __restrict__ logits, long long sn, long long sc, long long sy, long long sx,
-                         const int64_t* __restrict__ labels, int N, int C, int H, int W, int ignore_label,
-                         float thresh, float* __restrict__ p, float* __restrict__ nll, uint32_t* state) {
-    __shared__ float s_red[33];
-    PtAccum acc;
-    const long long total = (long long)N * H * W;
-    const long long hw = (long long)H * W;
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += (long long)gridDim.x * kThreads) {
-        int n = (int)(i / hw);
-        long long r = i - (long long)n * hw;
-        int y = (int)(r / W), x = (int)(r - (long long)y * W);
-        long long lab = labels[i];
-        bool valid = lab != (long long)ignore_label;
-        int t = valid ? (int)lab : 0;
-        const T* base = logits + n * sn + y * sy + x * sx;
-        float m = ld_as_float<T>(base);
-        for (int c = 1; c < C; ++c) m = fmaxf(m, ld_as_float<T>(base + c * sc));
-        float s = 0.f, et = 0.f, xt = 0.f;
-        for (int c = 0; c < C; ++c) {
-            float xv = ld_as_float<T>(base + c * sc);
-            float e = tsb_exp_det(__fsub_rn(xv, m));
-            s = __fadd_rn(s, e);
-            if (c == t) { et = e; xt = xv; }
+        if constexpr (CMAX > 0) {
+            float v[CMAX];
+#pragma unroll
+            for (int c = 0; c < CMAX; ++c)
+                if (c < C) v[c] = ld_as_float<T>(base + c * sc);
+            softmax_target<CMAX>(v, C, t, p_t, nl);
+        } else {
+            float m = ld_as_float<T>(base);
+            for (int c = 1; c < C; ++c) m = fmaxf(m, ld_as_float<T>(base + c * sc));
+            float s = 0.f, et = 0.f, xt = 0.f;
+            for (int c = 0; c < C; ++c) {
+                float xv = ld_as_float<T>(base + c * sc);
+                float e = tsb_exp_det(__fsub_rn(xv, m));
+                s = __fadd_rn(s, e);
+                if (c == t) { et = e; xt = xv; }
+            }
+            p_t = __fdiv_rn(et, s);
+            nl = logf(s) - (xt - m);
         }
-        float p_t = __fdiv_rn(et, s);
-        float nl = logf(s) - (xt - m);
         pt_emit(i, valid, p_t, nl, thresh, p, nll, acc);
     }
     pt_flush(acc, state, s_red);
 }
 
 // ---------------------------------------------------------------------------------------------
-// Fused bilinear-upsample kernels work on BANDS: CTA = (x-strip of kStrip hi-res columns, low-res row i,
+// Fused bilinear-upsample kernels work on BANDS (band.cuh): CTA = (x-strip of kStrip hi-res columns, low-res row i,
 // image n). All hi-res rows y with floor(ry*y) == i share the two low-res source rows (i, i1), which are
 // staged once in shared memory together with the per-column lerp coefficients.
+// Generic band kernels (class counts other than 19 / 21): the gradient kernel forms the horizontally blended source
+// rows once per band and keeps them in registers (measured 2.16 -> 1.85 ms/step); the p_target kernel blends them again
+// for every row, because keeping them costs it 111 registers, which halves the occupancy of an issue-bound kernel
+// (measured 1.72 -> 1.85 ms when kept).
 // ---------------------------------------------------------------------------------------------
 constexpr int kStrip = 256;          // hi-res columns per CTA (== kThreads)
-// low-res columns a strip can touch: kStrip*w/W + 3; the two staged source rows live in DYNAMIC shared memory
-// sized by the host from the actual scale (s_lo[2][maxcols][CMAX])
+constexpr int kPitch = kStrip + 1;   // class rows of per-column shared arrays: odd pitch → conflict-free column walks
+// low-res columns a strip can touch: band_maxcols(kStrip, w, W); the two staged source rows live in DYNAMIC shared
+// memory sized by the host from the actual scale (s_lo[2][maxcols][CMAX])
 
 template <int CMAX>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -148,15 +135,11 @@ ohem_ptarget_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const
     PtAccum acc;
     const float ry = area_scale(h, H), rx = area_scale(w, W);
     const int n = blockIdx.z, ci = blockIdx.y, x0 = blockIdx.x * kStrip, x1 = min(W, x0 + kStrip);
-    const int i1 = ci + (ci < h - 1 ? 1 : 0);
-    const BandGeom g = band_geom(ry, rx, ci, x0, x1, H, w);
+    const BandGeom g = band_geom(ry, rx, ci, x0, x1, h, H, w);
     if (g.ncols > maxcols) __trap();
     float* s_lo0 = s_lo_dyn;
     float* s_lo1 = s_lo_dyn + maxcols * CMAX;
-    for (int q = threadIdx.x; q < 2 * g.ncols * C; q += kThreads) {
-        int c = q % C, t2 = q / C, col = t2 % g.ncols, row = t2 / g.ncols;
-        (row ? s_lo1 : s_lo0)[col * CMAX + c] = __ldg(lo + (((long long)n * h + (row ? i1 : ci)) * w + g.jbase + col) * cs + c);
-    }
+    stage_rows<kThreads>(lo, cs, h, w, n, ci, g, C, CMAX, s_lo0, s_lo1);
     __syncthreads();
     const int x = x0 + threadIdx.x;
     const bool xin = x < x1;
@@ -419,40 +402,29 @@ ohem_grad_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const in
                     const float* __restrict__ p, int N, int C, int H, int W, int ignore_label,
                     const float* __restrict__ cw, const uint32_t* __restrict__ state,
                     const float* __restrict__ gscale, float* __restrict__ dlo, int maxcols) {
-    constexpr int kPitch = kStrip + 1;  // odd pitch → conflict-free column walks in phase 2
     extern __shared__ float s_dyn[];    // s_g0[CMAX][kPitch], s_g1[CMAX][kPitch], s_lo[2][maxcols][CMAX]
-    float (*s_g0)[kPitch] = reinterpret_cast<float (*)[kPitch]>(s_dyn);
-    float (*s_g1)[kPitch] = reinterpret_cast<float (*)[kPitch]>(s_dyn + CMAX * kPitch);
+    float* s_g0 = s_dyn;
+    float* s_g1 = s_dyn + CMAX * kPitch;
     float* s_lo0 = s_dyn + 2 * CMAX * kPitch;
     float* s_lo1 = s_lo0 + maxcols * CMAX;
     __shared__ float s_l0[kStrip], s_l1[kStrip];
-    __shared__ short s_seg[kStrip + 8];  // s_seg[j] = first strip column whose left stencil column is >= j
+    __shared__ short s_seg[kStrip + 8];
     const bool active = state[ST_ACTIVE] != 0;
     const float Tth = __uint_as_float(state[ST_THRESH]);
     const float scale = __uint_as_float(state[ST_INVDEN]) * (gscale ? *gscale : 1.f);
     const float ry = area_scale(h, H), rx = area_scale(w, W);
     const int n = blockIdx.z, ci = blockIdx.y, x0 = blockIdx.x * kStrip, x1 = min(W, x0 + kStrip);
     const int nx = x1 - x0;
-    const int i1 = ci + (ci < h - 1 ? 1 : 0);
-    const BandGeom g = band_geom(ry, rx, ci, x0, x1, H, w);
+    const BandGeom g = band_geom(ry, rx, ci, x0, x1, h, H, w);
     if (g.ncols > maxcols) __trap();
-    for (int q = threadIdx.x; q < 2 * g.ncols * C; q += kThreads) {
-        int c = q % C, t2 = q / C, col = t2 % g.ncols, row = t2 / g.ncols;
-        (row ? s_lo1 : s_lo0)[col * CMAX + c] = __ldg(lo + (((long long)n * h + (row ? i1 : ci)) * w + g.jbase + col) * cs + c);
-    }
+    stage_rows<kThreads>(lo, cs, h, w, n, ci, g, C, CMAX, s_lo0, s_lo1);
     const int x = x0 + threadIdx.x;
     const bool xin = x < x1;
     const Lerp lx = make_lerp(rx, xin ? x : x0, w);
     const int j0 = lx.i0 - g.jbase, j1 = lx.i1 - g.jbase;
-    s_l0[threadIdx.x] = xin ? lx.l0 : 0.f;
-    s_l1[threadIdx.x] = xin ? lx.l1 : 0.f;
-    // segment starts: columns with left stencil index j form the contiguous range [s_seg[j], s_seg[j+1])
-    for (int q = threadIdx.x; q < g.ncols + 2; q += kThreads) s_seg[q] = (short)nx;
+    seg_init<kThreads>(s_l0, s_l1, s_seg, threadIdx.x, true, xin, lx, g.ncols, nx);
     __syncthreads();
-    if (xin) {
-        const int jprev = (threadIdx.x == 0) ? -1 : (make_lerp(rx, x - 1, w).i0 - g.jbase);
-        for (int jj = jprev + 1; jj <= j0; ++jj) s_seg[jj] = (short)threadIdx.x;
-    }
+    seg_fill(s_seg, threadIdx.x, true, xin, rx, x, w, g.jbase, j0);
     // ---- phase 1: per-thread accumulation over the rows of the band (registers only)
     float G0[CMAX], G1[CMAX], t0[CMAX], t1[CMAX];
 #pragma unroll
@@ -508,37 +480,15 @@ ohem_grad_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const in
     }
 #pragma unroll
     for (int c = 0; c < CMAX; ++c)
-        if (c < C) { s_g0[c][threadIdx.x] = G0[c]; s_g1[c][threadIdx.x] = G1[c]; }
+        if (c < C) { s_g0[c * kPitch + threadIdx.x] = G0[c]; s_g1[c * kPitch + threadIdx.x] = G1[c]; }
     __syncthreads();
-    // ---- phase 2 (once per band): low-res column j receives the l0x-weighted sum of its own segment and the
-    //      l1x-weighted sum of the previous segment (or of its own when the stencil is clamped at the last column)
+    // ---- phase 2 (once per band)
     const int npairs = g.ncols * C;
     for (int q = threadIdx.x; q < npairs; q += kThreads) {
         const int j = q / C, c = q - j * C;
-        const int a0 = s_seg[j], a1 = s_seg[j + 1];
-        float top = 0.f, bot = 0.f;
-        for (int xx = a0; xx < a1; ++xx) {
-            const float wl = s_l0[xx];
-            top = fmaf(wl, s_g0[c][xx], top);
-            bot = fmaf(wl, s_g1[c][xx], bot);
-        }
-        const bool clamped = (g.jbase + j == w - 1);
-        const int b0 = clamped ? a0 : (j > 0 ? (int)s_seg[j - 1] : 0);
-        const int b1 = clamped ? a1 : (j > 0 ? a0 : 0);
-        for (int xx = b0; xx < b1; ++xx) {
-            const float wr = s_l1[xx];
-            top = fmaf(wr, s_g0[c][xx], top);
-            bot = fmaf(wr, s_g1[c][xx], bot);
-        }
-        if (clamped && j > 0) {  // the previous segment still points at this (last) column with its right weight
-            for (int xx = s_seg[j - 1]; xx < a0; ++xx) {
-                const float wr = s_l1[xx];
-                top = fmaf(wr, s_g0[c][xx], top);
-                bot = fmaf(wr, s_g1[c][xx], bot);
-            }
-        }
-        if (top != 0.f) atomicAdd(dlo + (((long long)n * h + ci) * w + g.jbase + j) * cs + c, top);
-        if (bot != 0.f) atomicAdd(dlo + (((long long)n * h + i1) * w + g.jbase + j) * cs + c, bot);
+        const float2 s = col_sums(s_g0, s_g1, [&](int xx) { return c * kPitch + xx; }, s_seg, s_l0, s_l1, g, w, j, 0.f, 0.f);
+        if (s.x != 0.f) atomicAdd(dlo + (((long long)n * h + ci) * w + g.jbase + j) * cs + c, s.x);
+        if (s.y != 0.f) atomicAdd(dlo + (((long long)n * h + g.i1) * w + g.jbase + j) * cs + c, s.y);
     }
 }
 
@@ -559,40 +509,30 @@ ohem_grad_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const in
 //     columns), which leaves ~80 registers and 3 CTAs / SM.
 // Arithmetic (operation order, roundings) is unchanged: p, T and the kept set stay bit-exact against the oracle.
 // =============================================================================================
-constexpr int kPitchX = kStrip + 1;
-
 template <int CX>
 __global__ void __launch_bounds__(kThreads, 3)
 ohem_ptarget_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64_t* __restrict__ labels, int N,
                          int H, int W, int ignore_label, float thresh, float* __restrict__ p, float* __restrict__ nll,
                          uint32_t* state, int maxcols) {
     __shared__ float s_red[33];
-    extern __shared__ float s_dyn_x[];           // sT0[CX][kPitchX] | sT1[CX][kPitchX] | s_lo0[maxcols][CX] | s_lo1[...]
+    extern __shared__ float s_dyn_x[];           // sT0[CX][kPitch] | sT1[CX][kPitch] | s_lo0[maxcols][CX] | s_lo1[...]
     float* sT0 = s_dyn_x;
-    float* sT1 = s_dyn_x + CX * kPitchX;
-    float* s_lo0 = s_dyn_x + 2 * CX * kPitchX;
+    float* sT1 = s_dyn_x + CX * kPitch;
+    float* s_lo0 = s_dyn_x + 2 * CX * kPitch;
     float* s_lo1 = s_lo0 + maxcols * CX;
     PtAccum acc;
     const float ry = area_scale(h, H), rx = area_scale(w, W);
     const int n = blockIdx.z, ci = blockIdx.y, x0 = blockIdx.x * kStrip, x1 = min(W, x0 + kStrip);
-    const int i1 = ci + (ci < h - 1 ? 1 : 0);
-    const BandGeom g = band_geom(ry, rx, ci, x0, x1, H, w);
+    const BandGeom g = band_geom(ry, rx, ci, x0, x1, h, H, w);
     if (g.ncols > maxcols) __trap();
-    for (int q = threadIdx.x; q < 2 * g.ncols * CX; q += kThreads) {
-        const int c = q % CX, t2 = q / CX, col = t2 % g.ncols, row = t2 / g.ncols;
-        (row ? s_lo1 : s_lo0)[col * CX + c] = __ldg(lo + (((long long)n * h + (row ? i1 : ci)) * w + g.jbase + col) * cs + c);
-    }
+    stage_rows<kThreads>(lo, cs, h, w, n, ci, g, CX, CX, s_lo0, s_lo1);
     __syncthreads();
     const int tid = threadIdx.x;
     const int x = x0 + tid;
     const bool xin = x < x1;
     const Lerp lx = make_lerp(rx, xin ? x : x0, w);
     const int j0 = lx.i0 - g.jbase, j1 = lx.i1 - g.jbase;
-#pragma unroll
-    for (int c = 0; c < CX; ++c) {
-        sT0[c * kPitchX + tid] = lerp_h(lx, s_lo0[j0 * CX + c], s_lo0[j1 * CX + c]);
-        sT1[c * kPitchX + tid] = lerp_h(lx, s_lo1[j0 * CX + c], s_lo1[j1 * CX + c]);
-    }
+    blend_rows(lx, j0, j1, s_lo0, s_lo1, CX, CX, 0, 1, CX, sT0, sT1, [&](int c) { return c * kPitch + tid; });
     long long lab_next = xin ? labels[((long long)n * H + g.y_lo) * W + x] : 0;
     for (int y = g.y_lo; y <= g.y_hi; ++y) {
         const long long lab = lab_next;
@@ -604,7 +544,7 @@ ohem_ptarget_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, con
         const int t = valid ? (int)lab : 0;
         float v[CX];
 #pragma unroll
-        for (int c = 0; c < CX; ++c) v[c] = lerp_v(ly, sT0[c * kPitchX + tid], sT1[c * kPitchX + tid]);
+        for (int c = 0; c < CX; ++c) v[c] = lerp_v(ly, sT0[c * kPitch + tid], sT1[c * kPitch + tid]);
         float m = v[0];
 #pragma unroll
         for (int c = 1; c < CX; ++c) m = fmaxf(m, v[c]);
@@ -612,7 +552,7 @@ ohem_ptarget_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, con
 #pragma unroll
         for (int c = 0; c < CX; ++c) ssum = __fadd_rn(ssum, tsb_exp_det(__fsub_rn(v[c], m)));
         // target class: same operands, same operations as v[t] above → identical bits
-        const float xt = lerp_v(ly, sT0[t * kPitchX + tid], sT1[t * kPitchX + tid]);
+        const float xt = lerp_v(ly, sT0[t * kPitch + tid], sT1[t * kPitch + tid]);
         const float et = tsb_exp_det(__fsub_rn(xt, m));
         const float p_t = __fdiv_rn(et, ssum);
         const float nl = logf(ssum) - (xt - m);
@@ -627,10 +567,10 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
                       const float* __restrict__ p, int N, int H, int W, int ignore_label, const float* __restrict__ cw,
                       const uint32_t* __restrict__ state, const float* __restrict__ gscale, float* __restrict__ dlo,
                       int maxcols, int phase) {
-    extern __shared__ float s_dyn_x[];   // sT0 / s_g0 [CX][kPitchX] | sT1 / s_g1 | s_lo0 | s_lo1
+    extern __shared__ float s_dyn_x[];   // sT0 / s_g0 [CX][kPitch] | sT1 / s_g1 | s_lo0 | s_lo1
     float* sT0 = s_dyn_x;
-    float* sT1 = s_dyn_x + CX * kPitchX;
-    float* s_lo0 = s_dyn_x + 2 * CX * kPitchX;
+    float* sT1 = s_dyn_x + CX * kPitch;
+    float* s_lo0 = s_dyn_x + 2 * CX * kPitch;
     float* s_lo1 = s_lo0 + maxcols * CX;
     __shared__ float s_l0[kStrip], s_l1[kStrip];
     __shared__ short s_seg[kStrip + 8];
@@ -644,31 +584,18 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
     if (ci >= h || x0 >= W) return;
     const int x1 = min(W, x0 + kStrip);
     const int nx = x1 - x0;
-    const int i1 = ci + (ci < h - 1 ? 1 : 0);
-    const BandGeom g = band_geom(ry, rx, ci, x0, x1, H, w);
+    const BandGeom g = band_geom(ry, rx, ci, x0, x1, h, H, w);
     if (g.ncols > maxcols) __trap();
-    for (int q = threadIdx.x; q < 2 * g.ncols * CX; q += kThreads) {
-        const int c = q % CX, t2 = q / CX, col = t2 % g.ncols, row = t2 / g.ncols;
-        (row ? s_lo1 : s_lo0)[col * CX + c] = __ldg(lo + (((long long)n * h + (row ? i1 : ci)) * w + g.jbase + col) * cs + c);
-    }
+    stage_rows<kThreads>(lo, cs, h, w, n, ci, g, CX, CX, s_lo0, s_lo1);
     const int tid = threadIdx.x;
     const int x = x0 + tid;
     const bool xin = x < x1;
     const Lerp lx = make_lerp(rx, xin ? x : x0, w);
     const int j0 = lx.i0 - g.jbase, j1 = lx.i1 - g.jbase;
-    s_l0[tid] = xin ? lx.l0 : 0.f;
-    s_l1[tid] = xin ? lx.l1 : 0.f;
-    for (int q = tid; q < g.ncols + 2; q += kThreads) s_seg[q] = (short)nx;
+    seg_init<kThreads>(s_l0, s_l1, s_seg, tid, true, xin, lx, g.ncols, nx);
     __syncthreads();
-    if (xin) {
-        const int jprev = (tid == 0) ? -1 : (make_lerp(rx, x - 1, w).i0 - g.jbase);
-        for (int jj = jprev + 1; jj <= j0; ++jj) s_seg[jj] = (short)tid;
-    }
-#pragma unroll
-    for (int c = 0; c < CX; ++c) {
-        sT0[c * kPitchX + tid] = lerp_h(lx, s_lo0[j0 * CX + c], s_lo0[j1 * CX + c]);
-        sT1[c * kPitchX + tid] = lerp_h(lx, s_lo1[j0 * CX + c], s_lo1[j1 * CX + c]);
-    }
+    seg_fill(s_seg, tid, true, xin, rx, x, w, g.jbase, j0);
+    blend_rows(lx, j0, j1, s_lo0, s_lo1, CX, CX, 0, 1, CX, sT0, sT1, [&](int c) { return c * kPitch + tid; });
     // ---- phase 1: per-thread accumulation over the rows of the band
     float G0[CX], G1[CX];
 #pragma unroll
@@ -696,7 +623,7 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
         const float wt = (cw ? __ldg(cw + t) : 1.f) * scale;
         float v[CX];
 #pragma unroll
-        for (int c = 0; c < CX; ++c) v[c] = lerp_v(ly, sT0[c * kPitchX + tid], sT1[c * kPitchX + tid]);
+        for (int c = 0; c < CX; ++c) v[c] = lerp_v(ly, sT0[c * kPitch + tid], sT1[c * kPitch + tid]);
         float m = v[0];
 #pragma unroll
         for (int c = 1; c < CX; ++c) m = fmaxf(m, v[c]);
@@ -715,48 +642,35 @@ ohem_grad_up_x_kernel(const float* __restrict__ lo, int cs, int h, int w, const 
     }
     // hand-over to phase 2 in place: column `tid` of sT0 / sT1 was only ever read by this thread
 #pragma unroll
-    for (int c = 0; c < CX; ++c) { sT0[c * kPitchX + tid] = G0[c]; sT1[c * kPitchX + tid] = G1[c]; }
+    for (int c = 0; c < CX; ++c) { sT0[c * kPitch + tid] = G0[c]; sT1[c * kPitch + tid] = G1[c]; }
     __syncthreads();
-    // ---- phase 2 (once per band): low-res column j receives the l0x-weighted sum of its own segment and the
-    //      l1x-weighted sum of the previous segment (or of its own when the stencil is clamped at the last column)
+    // ---- phase 2 (once per band)
     const int npairs = g.ncols * CX;
     for (int q = tid; q < npairs; q += kThreads) {
         const int j = q / CX, c = q - j * CX;
-        const float* g0 = sT0 + c * kPitchX;
-        const float* g1 = sT1 + c * kPitchX;
-        const int a0 = s_seg[j], a1 = s_seg[j + 1];
-        float top = 0.f, bot = 0.f;
-        for (int xx = a0; xx < a1; ++xx) {
-            const float wl = s_l0[xx];
-            top = fmaf(wl, g0[xx], top);
-            bot = fmaf(wl, g1[xx], bot);
-        }
-        const bool clamped = (g.jbase + j == w - 1);
-        const int b0 = clamped ? a0 : (j > 0 ? (int)s_seg[j - 1] : 0);
-        const int b1 = clamped ? a1 : (j > 0 ? a0 : 0);
-        for (int xx = b0; xx < b1; ++xx) {
-            const float wr = s_l1[xx];
-            top = fmaf(wr, g0[xx], top);
-            bot = fmaf(wr, g1[xx], bot);
-        }
-        if (clamped && j > 0) {
-            for (int xx = s_seg[j - 1]; xx < a0; ++xx) {
-                const float wr = s_l1[xx];
-                top = fmaf(wr, g0[xx], top);
-                bot = fmaf(wr, g1[xx], bot);
-            }
-        }
-        if (top != 0.f) dlo[(((long long)n * h + ci) * w + g.jbase + j) * cs + c] += top;
-        if (bot != 0.f) dlo[(((long long)n * h + i1) * w + g.jbase + j) * cs + c] += bot;
+        const float2 s = col_sums(sT0, sT1, [&](int xx) { return c * kPitch + xx; }, s_seg, s_l0, s_l1, g, w, j, 0.f, 0.f);
+        if (s.x != 0.f) dlo[(((long long)n * h + ci) * w + g.jbase + j) * cs + c] += s.x;
+        if (s.y != 0.f) dlo[(((long long)n * h + g.i1) * w + g.jbase + j) * cs + c] += s.y;
     }
 }
 
-}  // namespace
+// materialised pair: C <= 32 holds a pixel's logits in registers, larger C runs the any-C kernels (CMAX = 0)
+template <typename T>
+void ptarget_launch(int grid, cudaStream_t st, const void* logits, long long sn, long long sc, long long sy, long long sx,
+                    const int64_t* labels, int N, int C, int H, int W, int ignore_label, float thresh, float* p,
+                    float* nll, uint32_t* state) {
+    auto kernel = C <= 32 ? ohem_ptarget_kernel<T, 32> : ohem_ptarget_kernel<T, 0>;
+    kernel<<<grid, kThreads, 0, st>>>((const T*)logits, sn, sc, sy, sx, labels, N, C, H, W, ignore_label, thresh, p, nll, state);
+}
+template <typename T>
+void grad_launch(int grid, cudaStream_t st, const void* logits, long long sn, long long sc, long long sy, long long sx,
+                 const int64_t* labels, const float* p, int N, int C, int H, int W, int ignore_label, const float* cw,
+                 const uint32_t* state, const float* gscale, void* dlogits) {
+    auto kernel = C <= 32 ? ohem_grad_kernel<T, 32> : ohem_grad_kernel<T, 0>;
+    kernel<<<grid, kThreads, 0, st>>>((const T*)logits, sn, sc, sy, sx, labels, p, N, C, H, W, ignore_label, cw, state, gscale, (T*)dlogits);
+}
 
-// Generic band kernels (class counts other than 19 / 21): the gradient kernel forms the horizontally blended source
-// rows once per band and keeps them in registers (measured 2.16 -> 1.85 ms/step); the p_target kernel blends them again
-// for every row, because keeping them costs it 111 registers, which halves the occupancy of an issue-bound kernel
-// (measured 1.72 -> 1.85 ms when kept).
+}  // namespace
 
 // =============================================================================================
 // C ABI
@@ -773,27 +687,13 @@ extern "C" int tsb_ohem_ptarget(const void* logits, int dtype, long long sn, lon
     TSB_REQUIRE(logits && labels && p && nll && state, "tsb_ohem_ptarget: null pointer");
     TSB_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0, "tsb_ohem_ptarget: bad shape");
     TSB_REQUIRE(dtype == TSB_F32 || dtype == TSB_BF16, "tsb_ohem_ptarget: bad dtype");
-    long long total = (long long)N * H * W;
-    int grid = tsb_grid_for(total, kThreads, 8);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (C <= 32) {
-        if (dtype == TSB_F32)
-            ohem_ptarget_kernel<float, 32><<<grid, kThreads, 0, st>>>((const float*)logits, sn, sc, sy, sx, labels, N, C, H, W, ignore_label, thresh, p, nll, state);
-        else
-            ohem_ptarget_kernel<__nv_bfloat16, 32><<<grid, kThreads, 0, st>>>((const __nv_bfloat16*)logits, sn, sc, sy, sx, labels, N, C, H, W, ignore_label, thresh, p, nll, state);
-    } else {
-        if (dtype == TSB_F32)
-            ohem_ptarget_kernel_anyc<float><<<grid, kThreads, 0, st>>>((const float*)logits, sn, sc, sy, sx, labels, N, C, H, W, ignore_label, thresh, p, nll, state);
-        else
-            ohem_ptarget_kernel_anyc<__nv_bfloat16><<<grid, kThreads, 0, st>>>((const __nv_bfloat16*)logits, sn, sc, sy, sx, labels, N, C, H, W, ignore_label, thresh, p, nll, state);
-    }
+    const int grid = tsb_grid_for((long long)N * H * W, kThreads, 8);
+    if (dtype == TSB_F32)
+        ptarget_launch<float>(grid, (cudaStream_t)stream, logits, sn, sc, sy, sx, labels, N, C, H, W, ignore_label, thresh, p, nll, state);
+    else
+        ptarget_launch<__nv_bfloat16>(grid, (cudaStream_t)stream, logits, sn, sc, sy, sx, labels, N, C, H, W, ignore_label, thresh, p, nll, state);
     TSB_CUDA_CHECK_LAUNCH("ohem_ptarget");
     return TSB_OK;
-}
-
-namespace {
-// low-res columns one strip can touch
-inline int band_maxcols(int w, int W) { return (int)(((long long)kStrip * w + W - 1) / W) + 3; }
 }
 
 extern "C" int tsb_ohem_ptarget_up(const float* logits_lo, int cs, int h, int w, const int64_t* labels, int N, int C,
@@ -803,19 +703,16 @@ extern "C" int tsb_ohem_ptarget_up(const float* logits_lo, int cs, int h, int w,
     TSB_REQUIRE(N > 0 && C > 0 && C <= 32 && cs >= C && H > 0 && W > 0 && h > 0 && w > 0,
                 "tsb_ohem_ptarget_up: bad shape (C must be <= 32)");
     TSB_REQUIRE(N <= 65535 && h <= 65535, "tsb_ohem_ptarget_up: N and h must fit a grid dimension");
-    const int maxcols = band_maxcols(w, W);
-    dim3 grid((W + kStrip - 1) / kStrip, h, N);
+    const int maxcols = band_maxcols(kStrip, w, W);
+    const dim3 grid((W + kStrip - 1) / kStrip, h, N);
+    const cudaStream_t st = (cudaStream_t)stream;
     if (C == 19 || C == 21) {      // exact-class-count kernels (Cityscapes / VOC)
-        const size_t smx = sizeof(float) * (2 * (size_t)C * kPitchX + 2 * (size_t)maxcols * C);
+        const size_t smx = sizeof(float) * (2 * (size_t)C * kPitch + 2 * (size_t)maxcols * C);
         if (smx <= 100 * 1024) {
-#define LX(CX)                                                                                                      \
-    do {                                                                                                            \
-        int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(ohem_ptarget_up_x_kernel<CX>), smx);            \
-        if (rc_) return rc_;                                                                                        \
-        ohem_ptarget_up_x_kernel<CX><<<grid, kThreads, smx, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, N, H, W, ignore_label, thresh, p, nll, state, maxcols); \
-    } while (0)
-            if (C == 19) LX(19); else LX(21);
-#undef LX
+            auto kernel = C == 19 ? ohem_ptarget_up_x_kernel<19> : ohem_ptarget_up_x_kernel<21>;
+            int rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(kernel), smx);
+            if (rc) return rc;
+            kernel<<<grid, kThreads, smx, st>>>(logits_lo, cs, h, w, labels, N, H, W, ignore_label, thresh, p, nll, state, maxcols);
             TSB_CUDA_CHECK_LAUNCH("ohem_ptarget_up_x");
             return TSB_OK;
         }
@@ -823,9 +720,8 @@ extern "C" int tsb_ohem_ptarget_up(const float* logits_lo, int cs, int h, int w,
     const int cmax = C <= 20 ? 20 : 32;
     const size_t smem = sizeof(float) * 2 * (size_t)maxcols * cmax;
     TSB_REQUIRE(smem <= 28 * 1024, "tsb_ohem_ptarget_up: up-scale factor W/w too small for the band kernel");
-#define L(CM) ohem_ptarget_up_kernel<CM><<<grid, kThreads, smem, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, N, C, H, W, ignore_label, thresh, p, nll, state, maxcols)
-    if (C <= 20) L(20); else L(32);
-#undef L
+    auto kernel = C <= 20 ? ohem_ptarget_up_kernel<20> : ohem_ptarget_up_kernel<32>;
+    kernel<<<grid, kThreads, smem, st>>>(logits_lo, cs, h, w, labels, N, C, H, W, ignore_label, thresh, p, nll, state, maxcols);
     TSB_CUDA_CHECK_LAUNCH("ohem_ptarget_up");
     return TSB_OK;
 }
@@ -864,18 +760,11 @@ extern "C" int tsb_ohem_grad(const void* logits, int dtype, long long sn, long l
                              tsb_stream_t stream) {
     TSB_REQUIRE(logits && labels && p && state && dlogits, "tsb_ohem_grad: null pointer");
     TSB_REQUIRE(dtype == TSB_F32 || dtype == TSB_BF16, "tsb_ohem_grad: bad dtype");
-    long long total = (long long)N * H * W;
-    int grid = tsb_grid_for(total, kThreads, 8);
-    cudaStream_t st = (cudaStream_t)stream;
-#define TSB_LAUNCH_GRAD(T, CM)                                                                                   \
-    ohem_grad_kernel<T, CM><<<grid, kThreads, 0, st>>>((const T*)logits, sn, sc, sy, sx, labels, p, N, C, H, W,  \
-                                                       ignore_label, class_weight, state, gscale, (T*)dlogits)
-    if (C <= 32) {
-        if (dtype == TSB_F32) TSB_LAUNCH_GRAD(float, 32); else TSB_LAUNCH_GRAD(__nv_bfloat16, 32);
-    } else {
-        if (dtype == TSB_F32) TSB_LAUNCH_GRAD(float, 0); else TSB_LAUNCH_GRAD(__nv_bfloat16, 0);
-    }
-#undef TSB_LAUNCH_GRAD
+    const int grid = tsb_grid_for((long long)N * H * W, kThreads, 8);
+    if (dtype == TSB_F32)
+        grad_launch<float>(grid, (cudaStream_t)stream, logits, sn, sc, sy, sx, labels, p, N, C, H, W, ignore_label, class_weight, state, gscale, dlogits);
+    else
+        grad_launch<__nv_bfloat16>(grid, (cudaStream_t)stream, logits, sn, sc, sy, sx, labels, p, N, C, H, W, ignore_label, class_weight, state, gscale, dlogits);
     TSB_CUDA_CHECK_LAUNCH("ohem_grad");
     return TSB_OK;
 }
@@ -886,38 +775,31 @@ extern "C" int tsb_ohem_grad_up(const float* logits_lo, int cs, int h, int w, co
     TSB_REQUIRE(logits_lo && labels && p && state && dlogits_lo, "tsb_ohem_grad_up: null pointer");
     TSB_REQUIRE(C > 0 && C <= 32 && cs >= C, "tsb_ohem_grad_up: C must be <= 32");
     TSB_REQUIRE(N <= 65535 && h <= 65535, "tsb_ohem_grad_up: N and h must fit a grid dimension");
-    const int maxcols = band_maxcols(w, W);
+    const int maxcols = band_maxcols(kStrip, w, W);
     TSB_REQUIRE(maxcols <= kStrip, "tsb_ohem_grad_up: up-scale factor W/w too small for the band kernel");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (C == 19 || C == 21) {
-        const size_t smx = sizeof(float) * (2 * (size_t)C * kPitchX + 2 * (size_t)maxcols * C);
+        const size_t smx = sizeof(float) * (2 * (size_t)C * kPitch + 2 * (size_t)maxcols * C);
         if (smx <= 72 * 1024) {
-            dim3 gridx(((W + kStrip - 1) / kStrip + 1) / 2, (h + 1) / 2, N);
-#define GX(CX)                                                                                                      \
-    do {                                                                                                            \
-        int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(ohem_grad_up_x_kernel<CX>), smx);               \
-        if (rc_) return rc_;                                                                                        \
-        for (int ph = 0; ph < 4; ++ph) {                                                                            \
-            ohem_grad_up_x_kernel<CX><<<gridx, kThreads, smx, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, p, N, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols, ph); \
-            TSB_CUDA_CHECK_LAUNCH("ohem_grad_up_x");                                                               \
-        }                                                                                                           \
-    } while (0)
-            if (C == 19) GX(19); else GX(21);
-#undef GX
+            const dim3 gridx(((W + kStrip - 1) / kStrip + 1) / 2, (h + 1) / 2, N);
+            auto kernel = C == 19 ? ohem_grad_up_x_kernel<19> : ohem_grad_up_x_kernel<21>;
+            int rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(kernel), smx);
+            if (rc) return rc;
+            for (int ph = 0; ph < 4; ++ph) {
+                kernel<<<gridx, kThreads, smx, st>>>(logits_lo, cs, h, w, labels, p, N, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols, ph);
+                TSB_CUDA_CHECK_LAUNCH("ohem_grad_up_x");
+            }
             return TSB_OK;
         }
     }
     const int cmax = C <= 20 ? 20 : 32;
-    const size_t smem = sizeof(float) * (2 * (size_t)cmax * (kStrip + 1) + 2 * (size_t)maxcols * cmax);
+    const size_t smem = sizeof(float) * (2 * (size_t)cmax * kPitch + 2 * (size_t)maxcols * cmax);
     TSB_REQUIRE(smem <= 96 * 1024, "tsb_ohem_grad_up: shared memory budget exceeded");
-    dim3 grid((W + kStrip - 1) / kStrip, h, N);
-    cudaStream_t st = (cudaStream_t)stream;
-#define L(CM)                                                                                                           \
-    do {                                                                                                                \
-        { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(ohem_grad_up_kernel<CM>), smem); if (rc_) return rc_; } \
-        ohem_grad_up_kernel<CM><<<grid, kThreads, smem, st>>>(logits_lo, cs, h, w, labels, p, N, C, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols); \
-    } while (0)
-    if (C <= 20) L(20); else L(32);
-#undef L
+    const dim3 grid((W + kStrip - 1) / kStrip, h, N);
+    auto kernel = C <= 20 ? ohem_grad_up_kernel<20> : ohem_grad_up_kernel<32>;
+    int rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(kernel), smem);
+    if (rc) return rc;
+    kernel<<<grid, kThreads, smem, st>>>(logits_lo, cs, h, w, labels, p, N, C, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols);
     TSB_CUDA_CHECK_LAUNCH("ohem_grad_up");
     return TSB_OK;
 }
