@@ -241,9 +241,12 @@ int tsb_transpose_pad(const void* in, int idtype, int ics, void* out_bf16, int o
  * conv3x3 (resnet.py:11-14), the 1x1 heads (bisenet network.py:156-161) and their cuDNN
  * dgrad / wgrad. bf16 operands, fp32 accumulation.
  *
- * x : bf16 NHWC [N,H,W,C] (channel stride xcs, C % 64 == 0)
+ * x : bf16 NHWC [N,H,W,C] (channel stride xcs >= C, C % 64 == 0)
  * w : bf16 [K,R,S,C] (tsb_pack_weight)   — fprop;  wt: bf16 [C,R,S,K] flipped — dgrad
- * y : NHWC [N,P,Q,*] with channel stride ycs; dtype BF16 or F32; K_store channels written
+ * y : NHWC [N,P,Q,*] with channel stride ycs >= K; dtype BF16 or F32; K_store = ceil8(K) channels written, those
+ *     past K as zeros
+ * Every activation may be a channel slice of a wider buffer: its pointer 16-byte aligned (a multiple of 8 bf16
+ * channels), its channel stride a multiple of 8. Channels past C (past K for dy) are never read.
  * ============================================================================================== */
 typedef struct {
     int N, H, W, C;          /* input  */
@@ -261,15 +264,20 @@ int tsb_conv2d_fprop(const tsb_conv_shape* s, const void* x, int xcs, const void
  * res (optional, bf16) must be laid out exactly like y (rescs == ycs): the shortcut of a residual block. */
 int tsb_conv2d_fprop_fused(const tsb_conv_shape* s, const void* x, int xcs, const void* w, const float* bias,
                            const void* res, int rescs, int relu, void* y, int ydtype, int ycs, tsb_stream_t stream);
-/* dgrad: dx = conv_transpose(dy, w). wt is the flipped-transposed pack. dx bf16 (channel stride dxcs).
- * If accumulate != 0, dx += result (residual / multi-consumer gradient accumulation in the epilogue). */
+/* dgrad: dx = conv_transpose(dy, w). wt is the flipped-transposed pack. K % 64 == 0, dycs >= K; C % 8 == 0, dx bf16
+ * (channel stride dxcs >= C; channels [C, dxcs) are not written). If accumulate != 0, dx += result (residual /
+ * multi-consumer gradient accumulation in the epilogue); a stride-2 1x1 leaves the positions no tap reaches as they
+ * were, and writes zeros there when accumulate == 0. */
 int tsb_conv2d_dgrad(const tsb_conv_shape* s, const void* dy, int dycs, const void* wt, void* dx, int dxcs,
                      int accumulate, tsb_stream_t stream);
-/* wgrad: dw[K,R,S,C] (fp32, KRSC) += Σ_pixels dy ⊗ x  (red.global.add.f32; caller zeroes or accumulates) */
+/* wgrad: dw[K,R,S,C] (fp32, KRSC) += Σ_pixels dy ⊗ x (caller zeroes or accumulates); xcs >= C, dycs >= K (any K).
+ * The per-split partial sums go to ws and are added in a fixed order, so the result is bit-reproducible; without a
+ * workspace large enough for two splits the kernel adds into dw in place. */
 int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs, const void* dy, int dycs, float* dw, float* ws,
                      long long ws_floats, tsb_stream_t stream);
 /* stride-2 C_in=3 stem (7x7 pad 3 or 3x3 pad 1, same packed weight format) on the s2d-packed image (tsb_pack_image_s2d / tsb_pack_stem_weight):
- * xs2d [N,H/2,W/2+4,16] bf16, wp [K,4,4,16] bf16 → y [N,H/2,W/2,K]. */
+ * xs2d [N,H/2,W/2+4,16] bf16, wp [K,4,4,16] bf16 → y [N,H/2,W/2,K] (K % 8 == 0, channel stride ycs >= K, exactly K
+ * channels written). wgrad: dy with channel stride dycs >= K → dwp [K,4,64] fp32 (+=; tsb_unpack_stem_wgrad). */
 int tsb_conv_stem_fprop(const void* xs2d, int N, int H, int W, const void* wp, int K, void* y, int ycs, float* sum,
                         float* sumsq, float* ws, long long ws_floats, tsb_stream_t stream);
 int tsb_conv_stem_fprop_fused(const void* xs2d, int N, int H, int W, const void* wp, int K, const float* bias, int relu,

@@ -241,23 +241,29 @@ def test_stem_odd_image_size(cuda, HW, R):
 @pytest.mark.parametrize("case", [(2, 64, 32, 32, 64, 3, 1, 1, 1), (1, 64, 7, 260, 128, 3, 2, 1, 1),
                                   (2, 256, 16, 16, 256, 1, 1, 0, 1)], ids=["taps", "rows", "generic"])
 def test_wgrad_without_workspace_adds_in_place(cuda, case):
-    """with no reduction workspace the weight gradient runs as one pixel split that adds straight into dW: same result as
-    the split path (up to summation order), and it accumulates onto what dW already holds"""
+    """with no reduction workspace the weight gradient runs as one pixel split that adds straight into dW. On integer
+    operands (|x|, |dy| <= 2, an integer base: every partial sum is an exact fp32 integer) it equals the split path and
+    float64 exactly, and it accumulates onto what dW already holds"""
     import ctypes
     from torchseg_b200 import ops
     N, C, H, W, K, R, stride, pad, dil = case
     g = torch.Generator(device="cuda").manual_seed(14)
     P, Q = ops.conv_out_size(H, R, stride, pad, dil), ops.conv_out_size(W, R, stride, pad, dil)
-    x = ops.to_nhwc(torch.randn(N, C, H, W, device=cuda, generator=g))
-    gy = ops.to_nhwc(torch.randn(N, K, P, Q, device=cuda, generator=g))
+    assert (N * P * Q * 4 + 64) < 2 ** 24
+    x = torch.randint(-2, 3, (N, C, H, W), device=cuda, generator=g).double()
+    gy = torch.randint(-2, 3, (N, K, P, Q), device=cuda, generator=g).double()
+    w = torch.zeros((K, C, R, R), dtype=torch.float64, device=cuda, requires_grad=True)
+    F.conv2d(x, w, None, stride, pad, dil).backward(gy)
+    xd, gyd = ops.to_nhwc(x), ops.to_nhwc(gy)
     ref = torch.zeros((K, R, R, C), dtype=torch.float32, device=cuda)
-    ops.conv_wgrad(x, gy, K, R, stride, pad, dil, ref)
-    base = torch.randn((K, R, R, C), device=cuda, generator=g)
+    ops.conv_wgrad(xd, gyd, K, R, stride, pad, dil, ref)
+    assert torch.equal(ref.permute(0, 3, 1, 2), w.grad.float()), "split wgrad differs"
+    base = torch.randint(-64, 65, (K, R, R, C), device=cuda, generator=g).float()
     dw = base.clone()
     shp = ops.make_shape(N, H, W, C, K, R, stride, pad, dil)
-    ops.call("tsb_conv2d_wgrad", ctypes.byref(shp), ops.ptr(x), ops.cs_of(x), ops.ptr(gy), ops.cs_of(gy), ops.ptr(dw), None, 0,
-             ops.stream())
-    assert rel_err(dw - base, ref) < 1e-4
+    ops.call("tsb_conv2d_wgrad", ctypes.byref(shp), ops.ptr(xd), ops.cs_of(xd), ops.ptr(gyd), ops.cs_of(gyd), ops.ptr(dw),
+             None, 0, ops.stream())
+    assert torch.equal(dw, base + ref), "in-place wgrad differs"
 
 
 def test_conv_statistics_need_a_workspace(cuda):

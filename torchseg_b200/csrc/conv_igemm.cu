@@ -160,7 +160,8 @@ static int fprop_impl(const tsb_conv_shape* s, const void* x, int xcs, const voi
     TSB_REQUIRE(s->C % 64 == 0, "tsb_conv2d_fprop: C must be a multiple of 64 (got %d)", s->C);
     TSB_REQUIRE(xcs % 8 == 0 && xcs >= s->C && tsb_aligned16(x) && tsb_aligned16(w), "tsb_conv2d_fprop: x alignment");
     TSB_REQUIRE(ydtype == TSB_BF16 || ydtype == TSB_F32, "tsb_conv2d_fprop: bad ydtype");
-    TSB_REQUIRE(ycs % 8 == 0 && tsb_aligned16(y), "tsb_conv2d_fprop: y channel stride must be a multiple of 8");
+    TSB_REQUIRE(ycs % 8 == 0 && ycs >= s->K && tsb_aligned16(y),
+                "tsb_conv2d_fprop: y channel stride must be a multiple of 8 and at least K (got ycs %d, K %d)", ycs, s->K);
     TSB_REQUIRE((sum == nullptr) == (sumsq == nullptr), "tsb_conv2d_fprop: sum and sumsq go together");
     TSB_REQUIRE(!(sum && ydtype != TSB_BF16), "tsb_conv2d_fprop: statistics need bf16 output");
     cudaStream_t st = (cudaStream_t)stream;
@@ -175,8 +176,7 @@ static int fprop_impl(const tsb_conv_shape* s, const void* x, int xcs, const voi
     convv2::Desc d;
     memset(&d, 0, sizeof(d));
     const int nt = forward_taps(s, d.taps);
-    int kst = (s->K + 7) / 8 * 8;
-    if (kst > ycs) kst = ycs;
+    const int kst = (s->K + 7) / 8 * 8;   // <= ycs: ycs is a multiple of 8 and at least K
     d.act = x; d.aN = N; d.aH = H; d.aW = W; d.aC = s->C; d.acs = xcs; d.act_stride = s->stride; d.flat = flat;
     d.ntaps = nt; d.kchunks = s->C / 64;
     d.w = w; d.w_rows = s->K; d.w_k = (long long)s->R * s->S * s->C; d.ncols = kst;
@@ -301,8 +301,8 @@ extern "C" int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs,
     if (rc) return rc;
     TSB_REQUIRE(x && dy && dw, "tsb_conv2d_wgrad: null pointer");
     TSB_REQUIRE(s->C % 64 == 0, "tsb_conv2d_wgrad: C must be a multiple of 64 (got %d)", s->C);
-    TSB_REQUIRE(xcs % 8 == 0 && dycs % 8 == 0 && dycs >= s->K && tsb_aligned16(x) && tsb_aligned16(dy) && tsb_aligned16(dw),
-                "tsb_conv2d_wgrad: alignment");
+    TSB_REQUIRE(xcs % 8 == 0 && xcs >= s->C && dycs % 8 == 0 && dycs >= s->K && tsb_aligned16(x) && tsb_aligned16(dy) &&
+                tsb_aligned16(dw), "tsb_conv2d_wgrad: layout (xcs >= C, dycs >= K, multiples of 8, 16-byte aligned)");
     cudaStream_t st = (cudaStream_t)stream;
     int N = s->N, H = s->H, W = s->W, P = s->P, Q = s->Q;
     const bool flat = (s->R == 1 && s->stride == 1 && s->pad == 0);
@@ -348,7 +348,8 @@ extern "C" int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs,
 static int stem_fprop_impl(const void* xs2d, int N, int H, int W, const void* wp, int K, void* y, int ycs, float* sum,
                            float* sumsq, float* ws, long long ws_floats, const float* bias, int relu, tsb_stream_t stream) {
     TSB_REQUIRE(xs2d && wp && y && N > 0 && H > 0 && W > 0 && K > 0, "tsb_conv_stem_fprop: bad args");
-    TSB_REQUIRE(H % 2 == 0 && W % 2 == 0 && ycs % 8 == 0 && K % 8 == 0, "tsb_conv_stem_fprop: H,W even; K, ycs multiples of 8");
+    TSB_REQUIRE(H % 2 == 0 && W % 2 == 0 && ycs % 8 == 0 && K % 8 == 0 && ycs >= K,
+                "tsb_conv_stem_fprop: H,W even; K, ycs multiples of 8; ycs >= K");
     TSB_REQUIRE((sum == nullptr) == (sumsq == nullptr), "tsb_conv_stem_fprop: sum and sumsq go together");
     const int H2 = H / 2, W2 = W / 2;
     convv2::Desc d;
@@ -379,7 +380,8 @@ extern "C" int tsb_conv_stem_fprop_fused(const void* xs2d, int N, int H, int W, 
 extern "C" int tsb_conv_stem_wgrad(const void* xs2d, int N, int H, int W, const void* dy, int dycs, int K, float* dwp,
                                    float* ws, long long ws_floats, tsb_stream_t stream) {
     TSB_REQUIRE(xs2d && dy && dwp && N > 0 && H > 0 && W > 0 && K > 0, "tsb_conv_stem_wgrad: bad args");
-    TSB_REQUIRE(H % 2 == 0 && W % 2 == 0 && dycs % 8 == 0 && K % 8 == 0, "tsb_conv_stem_wgrad: H,W even; K, dycs multiples of 8");
+    TSB_REQUIRE(H % 2 == 0 && W % 2 == 0 && dycs % 8 == 0 && K % 8 == 0 && dycs >= K,
+                "tsb_conv_stem_wgrad: H,W even; K, dycs multiples of 8; dycs >= K");
     const int H2 = H / 2, W2 = W / 2;
     WgParams prm;
     memset(&prm, 0, sizeof(prm));
