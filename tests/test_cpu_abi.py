@@ -86,6 +86,13 @@ def test_argument_validation_without_gpu(lib):
         ("tsb_chan_scale_bwd", (A, C, A, 8, A, 1.0, A, C, A, 1, npix, C, A, WS, None), b">= C"),
         ("tsb_cast_scale", (A, 1, C, A, 1, 8, npix, C, None, None), b">= C"),
         ("tsb_bias_grad", (A, 16, npix, 19, A, A, WS, None), b">= K"),
+        # C = 0 (and N = 0) would reach the host-side geometry of the column reductions as a divisor
+        ("tsb_bn_stats", (A, C, npix, 0, A, A, A, WS, None), b"multiples of 8"),
+        ("tsb_bn_bwd_reduce", (A, C, None, 0, A, C, A, A, 0, npix, 0, A, A, None, None, A, WS, None), b"multiples of 8"),
+        ("tsb_chan_scale_bwd", (A, C, A, C, A, 1.0, A, C, A, 1, npix, 0, A, WS, None), b"multiples of 8"),
+        ("tsb_adaptive_avgpool_fwd", (A, C, 1, 0, 4, 4, 2, A, A, WS, None), b"multiples of 8"),
+        ("tsb_adaptive_avgpool_fwd", (A, C, 0, C, 4, 4, 2, A, A, WS, None), b"N <= 0"),
+        ("tsb_bilinear_fwd_nhwc_to_nchw", (A, 1, 8, A, 1, C, 2, 2, 4, 4, None), b"ics >= C"),
     ]
     for name in ("tsb_add", "tsb_add_relu", "tsb_relu_bwd"):
         cases += [(name, (A, C, M, C, A, C, npix, C, None), b"16B aligned"),

@@ -6,8 +6,6 @@
 #include "nhwc_vec.cuh"
 
 namespace {
-constexpr int kThreads = 256;
-
 // Per-CTA partial sums go to slot blockIdx.x of the deterministic workspace (tsb_det_reduce sums the slots in order).
 __device__ __forceinline__ void store_part_v4(float* base, long long stride, float a, float b, float c, float d) {
     *reinterpret_cast<float4*>(base + blockIdx.x * stride) = make_float4(a, b, c, d);
@@ -40,8 +38,7 @@ __device__ __forceinline__ void column_reduce(long long npix, int C8, float* con
                 for (int k = 0; k < 8; ++k) s_buf[((lane * groups + g) * NACC + a) * 8 + k] = acc[a][k];
         }
         __syncthreads();
-        // thread (lane, g) finishes accumulator slots striped over lanes
-        // (16-byte vector reductions: a quarter of the atomic operations that all CTAs send to the same few L2 slices)
+        // thread (lane, g) sums accumulator quads striped over lanes and stores each into this CTA's workspace slot
         if (cg < C8 && lane < lanes) {
             for (int quad = lane; quad < NACC * 2; quad += lanes) {
                 float s[4] = {0.f, 0.f, 0.f, 0.f};
@@ -349,11 +346,7 @@ __global__ void __launch_bounds__(kThreads)
 chan_scale_fwd_kernel(const __nv_bfloat16* __restrict__ x, int xcs, const float* __restrict__ a, float base,
                       const __nv_bfloat16* __restrict__ add, int acs, __nv_bfloat16* __restrict__ y, int ycs, int HW,
                       int C8, long long total) {
-    const long long stride = (long long)gridDim.x * kThreads;
-    VecWalk wk(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride);
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += stride, wk.next()) {
-        const int c8 = wk.c8;
-        const long long p = wk.p;
+    for_each_vec(total, C8, [&](long long p, int c8) {
         int n = (int)(p / HW);
         float v[8], av[8];
         Vec8<__nv_bfloat16>::load(x + p * xcs + c8 * 8, v);
@@ -367,7 +360,7 @@ chan_scale_fwd_kernel(const __nv_bfloat16* __restrict__ x, int xcs, const float*
             for (int k = 0; k < 8; ++k) v[k] += r[k];
         }
         Vec8<__nv_bfloat16>::store(y + p * ycs + c8 * 8, v);
-    }
+    });
 }
 
 // grid = (chunks, N): per image column reduction for da plus elementwise dx
@@ -423,31 +416,14 @@ chan_scale_bwd_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv
     }
 }
 
-static inline size_t colred_smem(int C8, int nacc) {
-    int groups = C8 < kThreads ? C8 : kThreads;
-    int lanes = kThreads / groups;
-    return sizeof(float) * (size_t)lanes * groups * nacc * 8;
-}
-static inline int colred_grid(long long npix, int C8) {
-    int groups = C8 < kThreads ? C8 : kThreads;
-    int lanes = kThreads / groups;
-    long long per_block = (long long)lanes * 16;  // >= 16 pixels per lane
-    long long need = (npix + per_block - 1) / per_block;
-    long long cap = (long long)tsb_num_sms() * 8;
-    if (need < 1) need = 1;
-    return (int)(need < cap ? need : cap);
-}
 }  // namespace
-
-// an NHWC bf16 operand read or written with 16-byte vectors: C and its channel stride multiples of 8, cs >= C, aligned
-#define TSB_VEC_OK(C, cs, ptr) ((C) % 8 == 0 && (cs) % 8 == 0 && (cs) >= (C) && tsb_aligned16(ptr))
 
 extern "C" int tsb_bn_stats(const void* x, int cs, long long npix, int C, float* sum, float* sumsq, float* ws,
                             long long ws_floats, tsb_stream_t stream) {
     TSB_REQUIRE(x && sum && sumsq && npix > 0, "tsb_bn_stats: bad args");
     TSB_REQUIRE(TSB_VEC_OK(C, cs, x), "tsb_bn_stats: C and cs must be multiples of 8, cs >= C, x 16B aligned");
     int C8 = C / 8;
-    const int grid = colred_grid(npix, C8);
+    const int grid = colred_grid(npix, C8, 16, tsb_num_sms() * 8LL);
     TSB_REQUIRE(ws && (long long)grid * 2 * C <= ws_floats, "tsb_bn_stats: workspace needs %lld floats", (long long)grid * 2 * C);
     TSB_REQUIRE(tsb_aligned16(ws), "tsb_bn_stats: ws must be 16B aligned");
     bn_stats_kernel<<<grid, kThreads, colred_smem(C8, 2), (cudaStream_t)stream>>>((const __nv_bfloat16*)x, cs, npix, C8, ws, ws + C, 2LL * C);
@@ -494,7 +470,7 @@ extern "C" int tsb_bn_bwd_reduce(const void* dy, int dycs, const void* y, int yc
                 "tsb_bn_bwd_reduce: per-channel vectors must be 16B aligned");
     int C8 = C / 8;
     cudaStream_t st = (cudaStream_t)stream;
-    const int grid = colred_grid(npix, C8);
+    const int grid = colred_grid(npix, C8, 16, tsb_num_sms() * 8LL);
     TSB_REQUIRE(ws && (long long)grid * 2 * C <= ws_floats, "tsb_bn_bwd_reduce: workspace needs %lld floats", (long long)grid * 2 * C);
     TSB_REQUIRE(tsb_aligned16(ws), "tsb_bn_bwd_reduce: ws must be 16B aligned");
 #define L(M) bn_bwd_reduce_kernel<M><<<grid, kThreads, colred_smem(C8, 2), st>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)y, ycs, (const __nv_bfloat16*)x, xcs, mean, invstd, scale, shift, npix, C8, ws, ws + C, 2LL * C)
@@ -554,12 +530,7 @@ extern "C" int tsb_chan_scale_bwd(const void* dy, int dycs, const void* x, int x
     TSB_REQUIRE(dy && x && a && dx && da && N > 0 && HW > 0, "tsb_chan_scale_bwd: bad args");
     TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, dxcs, dx) && tsb_aligned16(a), "tsb_chan_scale_bwd: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned");
     int C8 = C / 8;
-    int groups = C8 < kThreads ? C8 : kThreads;
-    int lanes = kThreads / groups;
-    int chunks = (HW + lanes * 16 - 1) / (lanes * 16);
-    int cap = (tsb_num_sms() * 8 + N - 1) / N;
-    if (chunks > cap) chunks = cap;
-    if (chunks < 1) chunks = 1;
+    const int chunks = colred_grid(HW, C8, 16, (tsb_num_sms() * 8 + N - 1) / N);
     TSB_REQUIRE(ws && (long long)chunks * N * C <= ws_floats, "tsb_chan_scale_bwd: workspace needs %lld floats", (long long)chunks * N * C);
     chan_scale_bwd_kernel<<<dim3(chunks, N), kThreads, colred_smem(C8, 1), (cudaStream_t)stream>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)x, xcs, a, base, (__nv_bfloat16*)dx, dxcs, ws, HW, C8);
     TSB_CUDA_CHECK_LAUNCH("chan_scale_bwd");

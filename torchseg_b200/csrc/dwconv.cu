@@ -7,7 +7,6 @@
 #include "nhwc_vec.cuh"
 
 namespace {
-constexpr int kThreads = 256;
 constexpr int kMaxC = 4096;   // [9][C] fp32 weights in shared memory: 144 KB at the limit
 
 __device__ __forceinline__ void stage_weights(const float* __restrict__ w, int C, float* s_w) {
@@ -18,13 +17,6 @@ __device__ __forceinline__ void stage_weights(const float* __restrict__ w, int C
     __syncthreads();
 }
 
-__device__ __forceinline__ void lds8(const float* p, float f[8]) {
-    const float4 a = *reinterpret_cast<const float4*>(p);
-    const float4 b = *reinterpret_cast<const float4*>(p + 4);
-    f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
-    f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-
 // y[n,p,q,c] = Σ_{r,s} x[n, p·st−1+r, q·st−1+s, c] · w[c,r,s]; taps in the zero halo add nothing
 template <int ST>
 __global__ void __launch_bounds__(kThreads)
@@ -33,11 +25,8 @@ dw_fprop_kernel(const __nv_bfloat16* __restrict__ x, int xcs, const float* __res
     extern __shared__ float s_w[];
     const int C = C8 * 8;
     stage_weights(w, C, s_w);
-    const long long stride = (long long)gridDim.x * kThreads;
-    const long long start = (long long)blockIdx.x * kThreads + threadIdx.x;
-    VecWalk wk(C8, start, stride);
-    for (long long i = start; i < total; i += stride, wk.next()) {
-        const int pix = (int)wk.p, c8 = wk.c8;
+    for_each_vec(total, C8, [&](long long p64, int c8) {
+        const int pix = (int)p64;
         const int q = pix % Q, np = pix / Q;
         const int p = np % P, n = np / P;
         const int h0 = p * ST - 1, w0 = q * ST - 1;
@@ -54,13 +43,13 @@ dw_fprop_kernel(const __nv_bfloat16* __restrict__ x, int xcs, const float* __res
                 if (ww < 0 || ww >= W) continue;
                 float xv[8], wv[8];
                 Vec8<__nv_bfloat16>::load(x + ((long long)(n * H + h) * W + ww) * xcs + c8 * 8, xv);
-                lds8(s_w + (r * 3 + s) * C + c8 * 8, wv);
+                Vec8<float>::load(s_w + (r * 3 + s) * C + c8 * 8, wv);
 #pragma unroll
                 for (int k = 0; k < 8; ++k) acc[k] = fmaf(xv[k], wv[k], acc[k]);
             }
         }
         Vec8<__nv_bfloat16>::store(y + (long long)pix * ycs + c8 * 8, acc);
-    }
+    });
 }
 
 // dx[n,h,w,c] (+)= Σ_{r,s} dy[n,p,q,c] · w[c,r,s] over the (p, q) with p·st−1+r = h, q·st−1+s = w: the exact gather form
@@ -94,7 +83,7 @@ dw_dgrad_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const float* __r
                 const int q = qw >> (ST - 1);
                 float gv[8], wv[8];
                 Vec8<__nv_bfloat16>::load(dy + ((long long)(n * P + p) * Q + q) * dycs + c8 * 8, gv);
-                lds8(s_w + (r * 3 + s) * C + c8 * 8, wv);
+                Vec8<float>::load(s_w + (r * 3 + s) * C + c8 * 8, wv);
 #pragma unroll
                 for (int k = 0; k < 8; ++k) acc[k] = fmaf(gv[k], wv[k], acc[k]);
             }
@@ -175,12 +164,6 @@ dw_wgrad_kernel(const __nv_bfloat16* __restrict__ x, int xcs, const __nv_bfloat1
 
 int dw_grid(long long work) { return tsb_grid_for(work, kThreads, 8); }
 
-int wgrad_grid(int npix, int C8) {
-    const int groups = C8 < kThreads ? C8 : kThreads;
-    const int lanes = kThreads / groups;
-    return tsb_grid_for(npix, lanes * 8, 8);   // >= 8 pixels per lane
-}
-
 // shared argument checks; P, Q are the output size (p·st−1+r with padding 1: (H − 1) / st + 1)
 int check(const char* fn, const void* a, int acs, const void* b, int bcs, const float* w, int N, int H, int W, int C,
           int stride) {
@@ -188,9 +171,9 @@ int check(const char* fn, const void* a, int acs, const void* b, int bcs, const 
     TSB_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0, "%s: bad shape N=%d H=%d W=%d C=%d", fn, N, H, W, C);
     TSB_REQUIRE(C % 8 == 0 && C <= kMaxC, "%s: C=%d must be a multiple of 8 and at most %d", fn, C, kMaxC);
     TSB_REQUIRE(stride == 1 || stride == 2, "%s: stride %d is not supported (3x3, padding 1, stride 1 or 2)", fn, stride);
-    TSB_REQUIRE(acs % 8 == 0 && bcs % 8 == 0 && acs >= C && bcs >= C,
-                "%s: channel strides (%d, %d) must be multiples of 8 and at least C=%d", fn, acs, bcs, C);
-    TSB_REQUIRE(tsb_aligned16(a) && tsb_aligned16(b), "%s: activations must be 16-byte aligned", fn);
+    TSB_REQUIRE(TSB_VEC_OK(C, acs, a) && TSB_VEC_OK(C, bcs, b),
+                "%s: channel strides (%d, %d) must be multiples of 8 and at least C=%d, activations 16-byte aligned", fn,
+                acs, bcs, C);
     TSB_REQUIRE((long long)N * H * W < (1LL << 31), "%s: N*H*W must be below 2^31", fn);
     return TSB_OK;
 }
@@ -241,11 +224,10 @@ extern "C" int tsb_dwconv_wgrad(const void* x, int xcs, const void* dy, int dycs
     if (rc) return rc;
     const int P = (H - 1) / stride + 1, Q = (W - 1) / stride + 1, C8 = C / 8;
     const int npix = N * P * Q;
-    const int grid = wgrad_grid(npix, C8);
+    const int grid = colred_grid(npix, C8, 8, tsb_num_sms() * 8LL);
     TSB_REQUIRE(ws && (long long)grid * C * 9 <= ws_floats, "tsb_dwconv_wgrad: workspace needs %lld floats",
                 (long long)grid * C * 9);
-    const int groups = C8 < kThreads ? C8 : kThreads;
-    const size_t smem = sizeof(float) * (size_t)(kThreads / groups) * groups * 8;
+    const size_t smem = colred_smem(C8, 1);
     cudaStream_t st = (cudaStream_t)stream;
     if (stride == 1)
         dw_wgrad_kernel<1><<<grid, kThreads, smem, st>>>((const __nv_bfloat16*)x, xcs, (const __nv_bfloat16*)dy, dycs, H, W, P, Q, C8, npix, ws);

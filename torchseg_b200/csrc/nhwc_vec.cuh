@@ -1,6 +1,39 @@
-// 8-channel (16-byte for bf16) vector access helpers for NHWC tensors with a channel stride.
+// 8-channel (16-byte for bf16) vector access helpers for NHWC tensors with a channel stride, and the grid-stride walk
+// of the streaming NHWC kernels built on them.
 #pragma once
 #include "tsb_common.cuh"
+
+// Threads per CTA of every NHWC streaming kernel; the walk's stride and the column-reduction geometry depend on it.
+constexpr int kThreads = 256;
+
+// an NHWC operand read or written with 16-byte vectors: C > 0, C and its channel stride multiples of 8, cs >= C, aligned
+#define TSB_VEC_OK(C, cs, ptr) ((C) > 0 && (C) % 8 == 0 && (cs) % 8 == 0 && (cs) >= (C) && tsb_aligned16(ptr))
+
+// Host-side geometry of the per-channel column reductions (one kThreads CTA = `groups` 8-channel groups per pass x
+// `lanes` pixel lanes): shared memory for nacc accumulators per channel and lane, and the number of CTAs (workspace
+// slots) that gives every lane at least pix_per_lane of npix pixels, at most `cap`.
+static inline int colred_groups(int C8) { return C8 < kThreads ? C8 : kThreads; }
+static inline size_t colred_smem(int C8, int nacc) {
+    const int groups = colred_groups(C8);
+    return sizeof(float) * (size_t)(kThreads / groups) * groups * nacc * 8;
+}
+static inline int colred_grid(long long npix, int C8, int pix_per_lane, long long cap) {
+    const long long per_cta = (long long)(kThreads / colred_groups(C8)) * pix_per_lane;
+    long long need = (npix + per_cta - 1) / per_cta;
+    if (need > cap) need = cap;
+    return (int)(need < 1 ? 1 : need);
+}
+
+// Calls f(DType<TI>{}, DType<TO>{}) for the fp32 / bf16 pair named by two TSB_* dtype codes; false for any other code.
+template <typename T> struct DType { using type = T; };
+template <typename F> bool dispatch_dtype_pair(int a, int b, F&& f) {
+    if (a == TSB_BF16 && b == TSB_BF16) f(DType<__nv_bfloat16>{}, DType<__nv_bfloat16>{});
+    else if (a == TSB_BF16 && b == TSB_F32) f(DType<__nv_bfloat16>{}, DType<float>{});
+    else if (a == TSB_F32 && b == TSB_BF16) f(DType<float>{}, DType<__nv_bfloat16>{});
+    else if (a == TSB_F32 && b == TSB_F32) f(DType<float>{}, DType<float>{});
+    else return false;
+    return true;
+}
 
 #ifdef __CUDACC__
 template <typename T> struct Vec8;
@@ -52,5 +85,15 @@ struct VecWalk {
         if (c8 >= C8) { c8 -= C8; ++p; }
     }
 };
+
+// The grid-stride walk over the `total` = pixels x C8 (pixel, 8-channel group) pairs of a kThreads-thread launch:
+// body(p, c8) for each pair of this thread.
+template <typename F>
+__device__ __forceinline__ void for_each_vec(long long total, int C8, F&& body) {
+    const long long stride = (long long)gridDim.x * kThreads;
+    const long long start = (long long)blockIdx.x * kThreads + threadIdx.x;
+    VecWalk wk(C8, start, stride);
+    for (long long i = start; i < total; i += stride, wk.next()) body(wk.p, wk.c8);
+}
 #endif
 

@@ -3,8 +3,6 @@
 #include "nhwc_vec.cuh"
 
 namespace {
-constexpr int kThreads = 256;
-
 // NCHW fp32 [N,3,H,W] → s2d NHWC16 bf16 [N, H/2, W/2+4, 16]; pixel column 0,1 and W/2+2, W/2+3 are zero
 // padding; channel (py*2+px)*3+c. One thread per packed pixel (32 bytes = two 16-byte stores).
 __global__ void __launch_bounds__(kThreads)
@@ -88,74 +86,46 @@ __global__ void __launch_bounds__(kThreads)
 cast_scale_kernel(const TS* __restrict__ src, int scs, TD* __restrict__ dst, int dcs, long long npix, int C8,
                   const float* __restrict__ scale_dev) {
     const float sc = scale_dev ? *scale_dev : 1.f;
-    const long long total = npix * C8;
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);   // no 64-bit division per vector
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long p = wk_.p;
+    for_each_vec(npix * C8, C8, [&](long long p, int c8) {
         float v[8];
         Vec8<TS>::load(src + p * scs + c8 * 8, v);
 #pragma unroll
         for (int k = 0; k < 8; ++k) v[k] *= sc;
         Vec8<TD>::store(dst + p * dcs + c8 * 8, v);
-    }
+    });
 }
 
+// y = a + b; y = relu(a + b), the tail of RefineResidual / BNRefine (seg_oprs.py:158-162,184-188); and the ReLU
+// backward dx = (y > 0) ? dy : 0 with a = dy, b = y
+struct AddOp { __device__ float operator()(float a, float b) const { return a + b; } };
+struct AddReluOp { __device__ float operator()(float a, float b) const { return fmaxf(a + b, 0.f); } };
+struct ReluBwdOp { __device__ float operator()(float a, float b) const { return b > 0.f ? a : 0.f; } };
+
+template <typename Op>
 __global__ void __launch_bounds__(kThreads)
-add_kernel(const __nv_bfloat16* __restrict__ a, int acs, const __nv_bfloat16* __restrict__ b, int bcs,
-           __nv_bfloat16* __restrict__ y, int ycs, long long npix, int C8) {
-    const long long total = npix * C8;
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);   // no 64-bit division per vector
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long p = wk_.p;
+binary_kernel(const __nv_bfloat16* __restrict__ a, int acs, const __nv_bfloat16* __restrict__ b, int bcs,
+              __nv_bfloat16* __restrict__ y, int ycs, long long npix, int C8) {
+    for_each_vec(npix * C8, C8, [&](long long p, int c8) {
         float u[8], v[8];
         Vec8<__nv_bfloat16>::load(a + p * acs + c8 * 8, u);
         Vec8<__nv_bfloat16>::load(b + p * bcs + c8 * 8, v);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) u[k] += v[k];
+        for (int k = 0; k < 8; ++k) u[k] = Op()(u[k], v[k]);
         Vec8<__nv_bfloat16>::store(y + p * ycs + c8 * 8, u);
-    }
+    });
 }
 
-// y = relu(a + b): tail of RefineResidual / BNRefine (seg_oprs.py:158-162,184-188)
-__global__ void __launch_bounds__(kThreads)
-add_relu_kernel(const __nv_bfloat16* __restrict__ a, int acs, const __nv_bfloat16* __restrict__ b, int bcs,
-                __nv_bfloat16* __restrict__ y, int ycs, long long npix, int C8) {
-    const long long total = npix * C8;
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);   // no 64-bit division per vector
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long p = wk_.p;
-        float u[8], v[8];
-        Vec8<__nv_bfloat16>::load(a + p * acs + c8 * 8, u);
-        Vec8<__nv_bfloat16>::load(b + p * bcs + c8 * 8, v);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) u[k] = fmaxf(u[k] + v[k], 0.f);
-        Vec8<__nv_bfloat16>::store(y + p * ycs + c8 * 8, u);
-    }
-}
-
-// dx = (y > 0) ? dy : 0
-__global__ void __launch_bounds__(kThreads)
-relu_bwd_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_bfloat16* __restrict__ y, int ycs,
-                __nv_bfloat16* __restrict__ dx, int dxcs, long long npix, int C8) {
-    const long long total = npix * C8;
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);   // no 64-bit division per vector
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long p = wk_.p;
-        float u[8], v[8];
-        Vec8<__nv_bfloat16>::load(dy + p * dycs + c8 * 8, u);
-        Vec8<__nv_bfloat16>::load(y + p * ycs + c8 * 8, v);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) u[k] = v[k] > 0.f ? u[k] : 0.f;
-        Vec8<__nv_bfloat16>::store(dx + p * dxcs + c8 * 8, u);
-    }
+template <typename Op>
+int binary_launch(const char* fn, const void* a, int acs, const void* b, int bcs, void* y, int ycs, long long npix,
+                  int C, tsb_stream_t stream) {
+    TSB_REQUIRE(a && b && y && npix > 0, "%s: bad args", fn);
+    TSB_REQUIRE(TSB_VEC_OK(C, acs, a) && TSB_VEC_OK(C, bcs, b) && TSB_VEC_OK(C, ycs, y),
+                "%s: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned", fn);
+    const int C8 = C / 8;
+    binary_kernel<Op><<<tsb_grid_for(npix * C8, kThreads, 8), kThreads, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16*)a, acs, (const __nv_bfloat16*)b, bcs, (__nv_bfloat16*)y, ycs, npix, C8);
+    TSB_CUDA_CHECK_LAUNCH(fn);
+    return TSB_OK;
 }
 
 // dst[pix, 0..Kp) (bf16) = src[pix, 0..K) zero-extended: gradient of a K-class head (K = 19, 150, 1 ...) into the
@@ -164,17 +134,14 @@ template <typename TS>
 __global__ void __launch_bounds__(kThreads)
 cast_pad_kernel(const TS* __restrict__ src, int scs, int K, __nv_bfloat16* __restrict__ dst, int dcs, int Kp8,
                 long long npix) {
-    const long long total = npix * Kp8;
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(Kp8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += stride_, wk_.next()) {
-        const int c0 = wk_.c8 * 8;
-        const TS* s = src + wk_.p * scs + c0;
+    for_each_vec(npix * Kp8, Kp8, [&](long long p, int c8) {
+        const int c0 = c8 * 8;
+        const TS* s = src + p * scs + c0;
         float v[8];
 #pragma unroll
         for (int k = 0; k < 8; ++k) v[k] = (c0 + k < K) ? (float)s[k] : 0.f;
-        Vec8<__nv_bfloat16>::store(dst + wk_.p * dcs + c0, v);
-    }
+        Vec8<__nv_bfloat16>::store(dst + p * dcs + c0, v);
+    });
 }
 
 // db[k] += Σ_pix dy[pix,k]; one warp per pixel stripe, lanes over channels (K <= 64 typical: 19 padded). Each CTA
@@ -346,20 +313,17 @@ extern "C" int tsb_unpack_stem_wgrad(const float* dwp, int K, int R, float* dw, 
 
 extern "C" int tsb_cast_scale(const void* src, int sdtype, int scs, void* dst, int ddtype, int dcs, long long npix, int C,
                               const float* scale_dev, tsb_stream_t stream) {
-    TSB_REQUIRE(src && dst && npix > 0 && C > 0, "tsb_cast_scale: bad args");
-    TSB_REQUIRE(scs >= C && dcs >= C, "tsb_cast_scale: channel strides must be >= C");
-    TSB_REQUIRE(C % 8 == 0 && scs % 8 == 0 && dcs % 8 == 0 && tsb_aligned16(src) && tsb_aligned16(dst),
-                "tsb_cast_scale: C and channel strides must be multiples of 8, pointers 16B aligned");
+    TSB_REQUIRE(src && dst && npix > 0, "tsb_cast_scale: bad args");
+    TSB_REQUIRE(TSB_VEC_OK(C, scs, src) && TSB_VEC_OK(C, dcs, dst),
+                "tsb_cast_scale: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned");
     int C8 = C / 8;
     int grid = tsb_grid_for(npix * C8, kThreads, 8);
-    cudaStream_t st = (cudaStream_t)stream;
-#define L(TS, TD) cast_scale_kernel<TS, TD><<<grid, kThreads, 0, st>>>((const TS*)src, scs, (TD*)dst, dcs, npix, C8, scale_dev)
-    if (sdtype == TSB_F32 && ddtype == TSB_BF16) L(float, __nv_bfloat16);
-    else if (sdtype == TSB_BF16 && ddtype == TSB_F32) L(__nv_bfloat16, float);
-    else if (sdtype == TSB_F32 && ddtype == TSB_F32) L(float, float);
-    else if (sdtype == TSB_BF16 && ddtype == TSB_BF16) L(__nv_bfloat16, __nv_bfloat16);
-    else TSB_FAIL(TSB_ERR_ARG, "tsb_cast_scale: bad dtype");
-#undef L
+    const bool ok = dispatch_dtype_pair(sdtype, ddtype, [&](auto ts, auto td) {
+        using TS = typename decltype(ts)::type;
+        using TD = typename decltype(td)::type;
+        cast_scale_kernel<TS, TD><<<grid, kThreads, 0, (cudaStream_t)stream>>>((const TS*)src, scs, (TD*)dst, dcs, npix, C8, scale_dev);
+    });
+    TSB_REQUIRE(ok, "tsb_cast_scale: bad dtype");
     TSB_CUDA_CHECK_LAUNCH("cast_scale");
     return TSB_OK;
 }
@@ -367,7 +331,7 @@ extern "C" int tsb_cast_scale(const void* src, int sdtype, int scs, void* dst, i
 extern "C" int tsb_cast_pad(const void* src, int sdtype, int scs, int K, void* dst_bf16, int dcs, int Kp, long long npix,
                             tsb_stream_t stream) {
     TSB_REQUIRE(src && dst_bf16 && npix > 0 && K > 0 && Kp >= K, "tsb_cast_pad: bad args");
-    TSB_REQUIRE(Kp % 8 == 0 && dcs % 8 == 0 && dcs >= Kp && scs >= K && tsb_aligned16(dst_bf16), "tsb_cast_pad: Kp, dcs multiples of 8");
+    TSB_REQUIRE(TSB_VEC_OK(Kp, dcs, dst_bf16) && scs >= K, "tsb_cast_pad: Kp, dcs multiples of 8, dcs >= Kp, scs >= K, dst 16B aligned");
     TSB_REQUIRE(sdtype == TSB_F32 || sdtype == TSB_BF16, "tsb_cast_pad: bad dtype");
     int grid = tsb_grid_for(npix * (Kp / 8), kThreads, 8);
     if (sdtype == TSB_F32)
@@ -380,41 +344,17 @@ extern "C" int tsb_cast_pad(const void* src, int sdtype, int scs, int K, void* d
 
 extern "C" int tsb_add(const void* a, int acs, const void* b, int bcs, void* y, int ycs, long long npix, int C,
                        tsb_stream_t stream) {
-    TSB_REQUIRE(a && b && y && npix > 0, "tsb_add: bad args");
-    TSB_REQUIRE(acs >= C && bcs >= C && ycs >= C, "tsb_add: channel strides must be >= C");
-    TSB_REQUIRE(C % 8 == 0 && acs % 8 == 0 && bcs % 8 == 0 && ycs % 8 == 0 && tsb_aligned16(a) && tsb_aligned16(b) && tsb_aligned16(y),
-                "tsb_add: C and channel strides must be multiples of 8, pointers 16B aligned");
-    int C8 = C / 8;
-    int grid = tsb_grid_for(npix * C8, kThreads, 8);
-    add_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)a, acs, (const __nv_bfloat16*)b, bcs, (__nv_bfloat16*)y, ycs, npix, C8);
-    TSB_CUDA_CHECK_LAUNCH("add");
-    return TSB_OK;
+    return binary_launch<AddOp>("tsb_add", a, acs, b, bcs, y, ycs, npix, C, stream);
 }
 
 extern "C" int tsb_add_relu(const void* a, int acs, const void* b, int bcs, void* y, int ycs, long long npix, int C,
                             tsb_stream_t stream) {
-    TSB_REQUIRE(a && b && y && npix > 0, "tsb_add_relu: bad args");
-    TSB_REQUIRE(acs >= C && bcs >= C && ycs >= C, "tsb_add_relu: channel strides must be >= C");
-    TSB_REQUIRE(C % 8 == 0 && acs % 8 == 0 && bcs % 8 == 0 && ycs % 8 == 0 && tsb_aligned16(a) && tsb_aligned16(b) && tsb_aligned16(y),
-                "tsb_add_relu: C and channel strides must be multiples of 8, pointers 16B aligned");
-    int C8 = C / 8;
-    int grid = tsb_grid_for(npix * C8, kThreads, 8);
-    add_relu_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)a, acs, (const __nv_bfloat16*)b, bcs, (__nv_bfloat16*)y, ycs, npix, C8);
-    TSB_CUDA_CHECK_LAUNCH("add_relu");
-    return TSB_OK;
+    return binary_launch<AddReluOp>("tsb_add_relu", a, acs, b, bcs, y, ycs, npix, C, stream);
 }
 
 extern "C" int tsb_relu_bwd(const void* dy, int dycs, const void* y, int ycs, void* dx, int dxcs, long long npix, int C,
                             tsb_stream_t stream) {
-    TSB_REQUIRE(dy && y && dx && npix > 0, "tsb_relu_bwd: bad args");
-    TSB_REQUIRE(dycs >= C && ycs >= C && dxcs >= C, "tsb_relu_bwd: channel strides must be >= C");
-    TSB_REQUIRE(C % 8 == 0 && dycs % 8 == 0 && ycs % 8 == 0 && dxcs % 8 == 0 && tsb_aligned16(dy) && tsb_aligned16(y) && tsb_aligned16(dx),
-                "tsb_relu_bwd: C and channel strides must be multiples of 8, pointers 16B aligned");
-    int C8 = C / 8;
-    int grid = tsb_grid_for(npix * C8, kThreads, 8);
-    relu_bwd_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)y, ycs, (__nv_bfloat16*)dx, dxcs, npix, C8);
-    TSB_CUDA_CHECK_LAUNCH("relu_bwd");
-    return TSB_OK;
+    return binary_launch<ReluBwdOp>("tsb_relu_bwd", dy, dycs, y, ycs, dx, dxcs, npix, C, stream);
 }
 
 extern "C" int tsb_bias_grad(const void* dy, int dycs, long long npix, int K, float* db, float* ws, long long ws_floats,

@@ -139,8 +139,8 @@ extern "C" int tsb_softmax_rows_fwd(const void* in, int idtype, int ics, void* o
                                     tsb_stream_t stream) {
     TSB_REQUIRE(in && out && rows > 0 && C > 0, "tsb_softmax_rows_fwd: bad args");
     TSB_REQUIRE(idtype == TSB_BF16 || idtype == TSB_F32, "tsb_softmax_rows_fwd: bad dtype");
-    TSB_REQUIRE(C % 8 == 0 && Cp % 8 == 0 && Cp >= C && ics % 8 == 0 && ocs % 8 == 0 && ics >= C && ocs >= Cp &&
-                tsb_aligned16(in) && tsb_aligned16(out), "tsb_softmax_rows_fwd: C, Cp, strides must be multiples of 8");
+    TSB_REQUIRE(Cp >= C && TSB_VEC_OK(C, ics, in) && TSB_VEC_OK(Cp, ocs, out),
+                "tsb_softmax_rows_fwd: C, Cp, strides must be multiples of 8, Cp >= C, strides >= C / Cp, pointers 16B aligned");
     TSB_REQUIRE(Cp <= kSmThreads * kMaxVecPerThread * 8, "tsb_softmax_rows_fwd: at most %d channels", kSmThreads * kMaxVecPerThread * 8);
     TSB_REQUIRE(rows < (1ll << 31), "tsb_softmax_rows_fwd: too many rows");
     if (idtype == TSB_BF16)
@@ -154,9 +154,8 @@ extern "C" int tsb_softmax_rows_fwd(const void* in, int idtype, int ics, void* o
 extern "C" int tsb_softmax_rows_bwd(const void* S, int scs, const void* dS, int dscs, void* dA, int dacs, long long rows,
                                     int C, int Cp, tsb_stream_t stream) {
     TSB_REQUIRE(S && dS && dA && rows > 0 && C > 0, "tsb_softmax_rows_bwd: bad args");
-    TSB_REQUIRE(C % 8 == 0 && Cp % 8 == 0 && Cp >= C && scs % 8 == 0 && dscs % 8 == 0 && dacs % 8 == 0 && scs >= C &&
-                dscs >= C && dacs >= Cp && tsb_aligned16(S) && tsb_aligned16(dS) && tsb_aligned16(dA),
-                "tsb_softmax_rows_bwd: C, Cp, strides must be multiples of 8");
+    TSB_REQUIRE(Cp >= C && TSB_VEC_OK(C, scs, S) && TSB_VEC_OK(C, dscs, dS) && TSB_VEC_OK(Cp, dacs, dA),
+                "tsb_softmax_rows_bwd: C, Cp, strides must be multiples of 8, Cp >= C, strides >= C / Cp, pointers 16B aligned");
     TSB_REQUIRE(Cp <= kSmThreads * kMaxVecPerThread * 8, "tsb_softmax_rows_bwd: at most %d channels", kSmThreads * kMaxVecPerThread * 8);
     TSB_REQUIRE(rows < (1ll << 31), "tsb_softmax_rows_bwd: too many rows");
     softmax_rows_bwd_kernel<<<(unsigned)rows, kSmThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)S, scs, (const __nv_bfloat16*)dS, dscs, (__nv_bfloat16*)dA, dacs, C / 8, Cp / 8);

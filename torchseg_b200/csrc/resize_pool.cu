@@ -23,8 +23,6 @@ __device__ __forceinline__ void split_pix(long long pix, int W, int H, int& w, i
         n = (int)(t / H);
     }
 }
-constexpr int kThreads = 256;
-
 __host__ __device__ __forceinline__ float area_scale(int in_size, int out_size) {
     return out_size > 1 ? (float)(in_size - 1) / (float)(out_size - 1) : 0.0f;
 }
@@ -47,11 +45,7 @@ bilinear_fwd_kernel(const TI* __restrict__ in, int ics, TO* __restrict__ out, in
                     int Ho, int Wo) {
     const float ry = area_scale(Hi, Ho), rx = area_scale(Wi, Wo);
     const long long total = (long long)N * Ho * Wo * C8;
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);   // no 64-bit division per vector
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long pix = wk_.p;
+    for_each_vec(total, C8, [&](long long pix, int c8) {
         int x, y, n;
         split_pix(pix, Wo, Ho, x, y, n);
         Lerp ly = make_lerp(ry, y, Hi), lx = make_lerp(rx, x, Wi);
@@ -65,7 +59,7 @@ bilinear_fwd_kernel(const TI* __restrict__ in, int ics, TO* __restrict__ out, in
         for (int k = 0; k < 8; ++k)
             o[k] = ly.l0 * (lx.l0 * a[k] + lx.l1 * bb[k]) + ly.l1 * (lx.l0 * c[k] + lx.l1 * d[k]);
         Vec8<TO>::store(out + pix * ocs + c8 * 8, o);
-    }
+    });
 }
 
 // scalar-channel variant (C not a multiple of 8, e.g. 19-class logits) with NHWC or NCHW output
@@ -106,11 +100,7 @@ bilinear_bwd_kernel(const TO* __restrict__ dout, int ocs, TI* __restrict__ din, 
     const float ry = area_scale(Hi, Ho), rx = area_scale(Wi, Wo);
     const long long total = (long long)N * Hi * Wi * C8;
     constexpr int kMaxCand = 12;  // candidate output columns kept in registers (up-scale factors >= 1/4 per side)
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);   // no 64-bit division per vector
-    for (long long idx = (long long)blockIdx.x * kThreads + threadIdx.x; idx < total; idx += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long pix = wk_.p;
+    for_each_vec(total, C8, [&](long long pix, int c8) {
         int j, i, n;
         split_pix(pix, Wi, Hi, j, i, n);
         int y_lo, y_hi, x_lo, x_hi;
@@ -168,7 +158,7 @@ bilinear_bwd_kernel(const TO* __restrict__ dout, int ocs, TI* __restrict__ din, 
             for (int k = 0; k < 8; ++k) acc[k] += old[k];
         }
         Vec8<TI>::store(dst, acc);
-    }
+    });
 }
 
 // ---------------------------------------------------------------- adaptive average pool
@@ -226,11 +216,7 @@ __global__ void __launch_bounds__(kThreads)
 adaptive_avgpool_bwd_kernel(const float* __restrict__ dout, int N, int C8, int H, int W, int S,
                             __nv_bfloat16* __restrict__ din, int ics, int accumulate) {
     const long long total = (long long)N * H * W * C8;
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);   // no 64-bit division per vector
-    for (long long idx = (long long)blockIdx.x * kThreads + threadIdx.x; idx < total; idx += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long pix = wk_.p;
+    for_each_vec(total, C8, [&](long long pix, int c8) {
         int w, h, n;
         split_pix(pix, W, H, w, h, n);
         float acc[8];
@@ -259,7 +245,7 @@ adaptive_avgpool_bwd_kernel(const float* __restrict__ dout, int N, int C8, int H
             for (int k = 0; k < 8; ++k) acc[k] += old[k];
         }
         Vec8<__nv_bfloat16>::store(dst, acc);
-    }
+    });
 }
 
 // ---------------------------------------------------------------- max pool 3x3 stride 2 pad 1
@@ -269,11 +255,7 @@ __global__ void __launch_bounds__(kThreads)
 maxpool_fwd_kernel(const __nv_bfloat16* __restrict__ in, int ics, __nv_bfloat16* __restrict__ out, int ocs,
                    uint8_t* __restrict__ idx, int N, int C8, int H, int W, int P, int Q) {
     const long long total = (long long)N * P * Q * C8;
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);   // no 64-bit division per vector
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long pix = wk_.p;
+    for_each_vec(total, C8, [&](long long pix, int c8) {
         int q, p, n;
         split_pix(pix, Q, P, q, p, n);
         float m[8];
@@ -302,7 +284,7 @@ maxpool_fwd_kernel(const __nv_bfloat16* __restrict__ in, int ics, __nv_bfloat16*
             pk.y = am[4] | (am[5] << 8) | (am[6] << 16) | (am[7] << 24);
             *reinterpret_cast<uint2*>(idx + pix * (long long)(C8 * 8) + c8 * 8) = pk;
         }
-    }
+    });
 }
 
 // backward, gather form. One thread owns a 2x2 block of input pixels (h = 2a+dh, w = 2b+dw) x 8 channels: the
@@ -313,11 +295,7 @@ maxpool_bwd_kernel(const uint8_t* __restrict__ idx, const __nv_bfloat16* __restr
                    __nv_bfloat16* __restrict__ din, int dcs, int N, int C8, int H, int W, int P, int Q) {
     const int HB = (H + 1) / 2, WB = (W + 1) / 2;
     const long long total = (long long)N * HB * WB * C8;
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);   // no 64-bit division per vector
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long blk = wk_.p;
+    for_each_vec(total, C8, [&](long long blk, int c8) {
         int b, a, n;
         split_pix(blk, WB, HB, b, a, n);
         uint2 pk[4];
@@ -361,12 +339,8 @@ maxpool_bwd_kernel(const uint8_t* __restrict__ idx, const __nv_bfloat16* __restr
                 Vec8<__nv_bfloat16>::store(din + (((long long)n * H + h) * W + w) * dcs + c8 * 8, acc);
             }
         }
-    }
+    });
 }
-
-template <typename A, typename B> struct SameT { static constexpr bool v = false; };
-template <typename A> struct SameT<A, A> { static constexpr bool v = true; };
-
 
 // S = 1 (global average pool: ARM / FFM / global-context squeezes, seg_oprs.py:200,223, bisenet network.py:35): the backward is
 // a broadcast of dout[n, c] / (H·W) over the map. The generic kernel spends ~10 integer divisions per 16-byte vector on the bin
@@ -374,11 +348,7 @@ template <typename A> struct SameT<A, A> { static constexpr bool v = true; };
 __global__ void __launch_bounds__(kThreads)
 global_avgpool_bwd_kernel(const float* __restrict__ dout, int C8, long long hw, long long total, float inv_area,
                           __nv_bfloat16* __restrict__ din, int ics, int accumulate) {
-    const long long stride_ = (long long)gridDim.x * kThreads;
-    VecWalk wk_(C8, (long long)blockIdx.x * kThreads + threadIdx.x, stride_);
-    for (long long idx = (long long)blockIdx.x * kThreads + threadIdx.x; idx < total; idx += stride_, wk_.next()) {
-        const int c8 = wk_.c8;
-        const long long pix = wk_.p;
+    for_each_vec(total, C8, [&](long long pix, int c8) {
         const long long n = pix / hw;
         float g[8];
         ldg8f(dout + (n * C8 + c8) * 8, g);
@@ -392,7 +362,7 @@ global_avgpool_bwd_kernel(const float* __restrict__ dout, int C8, long long hw, 
             for (int k = 0; k < 8; ++k) g[k] += old[k];
         }
         Vec8<__nv_bfloat16>::store(dst, g);
-    }
+    });
 }
 
 }  // namespace
@@ -405,26 +375,17 @@ extern "C" int tsb_bilinear_fwd(const void* in, int idtype, int ics, void* out, 
     TSB_REQUIRE(TSB_DT_OK(idtype) && TSB_DT_OK(odtype), "tsb_bilinear_fwd: bad dtype");
     TSB_REQUIRE(N > 0 && C > 0 && Hi > 0 && Wi > 0 && Ho > 0 && Wo > 0 && ics >= C && ocs >= C, "tsb_bilinear_fwd: bad shape");
     cudaStream_t st = (cudaStream_t)stream;
-    const bool vec = (C % 8 == 0) && (ics % 8 == 0) && (ocs % 8 == 0) && tsb_aligned16(in) && tsb_aligned16(out);
-    if (vec) {
-        long long total = (long long)N * Ho * Wo * (C / 8);
-        int grid = tsb_grid_for(total, kThreads, 8);
-#define L(TI, TO) bilinear_fwd_kernel<TI, TO><<<grid, kThreads, 0, st>>>((const TI*)in, ics, (TO*)out, ocs, N, C / 8, Hi, Wi, Ho, Wo)
-        if (idtype == TSB_BF16 && odtype == TSB_BF16) L(__nv_bfloat16, __nv_bfloat16);
-        else if (idtype == TSB_BF16 && odtype == TSB_F32) L(__nv_bfloat16, float);
-        else if (idtype == TSB_F32 && odtype == TSB_BF16) L(float, __nv_bfloat16);
-        else L(float, float);
-#undef L
-    } else {
-        long long total = (long long)N * Ho * Wo * C;
-        int grid = tsb_grid_for(total, kThreads, 8);
-#define L(TI, TO) bilinear_fwd_scalar_kernel<TI, TO, false><<<grid, kThreads, 0, st>>>((const TI*)in, ics, (TO*)out, ocs, N, C, Hi, Wi, Ho, Wo)
-        if (idtype == TSB_BF16 && odtype == TSB_BF16) L(__nv_bfloat16, __nv_bfloat16);
-        else if (idtype == TSB_BF16 && odtype == TSB_F32) L(__nv_bfloat16, float);
-        else if (idtype == TSB_F32 && odtype == TSB_BF16) L(float, __nv_bfloat16);
-        else L(float, float);
-#undef L
-    }
+    const bool vec = TSB_VEC_OK(C, ics, in) && TSB_VEC_OK(C, ocs, out);
+    const long long total = (long long)N * Ho * Wo * (vec ? C / 8 : C);
+    const int grid = tsb_grid_for(total, kThreads, 8);
+    dispatch_dtype_pair(idtype, odtype, [&](auto ti, auto to) {
+        using TI = typename decltype(ti)::type;
+        using TO = typename decltype(to)::type;
+        if (vec)
+            bilinear_fwd_kernel<TI, TO><<<grid, kThreads, 0, st>>>((const TI*)in, ics, (TO*)out, ocs, N, C / 8, Hi, Wi, Ho, Wo);
+        else
+            bilinear_fwd_scalar_kernel<TI, TO, false><<<grid, kThreads, 0, st>>>((const TI*)in, ics, (TO*)out, ocs, N, C, Hi, Wi, Ho, Wo);
+    });
     TSB_CUDA_CHECK_LAUNCH("bilinear_fwd");
     return TSB_OK;
 }
@@ -432,6 +393,8 @@ extern "C" int tsb_bilinear_fwd(const void* in, int idtype, int ics, void* out, 
 extern "C" int tsb_bilinear_fwd_nhwc_to_nchw(const void* in, int idtype, int ics, float* out, int N, int C, int Hi,
                                              int Wi, int Ho, int Wo, tsb_stream_t stream) {
     TSB_REQUIRE(in && out && TSB_DT_OK(idtype), "tsb_bilinear_fwd_nhwc_to_nchw: bad args");
+    TSB_REQUIRE(N > 0 && C > 0 && Hi > 0 && Wi > 0 && Ho > 0 && Wo > 0 && ics >= C,
+                "tsb_bilinear_fwd_nhwc_to_nchw: bad shape (sizes must be positive, ics >= C)");
     long long total = (long long)N * Ho * Wo * C;
     int grid = tsb_grid_for(total, kThreads, 8);
     cudaStream_t st = (cudaStream_t)stream;
@@ -446,43 +409,33 @@ extern "C" int tsb_bilinear_fwd_nhwc_to_nchw(const void* in, int idtype, int ics
 extern "C" int tsb_bilinear_bwd(const void* dout, int odtype, int ocs, void* din, int idtype, int ics, int N, int C,
                                 int Hi, int Wi, int Ho, int Wo, int accumulate, tsb_stream_t stream) {
     TSB_REQUIRE(dout && din && TSB_DT_OK(idtype) && TSB_DT_OK(odtype), "tsb_bilinear_bwd: bad args");
-    TSB_REQUIRE(ics >= C && ocs >= C, "tsb_bilinear_bwd: channel strides must be >= C");
-    TSB_REQUIRE((C % 8 == 0) && (ics % 8 == 0) && (ocs % 8 == 0) && tsb_aligned16(dout) && tsb_aligned16(din),
-                "tsb_bilinear_bwd: C and channel strides must be multiples of 8, pointers 16B aligned");
+    TSB_REQUIRE(TSB_VEC_OK(C, ics, din) && TSB_VEC_OK(C, ocs, dout),
+                "tsb_bilinear_bwd: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned");
     long long total = (long long)N * Hi * Wi * (C / 8);
     int grid = tsb_grid_for(total, kThreads, 8);
-    cudaStream_t st = (cudaStream_t)stream;
-#define L(TO, TI) bilinear_bwd_kernel<TO, TI><<<grid, kThreads, 0, st>>>((const TO*)dout, ocs, (TI*)din, ics, N, C / 8, Hi, Wi, Ho, Wo, accumulate)
-    if (odtype == TSB_BF16 && idtype == TSB_BF16) L(__nv_bfloat16, __nv_bfloat16);
-    else if (odtype == TSB_BF16 && idtype == TSB_F32) L(__nv_bfloat16, float);
-    else if (odtype == TSB_F32 && idtype == TSB_BF16) L(float, __nv_bfloat16);
-    else L(float, float);
-#undef L
+    dispatch_dtype_pair(odtype, idtype, [&](auto to, auto ti) {
+        using TO = typename decltype(to)::type;
+        using TI = typename decltype(ti)::type;
+        bilinear_bwd_kernel<TO, TI><<<grid, kThreads, 0, (cudaStream_t)stream>>>((const TO*)dout, ocs, (TI*)din, ics, N, C / 8, Hi, Wi, Ho, Wo, accumulate);
+    });
     TSB_CUDA_CHECK_LAUNCH("bilinear_bwd");
     return TSB_OK;
 }
 
 extern "C" int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, int H, int W, int S, float* out, float* ws,
                                         long long ws_floats, tsb_stream_t stream) {
-    TSB_REQUIRE(in && out, "tsb_adaptive_avgpool_fwd: null pointer");
-    TSB_REQUIRE(ics >= C, "tsb_adaptive_avgpool_fwd: ics must be >= C");
-    TSB_REQUIRE(C % 8 == 0 && ics % 8 == 0 && tsb_aligned16(in), "tsb_adaptive_avgpool_fwd: C, ics must be multiples of 8, in 16B aligned");
+    TSB_REQUIRE(in && out && N > 0, "tsb_adaptive_avgpool_fwd: null pointer or N <= 0");
+    TSB_REQUIRE(TSB_VEC_OK(C, ics, in), "tsb_adaptive_avgpool_fwd: C, ics must be multiples of 8, ics >= C, in 16B aligned");
     TSB_REQUIRE(S >= 1 && S <= H && S <= W, "tsb_adaptive_avgpool_fwd: bad S");
     cudaStream_t st = (cudaStream_t)stream;
     TSB_CUDA_CALL(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)N * S * S * C, st));
     const int bins = N * S * S;
     const int max_bin_pix = ((H + S - 1) / S + 1) * ((W + S - 1) / S + 1);
-    int chunks = (2 * tsb_num_sms() + bins - 1) / bins;
     const int C8 = C / 8;
-    const int groups = C8 < kThreads ? C8 : kThreads;
-    const int lanes = kThreads / groups;
-    int max_chunks = (max_bin_pix + lanes * 4 - 1) / (lanes * 4);
-    if (chunks > max_chunks) chunks = max_chunks;
-    if (chunks < 1) chunks = 1;
-    size_t smem = sizeof(float) * (size_t)lanes * groups * 8;
+    const int chunks = colred_grid(max_bin_pix, C8, 4, (2 * tsb_num_sms() + bins - 1) / bins);
     TSB_REQUIRE(ws && (long long)chunks * bins * C <= ws_floats, "tsb_adaptive_avgpool_fwd: workspace needs %lld floats",
                 (long long)chunks * bins * C);
-    adaptive_avgpool_fwd_kernel<<<dim3(bins, chunks), kThreads, smem, st>>>((const __nv_bfloat16*)in, ics, N, C, H, W, S, ws);
+    adaptive_avgpool_fwd_kernel<<<dim3(bins, chunks), kThreads, colred_smem(C8, 1), st>>>((const __nv_bfloat16*)in, ics, N, C, H, W, S, ws);
     TSB_CUDA_CHECK_LAUNCH("adaptive_avgpool_fwd");
     return tsb_det_reduce(out, ws, chunks, (long long)bins * C, (long long)bins * C, st);
 }
@@ -490,9 +443,8 @@ extern "C" int tsb_adaptive_avgpool_fwd(const void* in, int ics, int N, int C, i
 extern "C" int tsb_adaptive_avgpool_bwd(const float* dout, int N, int C, int H, int W, int S, void* din, int ics,
                                         int accumulate, tsb_stream_t stream) {
     TSB_REQUIRE(dout && din, "tsb_adaptive_avgpool_bwd: null pointer");
-    TSB_REQUIRE(ics >= C, "tsb_adaptive_avgpool_bwd: ics must be >= C");
-    TSB_REQUIRE(C % 8 == 0 && ics % 8 == 0 && tsb_aligned16(din) && tsb_aligned16(dout),
-                "tsb_adaptive_avgpool_bwd: C, ics must be multiples of 8, pointers 16B aligned");
+    TSB_REQUIRE(TSB_VEC_OK(C, ics, din) && tsb_aligned16(dout),
+                "tsb_adaptive_avgpool_bwd: C, ics must be multiples of 8, ics >= C, pointers 16B aligned");
     long long total = (long long)N * H * W * (C / 8);
     int grid = tsb_grid_for(total, kThreads, 8);
     if (S == 1) {
@@ -509,9 +461,8 @@ extern "C" int tsb_adaptive_avgpool_bwd(const float* dout, int N, int C, int H, 
 extern "C" int tsb_maxpool3x3s2_fwd(const void* in, int ics, void* out, int ocs, void* argmax, int N, int C, int H,
                                     int W, tsb_stream_t stream) {
     TSB_REQUIRE(in && out, "tsb_maxpool3x3s2_fwd: null pointer");
-    TSB_REQUIRE(ics >= C && ocs >= C, "tsb_maxpool3x3s2_fwd: channel strides must be >= C");
-    TSB_REQUIRE(C % 8 == 0 && ics % 8 == 0 && ocs % 8 == 0 && tsb_aligned16(in) && tsb_aligned16(out) && tsb_aligned8(argmax),
-                "tsb_maxpool3x3s2_fwd: C, strides must be multiples of 8, in/out 16B and argmax 8B aligned");
+    TSB_REQUIRE(TSB_VEC_OK(C, ics, in) && TSB_VEC_OK(C, ocs, out) && tsb_aligned8(argmax),
+                "tsb_maxpool3x3s2_fwd: C, strides must be multiples of 8, strides >= C, in/out 16B and argmax 8B aligned");
     const int P = (H + 2 - 3) / 2 + 1, Q = (W + 2 - 3) / 2 + 1;
     long long total = (long long)N * P * Q * (C / 8);
     int grid = tsb_grid_for(total, kThreads, 8);
@@ -523,9 +474,8 @@ extern "C" int tsb_maxpool3x3s2_fwd(const void* in, int ics, void* out, int ocs,
 extern "C" int tsb_maxpool3x3s2_bwd(const void* argmax, const void* dout, int ocs, void* din, int dcs, int N, int C,
                                     int H, int W, tsb_stream_t stream) {
     TSB_REQUIRE(argmax && dout && din, "tsb_maxpool3x3s2_bwd: null pointer");
-    TSB_REQUIRE(ocs >= C && dcs >= C, "tsb_maxpool3x3s2_bwd: channel strides must be >= C");
-    TSB_REQUIRE(C % 8 == 0 && ocs % 8 == 0 && dcs % 8 == 0 && tsb_aligned16(dout) && tsb_aligned16(din) && tsb_aligned8(argmax),
-                "tsb_maxpool3x3s2_bwd: C, strides must be multiples of 8, dout/din 16B and argmax 8B aligned");
+    TSB_REQUIRE(TSB_VEC_OK(C, ocs, dout) && TSB_VEC_OK(C, dcs, din) && tsb_aligned8(argmax),
+                "tsb_maxpool3x3s2_bwd: C, strides must be multiples of 8, strides >= C, dout/din 16B and argmax 8B aligned");
     const int P = (H + 2 - 3) / 2 + 1, Q = (W + 2 - 3) / 2 + 1;
     long long total = (long long)N * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
     int grid = tsb_grid_for(total, kThreads, 8);
