@@ -388,6 +388,36 @@ size_t tsb_edge_labels_workspace_bytes(int n, int crop_h, int crop_w);
 int tsb_edge_labels(const long long* samples_dev, int n, int crop_h, int crop_w, int gt_pad, void* workspace,
                     size_t workspace_bytes, long long* out_aux, tsb_stream_t stream);
 
+/* ================================================================================================
+ * Evaluator (SURVEY §8 f2) — what Evaluator.sliding_eval / scale_process / whole_eval (torchseg_b200/engine/evaluator.py,
+ * TorchSeg furnace/engine/evaluator.py:163-251) do around the network forward, bit-identical to their cv2 / numpy / torch
+ * host path: one frame, one scale per call.
+ *
+ * tsb_eval_windows: uint8 HWC frame src[H][W][cin] (cin 1 = grey, replicated to 3 planes, or 3) → cv2.resize(src, None,
+ * fx, fx, INTER_LINEAR) of size (sh, sw) = (rint(H*fx), rint(W*fx)) — fixed point with coefficient scale 1/fx, INTER_AREA
+ * when 1/fx == 2, a copy when (sh, sw) == (H, W) (fx is then ignored) — placed at (top, left) of a padded canvas, then
+ * normalised through lut[3][256] (utils.gpu_pipeline.normalize_lut). Canvas pixels outside the frame are lut[c][0]
+ * (pad_zero = 0: the uint8 frame is padded, then normalised) or 0.0f (pad_zero = 1: normalised, then padded).
+ * out[n][3][wh][ww] fp32 = the canvas windows whose top-left corners are corners[n][2] = {y, x} (int32, device), mirrored
+ * left-right when `mirror`.
+ *
+ * tsb_eval_accumulate: lp[n][C][wh][ww] fp32 network log-probs of those windows and optionally lp_flip, the log-probs of
+ * the mirrored windows → acc[C][acc_h][acc_w] += exp(lp + mirror(lp_flip)) per window (accurate expf, fp32). Overlapping
+ * windows are SUMMED in window order (no atomics); pixels covered by no window are not touched.
+ *
+ * tsb_eval_resize_add: src = a strided fp32 [C][h][w] view (element (c, y, x) at c*plane_stride + y*row_stride + x)
+ * → cv2.resize(src as HWC, (W, H), INTER_LINEAR) in fp32 (a copy at the same size, INTER_AREA at an exact 2x down-scale)
+ * → total[C][H][W] (fp64) += resized. With pred != NULL the total is not stored; pred[H][W] (int64) receives the first
+ * index of the maximum of the updated total over C (numpy argmax). Bit-exact with cv2 for C not in {1, 3, 4}.
+ * ============================================================================================== */
+int tsb_eval_windows(const uint8_t* src, int H, int W, int cin, double fx, int sh, int sw, int top, int left,
+                     const float* lut, int pad_zero, const int* corners, int n, int wh, int ww, int mirror, float* out,
+                     tsb_stream_t stream);
+int tsb_eval_accumulate(const float* lp, const float* lp_flip, const int* corners, int n, int C, int wh, int ww,
+                        float* acc, int acc_h, int acc_w, tsb_stream_t stream);
+int tsb_eval_resize_add(const float* src, int C, int h, int w, long long plane_stride, long long row_stride,
+                        double* total, int H, int W, int64_t* pred, tsb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

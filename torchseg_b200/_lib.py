@@ -81,6 +81,9 @@ _SIGS = {
     "tsb_train_preprocess": [P, I, I, I, I, P, F, I, P, P, P],
     "tsb_edge_labels": [P, I, I, I, I, P, c_size_t, P, P],
     "tsb_p2p_allreduce_sum": [P, I, P, I, I, c_uint, P, I, I, P, P, P],
+    "tsb_eval_windows": [P, I, I, I, D, I, I, I, I, P, I, P, I, I, I, I, P, P],
+    "tsb_eval_accumulate": [P, P, P, I, I, I, I, P, I, I, P],
+    "tsb_eval_resize_add": [P, I, I, I, L, L, P, I, I, P, P],
 }
 EXPORTS = sorted(list(_SIGS) + ["tsb_last_error", "tsb_version", "tsb_launch_count", "tsb_p2p_buffer_bytes", "tsb_edge_labels_workspace_bytes"])
 

@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libtsb.so")
-SOURCES = ["tsb_api.cu", "ohem.cu", "resize_pool.cu", "bn.cu", "pack_opt.cu", "conv_igemm.cu", "conv_v2.cu", "conv_wgrad_taps.cu", "psa.cu", "p2p.cu", "data_pipeline.cu", "ce_up.cu", "dwconv.cu"]
+SOURCES = ["tsb_api.cu", "ohem.cu", "resize_pool.cu", "bn.cu", "pack_opt.cu", "conv_igemm.cu", "conv_v2.cu", "conv_wgrad_taps.cu", "psa.cu", "p2p.cu", "data_pipeline.cu", "ce_up.cu", "dwconv.cu", "eval.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -6,11 +6,12 @@
 // stay on the host (torchseg_b200/utils/gpu_pipeline.py) in the reference's order.
 //
 // Bit-exact by construction: OpenCV's 8-bit INTER_LINEAR is FIXED POINT (11-bit coefficients, int32 horizontal pass,
-// (((b0*(S0>>4))>>16) + ((b1*(S1>>4))>>16) + 2) >> 2 vertically — imgproc/src/resize.cpp); the coefficient arithmetic below
-// uses explicit IEEE double / float operations (no FMA contraction), and normalisation is a 3 x 256 table built on the host
+// (((b0*(S0>>4))>>16) + ((b1*(S1>>4))>>16) + 2) >> 2 vertically — imgproc/src/resize.cpp); the coefficient arithmetic
+// (resize_coef.cuh, shared with the evaluator) uses explicit IEEE double / float operations (no FMA contraction), and normalisation is a 3 x 256 table built on the host
 // with the reference's own float32 / float64 sequence. HBM-bound byte work: one thread per output pixel, coalesced
 // plane-wise stores (the 6 MB uint8 source of a Cityscapes frame replaces 20 MB of fp32 image + int64 label on the H2D path).
 #include "tsb_common.cuh"
+#include "resize_coef.cuh"
 
 namespace {
 
@@ -18,26 +19,6 @@ struct PreSample {           // mirror of the 10 x int64 descriptor row (include
     long long img, gt, H, W, flip, sh, sw, pos_h, pos_w, reserved;
 };
 
-struct Coef {
-    int i0, i1, w0, w1;
-};
-// resize.cpp: fx = (float)((dx + 0.5) * scale - 0.5); sx = cvFloor(fx); fx -= sx; [x only: clamp at the borders with fx = 0]
-__device__ __forceinline__ Coef linear_coef(int d, int src, int dst, bool border_zero) {
-    const double scale = __ddiv_rn(1.0, __ddiv_rn((double)dst, (double)src));
-    float f = (float)__dadd_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), -0.5);
-    int s = (int)floorf(f);
-    f = __fsub_rn(f, (float)s);
-    if (border_zero) {
-        if (s < 0) { f = 0.f; s = 0; }
-        if (s >= src - 1) { f = 0.f; s = src - 1; }
-    }
-    Coef c;
-    c.w0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
-    c.w1 = __float2int_rn(__fmul_rn(f, 2048.f));
-    c.i0 = min(max(s, 0), src - 1);
-    c.i1 = min(max(s + 1, 0), src - 1);
-    return c;
-}
 __device__ __forceinline__ int nearest_index(int d, int src, int dst) {   // x_ofs = min(cvFloor(x * ifx), size - 1)
     const double scale = __ddiv_rn(1.0, __ddiv_rn((double)dst, (double)src));
     const int s = (int)floor(__dmul_rn((double)d, scale));
@@ -75,7 +56,9 @@ train_preprocess_kernel(const PreSample* __restrict__ samples, int crop_h, int c
         *og = (long long)g[(size_t)gy * W + (flip ? W - 1 - gx : gx)];
     }
     // image: INTER_LINEAR, fixed point
-    const Coef cx = linear_coef(xs, W, sw, true), cy = linear_coef(ys, H, sh, false);
+    // random_scale passes dsize, so cv2's inv_scale is dst / src
+    const Coef cx = linear_coef(xs, W, __ddiv_rn((double)sw, (double)W), true);
+    const Coef cy = linear_coef(ys, H, __ddiv_rn((double)sh, (double)H), false);
     const int xa = flip ? W - 1 - cx.i0 : cx.i0, xb = flip ? W - 1 - cx.i1 : cx.i1;
     const uint8_t* p = reinterpret_cast<const uint8_t*>(S.img);
     const uint8_t* r0a = p + ((size_t)cy.i0 * W + xa) * 3;
@@ -87,9 +70,7 @@ train_preprocess_kernel(const PreSample* __restrict__ samples, int crop_h, int c
         const int cs = reverse_channels ? 2 - c : c;
         const int s0 = (int)r0a[cs] * cx.w0 + (int)r0b[cs] * cx.w1;
         const int s1 = (int)r1a[cs] * cx.w0 + (int)r1b[cs] * cx.w1;
-        int v = (((cy.w0 * (s0 >> 4)) >> 16) + ((cy.w1 * (s1 >> 4)) >> 16) + 2) >> 2;
-        v = min(max(v, 0), 255);
-        o[(size_t)c * plane] = __ldg(lut + c * 256 + v);
+        o[(size_t)c * plane] = __ldg(lut + c * 256 + linear_u8(cy, s0, s1));
     }
 }
 

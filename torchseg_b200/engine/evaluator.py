@@ -9,6 +9,12 @@ reference, so that predictions can be compared pixel by pixel: cv2 resizing of t
 accumulated score map back to the original size. Quirks kept: overlapping windows are SUMMED, not averaged
 (`score = data_scale`, evaluator.py:241-242); flipped scores are added before `exp` is taken.
 
+`sliding_eval_device` / `whole_eval_device` run all of that on the device instead (libtsb tsb_eval_windows,
+tsb_eval_accumulate, tsb_eval_resize_add): the uint8 frame is uploaded once, and the int64 prediction they return is
+identical, pixel for pixel, to what `sliding_eval` / `whole_eval` return for the same `val_func` (fp32 log-probs; image
+mean / std as float64, like the configs). Pair them with `metric.hist_info_torch` so that only the n_cl² confusion counts
+come back to the host.
+
 `multi_process_evaluation` / `worker` (evaluator.py:97-163): one spawned process per device, the dataset split in
 contiguous shreds, results returned through a queue; `run` uses it when more than one device is given. Not carried over:
 datasets / visualisation helpers."""
@@ -19,7 +25,9 @@ import numpy as np
 import torch
 
 from .logger import get_logger
-from ..utils.img_utils import normalize, pad_image_to_shape
+from .. import ops
+from ..utils.gpu_pipeline import normalize_lut
+from ..utils.img_utils import get_2dshape, normalize, pad_image_to_shape
 from ..utils.pyt_utils import ensure_dir, link_file, load_model
 
 logger = get_logger()
@@ -202,6 +210,80 @@ class Evaluator(object):
         score = score.permute(1, 2, 0).cpu().numpy()
         return cv2.resize(score, (ori_shape[1], ori_shape[0]), interpolation=cv2.INTER_LINEAR)
 
+    # ------------------------------------------------------------------ the same evaluation on the device
+    def sliding_eval_device(self, img, crop_size, stride_rate, device):
+        """sliding_eval with the resizes, windows, score sums and arg-max on the device: uint8 [rows, cols, 3] numpy frame →
+        int64 [rows, cols] device tensor, equal to sliding_eval(img, crop_size, stride_rate, device)"""
+        dev = _cuda_device(device)
+        src = torch.from_numpy(np.ascontiguousarray(img)).to(dev)
+        rows, cols = img.shape[:2]
+        total = torch.zeros((self.class_num, rows, cols), dtype=torch.float64, device=dev)     # sum over scales
+        pred = torch.zeros((rows, cols), dtype=torch.int64, device=dev)
+        for i, s in enumerate(self.multi_scales):
+            score = self._scale_process_device(src, s, crop_size, stride_rate, dev)
+            ops.eval_resize_add(score, total, pred if i == len(self.multi_scales) - 1 else None)
+        return pred
+
+    def whole_eval_device(self, img, output_size, input_size=None, device=None):
+        """whole_eval on the device: uint8 [rows, cols, 1 | 3] numpy frame → int64 device tensor of size output_size (or
+        the frame's), equal to whole_eval(img, output_size, input_size, device)"""
+        dev = _cuda_device(device)
+        src = torch.from_numpy(np.ascontiguousarray(img)).to(dev)
+        rows, cols = img.shape[:2]
+        th, tw = get_2dshape(input_size) if input_size is not None else (rows, cols)
+        win = (max(th, rows), max(tw, cols))                      # one window: the whole padded image
+        score = self._canvas_scores(src, None, rows, cols, (th, tw), True, [(0, 0)], win, dev, None)
+        out_h, out_w = (int(output_size[0]), int(output_size[1])) if output_size is not None else (rows, cols)
+        total = torch.zeros((score.shape[0], out_h, out_w), dtype=torch.float64, device=dev)
+        pred = torch.empty((out_h, out_w), dtype=torch.int64, device=dev)
+        ops.eval_resize_add(score, total, pred)
+        return pred
+
+    def _scale_process_device(self, src, s, crop_size, stride_rate, dev):
+        """scale_process for one scale: the margin-cropped [class, h, w] fp32 score view of the scaled frame. One window
+        (max side <= crop) pads the normalised image with 0.0, the sliding branch the uint8 image with 0."""
+        rows, cols = src.shape[:2]
+        sh, sw = int(round(rows * s)), int(round(cols * s))      # cv2's dsize for fx = fy = s (round half to even)
+        corners = self.window_grid(max(sh, crop_size), max(sw, crop_size), crop_size, stride_rate)
+        return self._canvas_scores(src, s, sh, sw, (crop_size, crop_size), max(sh, sw) <= crop_size, corners,
+                                   (crop_size, crop_size), dev, self.class_num)
+
+    def _canvas_scores(self, src, fx, sh, sw, pad_shape, pad_zero, corners, win, dev, class_num):
+        """the frame scaled by fx to (sh, sw), padded up to pad_shape (pad_image_to_shape's margins), cut into win-sized
+        windows at `corners`, crop_batch per forward, their scores summed on the canvas; returns the margin-cropped view"""
+        PH, PW = max(pad_shape[0], sh), max(pad_shape[1], sw)
+        ph, pw = PH - sh, PW - sw
+        m = (ph // 2, ph - ph // 2, pw // 2, pw - pw // 2)
+        wh, ww = win
+        lut = torch.from_numpy(normalize_lut(self.image_mean, self.image_std)).to(dev)
+        acc = None
+        for b0 in range(0, len(corners), self.crop_batch):
+            chunk = torch.tensor(corners[b0:b0 + self.crop_batch], dtype=torch.int32).to(dev)
+            x = ops.eval_windows(src, fx, sh, sw, m[0], m[2], lut, pad_zero, chunk, wh, ww)
+            xf = ops.eval_windows(src, fx, sh, sw, m[0], m[2], lut, pad_zero, chunk, wh, ww, mirror=True) if self.is_flip else None
+            lp, lpf = self._log_probs(x, xf, dev)
+            if acc is None:
+                C = lp.shape[1]
+                if class_num is not None and C != class_num:
+                    raise ValueError("val_func returns %d classes, the evaluator expects %d" % (C, class_num))
+                acc = torch.zeros((C, PH, PW), dtype=torch.float32, device=dev)
+            ops.eval_accumulate(lp, lpf, chunk, acc)
+        return acc[:, m[0]:PH - m[1], m[2]:PW - m[3]]
+
+    def _log_probs(self, x, xf, dev):
+        """the network calls of val_func_process (same module state, same order): log-probs of the windows and of the
+        mirrored windows, as contiguous fp32"""
+        self.val_func.eval()
+        if hasattr(self.val_func, "to"):
+            self.val_func.to(dev)
+        with torch.no_grad():
+            out = [self.val_func(x)] + ([self.val_func(xf)] if xf is not None else [])
+        for t in out:
+            if t.dtype != torch.float32:
+                raise TypeError("the device evaluator sums fp32 log-probs; val_func returned %s" % t.dtype)
+        out = [t.contiguous() for t in out]
+        return out[0], (out[1] if xf is not None else None)
+
     def val_func_process(self, input_data, device=None, batched=False):
         """evaluator.py:253-273: exp(log-prob(x) [+ flip(log-prob(flip(x)))]); returns [class, h, w] (or [n, class, h, w])"""
         arr = np.ascontiguousarray(input_data if batched else input_data[None], dtype=np.float32)
@@ -229,3 +311,13 @@ class Evaluator(object):
             p_img, margin = pad_image_to_shape(p_img, crop_size, cv2.BORDER_CONSTANT, value=0)
             return p_img.transpose(2, 0, 1), margin
         return p_img.transpose(2, 0, 1)
+
+
+def _cuda_device(device):
+    """the CUDA device of the device evaluator (None: the current one)"""
+    if device is None:
+        return torch.device("cuda", torch.cuda.current_device())
+    dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
+    if dev.type != "cuda":
+        raise ValueError("the device evaluator runs on a CUDA device, got %s" % dev)
+    return dev

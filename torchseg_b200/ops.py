@@ -1153,3 +1153,44 @@ def ohem_state_dict(state):
     return dict(num_valid=int(s[_lib.OHEM_ST_NUM_VALID]), count_le=int(s[_lib.OHEM_ST_COUNT_LE]),
                 active=bool(s[_lib.OHEM_ST_ACTIVE]), T=float(f[_lib.OHEM_ST_THRESH]), kept=int(s[_lib.OHEM_ST_KEPT]),
                 loss=float(f[_lib.OHEM_ST_LOSS]))
+
+
+# --------------------------------------------------------------------------------------------------
+# evaluator (engine/evaluator.py: sliding_eval_device / whole_eval_device), one frame and one scale per call
+# --------------------------------------------------------------------------------------------------
+def eval_windows(src, fx, sh, sw, top, left, lut, pad_zero, corners, wh, ww, mirror=False):
+    """uint8 [H,W,cin] frame on the device → cv2.resize(fx) → (sh, sw) at (top, left) of a padded canvas → normalised
+    through `lut` [3,256] → the [n,3,wh,ww] fp32 windows at `corners` (int32 [n,2] {y, x} on the device), optionally
+    mirrored. pad_zero: canvas padding is 0.0 instead of lut[c][0]."""
+    assert src.dtype == torch.uint8 and src.dim() == 3 and src.is_contiguous()
+    assert corners.dtype == torch.int32 and corners.is_contiguous() and lut.dtype == torch.float32
+    n = corners.shape[0]
+    out = torch.empty((n, 3, wh, ww), dtype=torch.float32, device=src.device)
+    H, W, cin = src.shape
+    call("tsb_eval_windows", ptr(src), H, W, cin, float(fx or 0.0), sh, sw, top, left, ptr(lut), int(bool(pad_zero)),
+         ptr(corners), n, wh, ww, int(bool(mirror)), ptr(out), stream())
+    return out
+
+
+def eval_accumulate(lp, lp_flip, corners, acc):
+    """acc [C,PH,PW] fp32 += exp(lp + mirror(lp_flip)) of each window at `corners`, in window order (overlaps SUMMED)"""
+    n, C, wh, ww = lp.shape
+    for t in (lp, lp_flip):
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or tuple(t.shape) != (n, C, wh, ww)):
+            raise TypeError("eval_accumulate: log-probs must be contiguous float32 [n, C, h, w] of one shape")
+    assert acc.dtype == torch.float32 and acc.is_contiguous() and acc.shape[0] == C
+    call("tsb_eval_accumulate", ptr(lp), ptr(lp_flip), ptr(corners), n, C, wh, ww, ptr(acc), acc.shape[1], acc.shape[2],
+         stream())
+    return acc
+
+
+def eval_resize_add(score, total, pred=None):
+    """total [C,H,W] fp64 += cv2.resize(score, (W, H), INTER_LINEAR) of a [C,h,w] fp32 view (any strides with a unit
+    column stride); with `pred` (int64 [H,W]) the first arg-max over C of the updated total is written instead"""
+    C, h, w = score.shape
+    assert score.dtype == torch.float32 and score.stride(2) == 1
+    assert total.dtype == torch.float64 and total.is_contiguous() and total.shape[0] == C
+    if pred is not None:
+        assert pred.dtype == torch.int64 and pred.is_contiguous() and tuple(pred.shape) == tuple(total.shape[1:])
+    call("tsb_eval_resize_add", ptr(score), C, h, w, score.stride(0), score.stride(1), ptr(total), total.shape[1],
+         total.shape[2], ptr(pred), stream())
