@@ -270,6 +270,24 @@ int tsb_conv2d_fprop_fused(const tsb_conv_shape* s, const void* x, int xcs, cons
  * were, and writes zeros there when accumulate == 0. */
 int tsb_conv2d_dgrad(const tsb_conv_shape* s, const void* dy, int dycs, const void* wt, void* dx, int dxcs,
                      int accumulate, tsb_stream_t stream);
+/* transposed convolution — replaces the nn.ConvTranspose2d of DeConvBnRelu (furnace/seg_opr/seg_oprs.py:49-73).
+ * ConvTranspose2d(Ci, Co, k, stride s, padding p, output_padding op, dilation d) maps x[N,Ci,H,W] to y[N,Co,Ho,Wo] with
+ * Ho = (H-1)*s - 2p + d(k-1) + op + 1. `s` describes the ADJOINT conv, whose dgrad this is: {N, H = Ho, W = Wo, C = Co,
+ * K = Ci, R = S = k, stride s, pad p, dil d, P = H, Q = W}. Its weight [K = Ci][C = Co][R][S] is the deconv weight
+ * W[Ci][Co][k][k] itself, so a channels_last ConvTranspose2d weight is the adjoint conv's KRSC, and
+ *   y       = tsb_conv_transpose2d_fprop(x, wt)       wt = flipped [Co][k][k][Ci] pack (tsb_pack_weight's second output)
+ *   dx      = tsb_conv2d_fprop(dy)                     with the [Ci][k][k][Co] pack
+ *   dW      = tsb_conv2d_wgrad(x := dy, dy := x)       straight into W's KRSC storage
+ *   dbias   = tsb_bias_grad(dy)
+ * The geometry limits follow: s in {1, 2}, k <= 4 (16 taps), square kernel / stride / pad / dilation, groups 1, and
+ * op < s (otherwise the adjoint conv's output is not H x W and P, Q are rejected as inconsistent). Ci % 64 == 0,
+ * Co % 8 == 0 (xcs >= Ci, ycs >= Co, multiples of 8). Epilogue as tsb_conv2d_fprop plus ReLU: y = relu?(acc + bias), bf16
+ * or fp32; optional statistics of the rounded bf16 outputs added into sum[Co], sumsq[Co] (caller zeroes). Stride 2 runs
+ * one launch per output parity class; positions no tap reaches (k = 1) hold relu?(bias) (0 without bias) and count in
+ * the statistics, and the slots of all classes are summed in a fixed order. */
+int tsb_conv_transpose2d_fprop(const tsb_conv_shape* s, const void* x, int xcs, const void* wt, const float* bias, int relu,
+                               void* y, int ydtype, int ycs, float* sum, float* sumsq, float* ws, long long ws_floats,
+                               tsb_stream_t stream);
 /* wgrad: dw[K,R,S,C] (fp32, KRSC) += Σ_pixels dy ⊗ x (caller zeroes or accumulates); xcs >= C, dycs >= K (any K).
  * The per-split partial sums go to ws and are added in a fixed order, so the result is bit-reproducible; without a
  * workspace large enough for two splits the kernel adds into dw in place. */

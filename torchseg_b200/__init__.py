@@ -10,12 +10,13 @@ __version__ = "0.1.0"
 
 
 def prepare_model(model):
-    """Put every nn.Conv2d weight into KRSC (channels_last) physical layout in place — the layout the TMA
-    descriptors of the conv kernels read and the wgrad kernel accumulates into. Values, shapes, parameter
-    identity and state_dict keys are unchanged."""
+    """Put every nn.Conv2d and nn.ConvTranspose2d weight into KRSC (channels_last) physical layout in place — the
+    layout the TMA descriptors of the conv kernels read and the wgrad kernel accumulates into (for a ConvTranspose2d
+    weight [Ci][Co][k][k], the KRSC of its adjoint conv). Values, shapes, parameter identity and state_dict keys are
+    unchanged."""
     import torch
     for m in model.modules():
-        if isinstance(m, nn.Conv2d):
+        if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
             w = m.weight.data
             K, C, R, S = w.shape
             krsc = w.permute(0, 2, 3, 1).contiguous()

@@ -66,6 +66,7 @@ _SIGS = {
     "tsb_conv_stem_fprop_fused": [P, I, I, I, P, I, P, I, P, I, P],
     "tsb_conv2d_dgrad": [P, P, I, P, P, I, I, P],
     "tsb_conv2d_wgrad": [P, P, I, P, I, P, P, L, P],
+    "tsb_conv_transpose2d_fprop": [P, P, I, P, P, I, P, I, I, P, P, P, L, P],
     "tsb_conv_stem_fprop": [P, I, I, I, P, I, P, I, P, P, P, L, P],
     "tsb_conv_stem_wgrad": [P, I, I, I, P, I, I, P, P, L, P],
     "tsb_bias_grad": [P, I, L, I, P, P, L, P],

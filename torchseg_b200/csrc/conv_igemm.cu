@@ -1,6 +1,7 @@
 // im2col-free implicit-GEMM convolution on Hopper wgmma tensor cores (sm_90a): the C ABI entry points.
 //
 //   fprop / dgrad / stem : the persistent kernel of conv_v2.cu;
+//   transposed fprop     : the dgrad-form launches with the fprop epilogue (bias, ReLU, bf16/fp32, BN statistics);
 //   wgrad                : the nine-tap kernel (3x3 stride 1, conv_wgrad_taps.cu), the row-tile kernel (long rows,
 //                          conv_v2.cu), else the generic kernel below:
 //                          D[128 out-ch, 64*nb in-ch] += dY^T[128, 64 px] * X_shift[64 px, 64*nb]; both operands are
@@ -203,21 +204,21 @@ extern "C" int tsb_conv2d_fprop_fused(const tsb_conv_shape* s, const void* x, in
     return fprop_impl(s, x, xcs, w, bias, y, ydtype, ycs, nullptr, nullptr, nullptr, 0, res, relu != 0, stream);
 }
 
-extern "C" int tsb_conv2d_dgrad(const tsb_conv_shape* s, const void* dy, int dycs, const void* wt, void* dx, int dxcs,
-                                int accumulate, tsb_stream_t stream) {
-    int rc = check_conv_shape(s, "tsb_conv2d_dgrad");
-    if (rc) return rc;
-    TSB_REQUIRE(dy && wt && dx, "tsb_conv2d_dgrad: null pointer");
-    TSB_REQUIRE(s->K % 64 == 0, "tsb_conv2d_dgrad: K must be a multiple of 64 (pad the classifier to 64), got %d", s->K);
-    TSB_REQUIRE(s->C % 8 == 0 && dycs % 8 == 0 && dycs >= s->K && dxcs % 8 == 0 && dxcs >= s->C && tsb_aligned16(dy) && tsb_aligned16(dx) && tsb_aligned16(wt),
-                "tsb_conv2d_dgrad: alignment");
-    cudaStream_t st = (cudaStream_t)stream;
+// The dgrad-form launches of conv geometry `s`: out[N,H,W,·] (channel stride ocs) = the transposed convolution of
+// act[N,P,Q,K] (channel stride acs) by the conv's weight, read through the flipped pack wt [C][R][S][K]. Stride 1 is one
+// launch; stride 2 is one launch per parity class (ph, pw) of the output, over that class's strided sub-grid, with the
+// taps that reach it. A class no tap reaches (a 1x1 kernel at stride 2) runs with no taps, so its positions receive
+// the epilogue of a zero accumulator. `epi` carries the epilogue fields (bias, relu, out_f32, k_store, accumulate,
+// sum/sumsq, ws). With statistics each launch leaves its per-CTA slots in the workspace after those of the previous
+// class, and all slots are added in class order, then CTA order, at the end: the result repeats bit for bit.
+static int adjoint_launches(const tsb_conv_shape* s, const void* act, int acs, const void* wt, void* out, int ocs,
+                            const convv2::Desc& epi, const char* who, cudaStream_t st) {
     const int classes = (s->stride == 1) ? 1 : 4;
+    int slots = 0;   // statistics slots written so far, 2 * C floats each
     for (int cls = 0; cls < classes; ++cls) {
         const int ph = cls >> 1, pw = cls & 1;
-        convv2::Desc d;
-        memset(&d, 0, sizeof(d));
-        int N = s->N, P = s->P, Q = s->Q;          // dY geometry (the A operand)
+        convv2::Desc d = epi;
+        int N = s->N, P = s->P, Q = s->Q;          // act geometry (the A operand)
         int Hl, Wl;                                 // launch output grid
         const bool flat = (s->R == 1 && s->stride == 1 && s->pad == 0);
         if (s->stride == 1) { Hl = s->H; Wl = s->W; }
@@ -225,7 +226,7 @@ extern "C" int tsb_conv2d_dgrad(const tsb_conv_shape* s, const void* dy, int dyc
         if (Hl <= 0 || Wl <= 0) continue;
         if (flat) {
             long long npix = (long long)N * P * Q;
-            TSB_REQUIRE(npix < (1ll << 31), "tsb_conv2d_dgrad: too many pixels");
+            TSB_REQUIRE(npix < (1ll << 31), "%s: too many pixels", who);
             Q = (int)npix; P = 1; N = 1; Hl = 1; Wl = Q;
         }
         int nt = 0;
@@ -244,28 +245,75 @@ extern "C" int tsb_conv2d_dgrad(const tsb_conv_shape* s, const void* dy, int dyc
             }
         }
         if (flat) {
-            d.out_n_stride = 0; d.out_p_stride = 0; d.out_q_stride = dxcs; d.out_base = 0;
+            d.out_n_stride = 0; d.out_p_stride = 0; d.out_q_stride = ocs; d.out_base = 0;
         } else if (s->stride == 1) {
-            d.out_n_stride = (long long)s->H * s->W * dxcs;
-            d.out_p_stride = (long long)s->W * dxcs;
-            d.out_q_stride = dxcs;
+            d.out_n_stride = (long long)s->H * s->W * ocs;
+            d.out_p_stride = (long long)s->W * ocs;
+            d.out_q_stride = ocs;
             d.out_base = 0;
         } else {
-            d.out_n_stride = (long long)s->H * s->W * dxcs;
-            d.out_p_stride = (long long)2 * s->W * dxcs;
-            d.out_q_stride = (long long)2 * dxcs;
-            d.out_base = ((long long)ph * s->W + pw) * dxcs;
+            d.out_n_stride = (long long)s->H * s->W * ocs;
+            d.out_p_stride = (long long)2 * s->W * ocs;
+            d.out_q_stride = (long long)2 * ocs;
+            d.out_base = ((long long)ph * s->W + pw) * ocs;
         }
-        d.act = dy; d.aN = N; d.aH = P; d.aW = Q; d.aC = s->K; d.acs = dycs; d.act_stride = 1; d.flat = flat;
+        d.act = act; d.aN = N; d.aH = P; d.aW = Q; d.aC = s->K; d.acs = acs; d.act_stride = 1; d.flat = flat;
         d.ntaps = nt; d.kchunks = s->K / 64;
         d.w = wt; d.w_rows = s->C; d.w_k = (long long)s->R * s->S * s->K; d.ncols = s->C;
         d.Nl = N; d.Pl = Hl; d.Ql = Wl;
-        d.k_real = s->C; d.k_store = s->C; d.out_f32 = 0; d.accumulate = accumulate;
-        d.out = dx;
-        rc = convv2::launch(d, st);
+        d.k_real = s->C;
+        d.out = out;
+        int used = 0;
+        if (epi.sum != nullptr) {
+            const long long off = (long long)slots * 2 * s->C;
+            TSB_REQUIRE(epi.ws && off < epi.ws_floats, "%s: statistics workspace too small", who);
+            d.ws = epi.ws + off; d.ws_floats = epi.ws_floats - off;
+        }
+        const int rc = convv2::launch(d, st, epi.sum != nullptr ? &used : nullptr);
         if (rc) return rc;
+        slots += used;
     }
-    return TSB_OK;
+    if (epi.sum == nullptr || slots == 0) return TSB_OK;
+    const int rc = tsb_det_reduce(epi.sum, epi.ws, slots, s->C, 2LL * s->C, st);
+    // the sumsq slots follow the sum slots of the same CTA: a stride of 2·C between slots
+    return rc ? rc : tsb_det_reduce(epi.sumsq, epi.ws + s->C, slots, s->C, 2LL * s->C, st);
+}
+
+extern "C" int tsb_conv2d_dgrad(const tsb_conv_shape* s, const void* dy, int dycs, const void* wt, void* dx, int dxcs,
+                                int accumulate, tsb_stream_t stream) {
+    int rc = check_conv_shape(s, "tsb_conv2d_dgrad");
+    if (rc) return rc;
+    TSB_REQUIRE(dy && wt && dx, "tsb_conv2d_dgrad: null pointer");
+    TSB_REQUIRE(s->K % 64 == 0, "tsb_conv2d_dgrad: K must be a multiple of 64 (pad the classifier to 64), got %d", s->K);
+    TSB_REQUIRE(s->C % 8 == 0 && dycs % 8 == 0 && dycs >= s->K && dxcs % 8 == 0 && dxcs >= s->C && tsb_aligned16(dy) && tsb_aligned16(dx) && tsb_aligned16(wt),
+                "tsb_conv2d_dgrad: alignment");
+    convv2::Desc epi;
+    memset(&epi, 0, sizeof(epi));
+    epi.k_store = s->C; epi.accumulate = accumulate;
+    return adjoint_launches(s, dy, dycs, wt, dx, dxcs, epi, "tsb_conv2d_dgrad", (cudaStream_t)stream);
+}
+
+extern "C" int tsb_conv_transpose2d_fprop(const tsb_conv_shape* s, const void* x, int xcs, const void* wt, const float* bias,
+                                          int relu, void* y, int ydtype, int ycs, float* sum, float* sumsq, float* ws,
+                                          long long ws_floats, tsb_stream_t stream) {
+    int rc = check_conv_shape(s, "tsb_conv_transpose2d_fprop");
+    if (rc) return rc;
+    TSB_REQUIRE(x && wt && y, "tsb_conv_transpose2d_fprop: null pointer");
+    TSB_REQUIRE(s->K % 64 == 0, "tsb_conv_transpose2d_fprop: input channels (K of the adjoint conv) must be a multiple of 64, got %d", s->K);
+    TSB_REQUIRE(s->C % 8 == 0, "tsb_conv_transpose2d_fprop: output channels (C of the adjoint conv) must be a multiple of 8, got %d", s->C);
+    TSB_REQUIRE(xcs % 8 == 0 && xcs >= s->K && tsb_aligned16(x) && tsb_aligned16(wt),
+                "tsb_conv_transpose2d_fprop: x channel stride must be a multiple of 8 and at least K (got xcs %d, K %d)", xcs, s->K);
+    TSB_REQUIRE(ydtype == TSB_BF16 || ydtype == TSB_F32, "tsb_conv_transpose2d_fprop: bad ydtype");
+    TSB_REQUIRE(ycs % 8 == 0 && ycs >= s->C && tsb_aligned16(y),
+                "tsb_conv_transpose2d_fprop: y channel stride must be a multiple of 8 and at least C (got ycs %d, C %d)", ycs, s->C);
+    TSB_REQUIRE((sum == nullptr) == (sumsq == nullptr), "tsb_conv_transpose2d_fprop: sum and sumsq go together");
+    TSB_REQUIRE(!(sum && ydtype != TSB_BF16), "tsb_conv_transpose2d_fprop: statistics need bf16 output");
+    convv2::Desc epi;
+    memset(&epi, 0, sizeof(epi));
+    epi.k_store = s->C; epi.out_f32 = (ydtype == TSB_F32);
+    epi.bias = bias; epi.relu = relu != 0; epi.sum = sum; epi.sumsq = sumsq;
+    epi.ws = ws; epi.ws_floats = ws_floats;
+    return adjoint_launches(s, x, xcs, wt, y, ycs, epi, "tsb_conv_transpose2d_fprop", (cudaStream_t)stream);
 }
 
 namespace {

@@ -261,7 +261,9 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_cons
                     }
                 }
                 if (do_stats) {
-                    // every value the statistics see, in the order of the fragment rows of one 128-pixel tile
+                    // every value the statistics see, in the order of the fragment rows of one 128-pixel tile; (pp, qq)
+                    // are launch-grid coordinates (a stride-2 parity class's own sub-grid for the transposed forward), so
+                    // only the stores above use the output strides
                     asm volatile("bar.sync 1, %0;" ::"n"(kConsumers * 128) : "memory");
 #pragma unroll
                     for (int s = 0; s < 2; ++s) {
@@ -499,7 +501,7 @@ int launch_v2(const V2Params& prm, int grid_x, int n_tiles, size_t smem, cudaStr
 
 namespace convv2 {
 
-int launch(const Desc& d, cudaStream_t st) {
+int launch(const Desc& d, cudaStream_t st, int* stat_slots) {
     V2Params prm;
     memset(&prm, 0, sizeof(prm));
     const int BN = (d.ncols <= 64) ? 64 : 128;
@@ -604,6 +606,7 @@ int launch(const Desc& d, cudaStream_t st) {
     int rc2 = (BN == 64) ? (resident ? launch_v2<64, true>(prm, grid_x, n_tiles, smem, st) : launch_v2<64, false>(prm, grid_x, n_tiles, smem, st))
                          : (resident ? launch_v2<128, true>(prm, grid_x, n_tiles, smem, st) : launch_v2<128, false>(prm, grid_x, n_tiles, smem, st));
     if (rc2 || d.sum == nullptr) return rc2;
+    if (stat_slots != nullptr) { *stat_slots = grid_x; return TSB_OK; }
     rc2 = tsb_det_reduce(d.sum, prm.part, grid_x, d.k_real, 2LL * d.k_real, st);
     if (rc2) return rc2;
     // the sumsq slots follow the sum slots of the same CTA: a stride of 2·k_real between CTAs

@@ -47,7 +47,9 @@ struct WgradDesc {
     long long ws_floats;
 };
 
-int launch(const Desc& d, cudaStream_t st);
+// With statistics and `stat_slots`, the per-CTA statistics are left in d.ws ([slot][2][k_real], one slot per CTA) and
+// their count is returned in *stat_slots for the caller to reduce; otherwise they are added into d.sum / d.sumsq here.
+int launch(const Desc& d, cudaStream_t st, int* stat_slots = nullptr);
 int launch_wgrad_rows(const WgradDesc& d, cudaStream_t st);
 int launch_wgrad_taps(const WgradDesc& d, int R, int pad, int dil, cudaStream_t st);   // conv_wgrad_taps.cu
 

@@ -78,6 +78,18 @@ def make_shape(N, H, W, C, K, R, stride, pad, dil):
     return ConvShape(N, H, W, C, K, R, R, stride, pad, dil, P, Q)
 
 
+def deconv_out_size(H, k, stride, pad, dil, out_pad):
+    return (H - 1) * stride - 2 * pad + dil * (k - 1) + out_pad + 1
+
+
+def make_deconv_shape(N, H, W, Ci, Co, k, stride, pad, dil, out_pad):
+    """the ADJOINT conv of ConvTranspose2d(Ci, Co, k, stride, pad, out_pad, dil) on an H x W input (include/tsb.h): an
+    ordinary conv from Ho x Wo x Co to H x W x Ci with the deconv weight as its [K = Ci][C = Co][R][S] weight"""
+    Ho = deconv_out_size(H, k, stride, pad, dil, out_pad)
+    Wo = deconv_out_size(W, k, stride, pad, dil, out_pad)
+    return ConvShape(N, Ho, Wo, Co, Ci, k, k, stride, pad, dil, H, W)
+
+
 # --------------------------------------------------------------------------------------------------
 # bf16 weight packs, cached per optimiser step
 # --------------------------------------------------------------------------------------------------
@@ -350,6 +362,22 @@ def conv_fprop(x, wb, K, R, stride, pad, dil, bias=None, out_dtype=_BF, out=None
     return out
 
 
+def conv_transpose_fprop(x, wt, Co, R, stride, pad, dil, out_pad, bias=None, relu=False, out_dtype=_BF, out=None,
+                        stats=None):
+    """y = relu?(conv_transpose(x, W) + bias) on the dgrad-form launches (tsb_conv_transpose2d_fprop); wt is the flipped
+    [Co][R][S][Ci] pack of the deconv weight W [Ci][Co][R][S]; optional BN statistics of the rounded output"""
+    N, Ci, H, W = x.shape
+    shp = make_deconv_shape(N, H, W, Ci, Co, R, stride, pad, dil, out_pad)
+    if out is None:
+        out = nhwc_empty(N, Co, shp.H, shp.W, dtype=out_dtype, device=x.device)
+    s1, s2 = (None, None) if stats is None else (stats[0], stats[1])
+    ev = conv_prof.begin()
+    call("tsb_conv_transpose2d_fprop", ctypes.byref(shp), ptr(x), cs_of(x), ptr(wt), ptr(bias), int(relu), ptr(out),
+         _lib.dt(out), cs_of(out), ptr(s1), ptr(s2), *det_ws(), stream())
+    conv_prof.end(ev, _conv_flops(shp))
+    return out
+
+
 def conv_fprop_fused(x, wb, K, R, stride, pad, dil, bias, res=None, relu=False):
     """inference conv with the BatchNorm folded into (wb, bias): y = relu?(conv(x) + bias (+ res)) in ONE kernel
     (tsb_conv2d_fprop_fused) — no raw tensor, no separate normalisation pass"""
@@ -385,19 +413,27 @@ class _FoldCache(object):
     def __init__(self):
         self.cache = {}
 
-    def get(self, w, bn, stem):
+    def get(self, w, bn, stem, transposed=False):
+        """transposed: w is a ConvTranspose2d weight [Ci][Co][R][S]; its output channels are the C axis of the KRSC view,
+        so the scale runs along C and the returned pack is the flipped [Co][R][S][Ci] operand of the transposed fprop"""
         key = (id(w), id(bn))
         ver = (w.data_ptr(), w._version, bn.weight._version, bn.bias._version, bn.running_mean._version,
-               bn.running_var._version, pack_cache.step, bool(stem))
+               bn.running_var._version, pack_cache.step, bool(stem), bool(transposed))
         hit = self.cache.get(key)
         if hit is not None and hit[0] == ver and hit[3]() is w:
             return hit[1], hit[2]
         with torch.no_grad():
             scale = (bn.weight.float() / torch.sqrt(bn.running_var.float() + bn.eps))
             bias = (bn.bias.float() - bn.running_mean.float() * scale).contiguous()
-            wk = (_krsc_ptr(w).float() * scale[:, None, None, None]).contiguous()
+            if transposed:
+                wk = (_krsc_ptr(w).float() * scale[None, None, None, :]).contiguous()
+            else:
+                wk = (_krsc_ptr(w).float() * scale[:, None, None, None]).contiguous()
             K, R, S, C = wk.shape
-            if stem:
+            if transposed:
+                wb = torch.empty((C, R, S, K), dtype=_BF, device=w.device)
+                call("tsb_pack_weight", ptr(wk), K, R, S, C, None, ptr(wb), stream())
+            elif stem:
                 wb = torch.empty((K, 4, 4, 16), dtype=_BF, device=w.device)
                 call("tsb_pack_stem_weight", ptr(wk), K, R, ptr(wb), stream())
             else:
@@ -486,14 +522,21 @@ class ConvBNActFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, w, gamma, beta, residual, running_mean, running_var, stride, pad, dil, relu, eps, momentum,
-                training, stem, in_share=None, res_share=None):
-        K = w.shape[0]
+                training, stem, in_share=None, res_share=None, out_pad=None):
+        # out_pad is not None: w is a ConvTranspose2d weight [Ci][Co][R][S] (DeConvBnRelu, seg_oprs.py:49-73) and the
+        # three conv calls are those of the adjoint conv (include/tsb.h): transposed fprop, fprop for dx, wgrad with x
+        # and dy exchanged for dW
+        transposed = out_pad is not None
+        K = w.shape[1] if transposed else w.shape[0]
         R = w.shape[2]
         dev = x.device
         if stem:
             N, _, H2, WP = x.shape  # xs2d [N, 16, H/2, W/2+4]
             H, W = H2 * 2, (WP - 4) * 2
             P, Q = H2, WP - 4
+        elif transposed:
+            N, C, H, W = x.shape
+            P, Q = deconv_out_size(H, R, stride, pad, dil, out_pad), deconv_out_size(W, R, stride, pad, dil, out_pad)
         else:
             N, C, H, W = x.shape
             P, Q = conv_out_size(H, R, stride, pad, dil), conv_out_size(W, R, stride, pad, dil)
@@ -506,6 +549,9 @@ class ConvBNActFn(torch.autograd.Function):
             call("tsb_conv_stem_fprop", ptr(x), N, H, W, ptr(wp), K, ptr(raw), K, ptr(stats[0]) if training else None,
                  ptr(stats[1]) if training else None, *det_ws(), stream())
             conv_prof.end(ev, 2.0 * N * P * Q * K * 147)
+        elif transposed:
+            _, wt = pack_cache.get(w, True)
+            conv_transpose_fprop(x, wt, K, R, stride, pad, dil, out_pad, out=raw, stats=stats)
         else:
             wb, _ = pack_cache.get(w, False)
             conv_fprop(x, wb, K, R, stride, pad, dil, out=raw, stats=stats)
@@ -524,7 +570,7 @@ class ConvBNActFn(torch.autograd.Function):
              int(relu), ptr(y), K, N * P * Q, K, stream())
         ctx.save_for_backward(x, w, gamma, raw, y, aux)
         ctx.beta_ref = beta
-        ctx.cfg = (stride, pad, dil, relu, stem, residual is not None, count, training)
+        ctx.cfg = (stride, pad, dil, relu, stem, residual is not None, count, training, transposed)
         # gradient sharing at a fork (GradShare): in_share — this conv's input x has other consumers in the same block;
         # res_share — the residual IS that x. The contributors chain their input gradients through one buffer (dgrad
         # epilogue accumulate) instead of handing autograd several tensors to add.
@@ -535,9 +581,9 @@ class ConvBNActFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x, w, gamma, raw, y, aux = ctx.saved_tensors
-        stride, pad, dil, relu, stem, has_res, count, training = ctx.cfg
+        stride, pad, dil, relu, stem, has_res, count, training, transposed = ctx.cfg
         assert training, "backward through eval-mode BN is not supported"
-        K = w.shape[0]
+        K = w.shape[1] if transposed else w.shape[0]
         R = w.shape[2]
         N, _, P, Q = raw.shape
         dev = dy.device
@@ -579,6 +625,12 @@ class ConvBNActFn(torch.autograd.Function):
             call("tsb_conv_stem_wgrad", ptr(x), N, H, W, ptr(draw), K, K, ptr(dwp), *det_ws(), stream())
             conv_prof.end(ev, 2.0 * N * P * Q * K * 147)
             call("tsb_unpack_stem_wgrad", ptr(dwp), K, R, ptr(dw), stream())
+        elif transposed:
+            Ci = w.shape[0]
+            conv_wgrad(draw, x, Ci, R, stride, pad, dil, dw)
+            if ctx.needs_input_grad[0]:
+                wb, _ = pack_cache.get(w, False)
+                dx = conv_fprop(draw, wb, Ci, R, stride, pad, dil)
         else:
             conv_wgrad(x, draw, K, R, stride, pad, dil, dw)
             if ctx.needs_input_grad[0]:
@@ -595,7 +647,7 @@ class ConvBNActFn(torch.autograd.Function):
             dres = ctx.res_share.contribute(dres)
         if direct:
             _notify(w, gamma, beta)
-        return dx, dw_view, dgamma, dbeta, dres, None, None, None, None, None, None, None, None, None, None, None, None
+        return dx, dw_view, dgamma, dbeta, dres, None, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 class StemPairFn(torch.autograd.Function):
@@ -730,6 +782,55 @@ class ConvFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             _, wt = pack_cache.get(w, True, pad_k=Kp)
             dx = conv_dgrad(dyb, wt, x.shape, Kp, R, stride, pad, dil)
+        if direct:
+            _notify(*([w, ctx.bias_ref] if has_bias else [w]))
+        return dx, dw_view, db, None, None, None, None, None
+
+
+class ConvTransposeFn(torch.autograd.Function):
+    """BN-free transposed convolution (+bias) (+ReLU in the epilogue), bf16 output: DeConvBnRelu with has_bn=False
+    (seg_oprs.py:49-73). w is the ConvTranspose2d weight [Ci][Co][R][S] in KRSC storage, Ci and Co multiples of 64 (the
+    module zero-pads ragged layers); the backward runs the adjoint conv's fprop (dx) and wgrad (dW), and tsb_bias_grad."""
+
+    @staticmethod
+    def forward(ctx, x, w, bias, stride, pad, dil, out_pad, relu):
+        Ci, Co, R, _ = w.shape
+        _, wt = pack_cache.get(w, True)
+        y = conv_transpose_fprop(x, wt, Co, R, stride, pad, dil, out_pad, bias=bias, relu=relu)
+        ctx.save_for_backward(x, w, y if relu else None)
+        ctx.bias_ref = bias
+        ctx.cfg = (stride, pad, dil, relu, bias is not None)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, y = ctx.saved_tensors
+        stride, pad, dil, relu, has_bias = ctx.cfg
+        Ci, Co, R, _ = w.shape
+        N, _, P, Q = dy.shape
+        dev = dy.device
+        if dy.dtype != _BF or dy.stride(1) != 1:
+            dy = to_nhwc(dy)
+        if relu:
+            dz = nhwc_empty(N, Co, P, Q, device=dev)
+            call("tsb_relu_bwd", ptr(dy), cs_of(dy), ptr(y), cs_of(y), ptr(dz), Co, N * P * Q, Co, stream())
+            dy = dz
+        direct = _direct_grad(w) and (not has_bias or _direct_grad(ctx.bias_ref))
+        if direct:
+            dw_view, dw = None, w.grad.permute(0, 2, 3, 1)
+        else:
+            dw_view, dw = _new_wgrad(w)
+        conv_wgrad(dy, x, Ci, R, stride, pad, dil, dw)
+        db = None
+        if has_bias:
+            db = ctx.bias_ref.grad if direct else torch.zeros((Co,), dtype=torch.float32, device=dev)
+            call("tsb_bias_grad", ptr(dy), cs_of(dy), N * P * Q, Co, ptr(db), *det_ws(), stream())
+            if direct:
+                db = None
+        dx = None
+        if ctx.needs_input_grad[0]:
+            wb, _ = pack_cache.get(w, False)
+            dx = conv_fprop(dy, wb, Ci, R, stride, pad, dil)
         if direct:
             _notify(*([w, ctx.bias_ref] if has_bias else [w]))
         return dx, dw_view, db, None, None, None, None, None

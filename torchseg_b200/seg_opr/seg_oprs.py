@@ -168,6 +168,84 @@ class ConvBnRelu(nn.Module):
         return y
 
 
+def _deconv_geometry(conv):
+    """(k, stride, pad, dil, out_pad) of an nn.ConvTranspose2d the transposed-conv kernels run (include/tsb.h)"""
+    k, st, pd, dl, op = (conv.kernel_size, conv.stride, conv.padding, conv.dilation, conv.output_padding)
+    if k[0] != k[1] or st[0] != st[1] or pd[0] != pd[1] or dl[0] != dl[1] or op[0] != op[1]:
+        raise NotImplementedError("DeConvBnRelu: non-square kernel, stride, padding, dilation or output padding")
+    if conv.groups != 1:
+        raise NotImplementedError("DeConvBnRelu: groups > 1 is not on the accelerated path")
+    if st[0] not in (1, 2):
+        raise NotImplementedError("DeConvBnRelu: stride must be 1 or 2 (got %d)" % st[0])
+    if k[0] > 4:
+        raise NotImplementedError("DeConvBnRelu: kernel size must be at most 4 (16 taps; got %d)" % k[0])
+    if op[0] >= st[0]:
+        raise NotImplementedError("DeConvBnRelu: output_padding must be smaller than the stride")
+    if not isinstance(pd[0], int):
+        raise NotImplementedError("DeConvBnRelu: string padding is not supported")
+    return k[0], st[0], pd[0], dl[0], op[0]
+
+
+def deconv_bn_act(x, conv, bn, relu):
+    """nn.ConvTranspose2d → norm_layer(train/eval) → ReLU (bn None: → +bias → ReLU) on the libtsb path. Channel counts
+    that are not multiples of 64 run zero-padded to the next multiple, as `_ragged` layers do; the output has exactly
+    conv.out_channels channels."""
+    k, stride, pad, dil, op = _deconv_geometry(conv)
+    xin = _as_act(x)
+    w, b = conv.weight, conv.bias
+    Ci, Co = conv.in_channels, conv.out_channels
+    Cp, Kp = _ceil_to(Ci, 64), _ceil_to(Co, 64)
+    padded = Cp != Ci or Kp != Co or xin.shape[1] != Ci
+    if padded:
+        if xin.shape[1] != Cp:
+            xin = _pad_act(xin[:, :Ci], Cp)
+        w = _pad_weight(w, Cp, Kp)   # [Ci][Co] → [Cp][Kp]: the same zero-padding of both leading dims
+    if bn is None:
+        if b is not None and padded:
+            b = _pad_vec(b, Kp)
+        y = ops.ConvTransposeFn.apply(xin, w, b, stride, pad, dil, op, bool(relu))
+        return y[:, :Co] if Kp != Co else y
+    if b is not None:
+        raise NotImplementedError("DeConvBnRelu with both bias and BN is not on the accelerated path")
+    momentum = bn.momentum if bn.momentum is not None else 0.1
+    gamma, beta, rm, rv = bn.weight, bn.bias, bn.running_mean, bn.running_var
+    if (not bn.training) and EVAL_FOLD_BN and not padded and not torch.is_grad_enabled():
+        # inference: W' = W·γ/σ along Co, b' = β − μ·γ/σ, epilogue = + b' → ReLU
+        wt, bias = ops.fold_cache.get(conv.weight, bn, False, transposed=True)
+        return ops.conv_transpose_fprop(xin, wt, Co, k, stride, pad, dil, op, bias=bias, relu=bool(relu))
+    if padded:
+        gamma, beta = _pad_vec(gamma, Kp, 1.0), _pad_vec(beta, Kp)
+        with torch.no_grad():
+            rm, rv = _pad_vec(rm, Kp), _pad_vec(rv, Kp, 1.0)
+    y = ops.ConvBNActFn.apply(xin, w, gamma, beta, None, rm, rv, stride, pad, dil, bool(relu), float(bn.eps),
+                              float(momentum), bool(bn.training), False, None, None, op)
+    if padded and bn.training and rm is not bn.running_mean:
+        with torch.no_grad():
+            bn.running_mean.copy_(rm[:Co])
+            bn.running_var.copy_(rv[:Co])
+    return y[:, :Co] if Kp != Co else y
+
+
+class DeConvBnRelu(nn.Module):
+    """seg_oprs.py:49-73 — same ctor, children named conv (a genuine nn.ConvTranspose2d) / bn / relu. Runs stride 1 or
+    2, kernel <= 4, square geometry, groups 1, output_pad < stride; anything else raises NotImplementedError."""
+
+    def __init__(self, in_planes, out_planes, ksize, stride, pad, output_pad, dilation=1, groups=1, has_bn=True,
+                 norm_layer=nn.BatchNorm2d, bn_eps=1e-5, has_relu=True, inplace=True, has_bias=False):
+        super(DeConvBnRelu, self).__init__()
+        self.conv = nn.ConvTranspose2d(in_planes, out_planes, kernel_size=ksize, stride=stride, padding=pad,
+                                       output_padding=output_pad, dilation=dilation, groups=groups, bias=has_bias)
+        self.has_bn = has_bn
+        if self.has_bn:
+            self.bn = norm_layer(out_planes, eps=bn_eps)
+        self.has_relu = has_relu
+        if self.has_relu:
+            self.relu = nn.ReLU(inplace=inplace)
+
+    def forward(self, x):
+        return deconv_bn_act(x, self.conv, self.bn if self.has_bn else None, self.has_relu)
+
+
 class ReluFn(torch.autograd.Function):
     """stand-alone ReLU on a small tensor (FFM squeeze branch [N,C,1,1], seg_oprs.py:224-226): expressed through
     tsb_bn_apply with scale 1 / shift 0 so it stays on the library path"""
