@@ -198,6 +198,14 @@ ce_up_bwd_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64
     }
 }
 
+// dynamic shared memory of the backward kernel, or 0 when it cannot run this geometry. The forward refuses those
+// geometries too, so that a loss it accepts can always be differentiated.
+static size_t bwd_smem(int C, int w, int W) {
+    const int maxcols = band_maxcols(kXS, w, W);
+    const size_t smem = sizeof(float) * (2 * (size_t)((C + 3) / 4) * kTQ + 4 * (size_t)maxcols * C);
+    return maxcols <= kXS && smem <= 110 * 1024 ? smem : 0;
+}
+
 }  // namespace
 
 extern "C" int tsb_ce_up_fwd(const float* logits_lo, int cs, int h, int w, const int64_t* labels, int N, int C, int H, int W,
@@ -205,6 +213,7 @@ extern "C" int tsb_ce_up_fwd(const float* logits_lo, int cs, int h, int w, const
     TSB_REQUIRE(logits_lo && labels && lse && state, "tsb_ce_up_fwd: null pointer");
     TSB_REQUIRE(N > 0 && N <= 65535 && h > 0 && h <= 65535 && w > 0 && H > 0 && W > 0, "tsb_ce_up_fwd: bad shape");
     TSB_REQUIRE(C >= 1 && C <= 4 * kJMax && cs >= C, "tsb_ce_up_fwd: 1 <= C <= %d", 4 * kJMax);
+    TSB_REQUIRE(bwd_smem(C, w, W) != 0, "tsb_ce_up_fwd: up-scale factor W/w too small for the backward band kernel");
     const int maxcols = band_maxcols(kXS, w, W);
     const int J = (C + 3) / 4;
     const size_t smem = sizeof(float) * (2 * (size_t)J * kTQ + 2 * (size_t)maxcols * C);
@@ -228,9 +237,8 @@ extern "C" int tsb_ce_up_bwd(const float* logits_lo, int cs, int h, int w, const
     TSB_REQUIRE(C >= 1 && C <= 4 * kJMax && cs >= C, "tsb_ce_up_bwd: 1 <= C <= %d", 4 * kJMax);
     const int maxcols = band_maxcols(kXS, w, W);
     TSB_REQUIRE(maxcols <= kXS, "tsb_ce_up_bwd: up-scale factor W/w too small for the band kernel");
-    const int J = (C + 3) / 4;
-    const size_t smem = sizeof(float) * (2 * (size_t)J * kTQ + 4 * (size_t)maxcols * C);
-    TSB_REQUIRE(smem <= 110 * 1024, "tsb_ce_up_bwd: shared memory budget exceeded");
+    const size_t smem = bwd_smem(C, w, W);
+    TSB_REQUIRE(smem != 0, "tsb_ce_up_bwd: shared memory budget exceeded");
     int rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(ce_up_bwd_kernel), smem);
     if (rc) return rc;
     ce_up_bwd_kernel<<<dim3((W + kXS - 1) / kXS, h, N), kT, smem, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, lse, C, H, W, ignore_label, state, gscale, dlogits_lo, maxcols);

@@ -504,7 +504,8 @@ ohem_grad_up_kernel(const float* __restrict__ lo, int cs, int h, int w, const in
 //   * the target class is fetched by ONE dynamic shared-memory read pair (its exp is recomputed: bit-identical, same
 //     inputs) instead of CX compare-selects;
 //   * gradient: softmax minus one-hot accumulates in the thread's own registers, and the bands run in four (row parity,
-//     strip parity) launches that add to the low-res gradient without atomics: the gradient is the same on every run;
+//     strip parity) launches that add to the low-res gradient without atomics: the gradient is the same on every run
+//     (the host picks this kernel only where same-parity strips touch disjoint low-res columns, grad_up_path);
 //     the accumulators' hand-over to phase 2 re-uses the T arrays in place (thread-private
 //     columns), which leaves ~80 registers and 3 CTAs / SM.
 // Arithmetic (operation order, roundings) is unchanged: p, T and the kept set stay bit-exact against the oracle.
@@ -670,6 +671,38 @@ void grad_launch(int grid, cudaStream_t st, const void* logits, long long sn, lo
     kernel<<<grid, kThreads, 0, st>>>((const T*)logits, sn, sc, sy, sx, labels, p, N, C, H, W, ignore_label, cw, state, gscale, (T*)dlogits);
 }
 
+// The exact-class gradient kernel runs strips s and s + 2 of one band row in the same launch and adds with plain stores,
+// which is only safe when their low-res columns are disjoint. That holds unless a strip spans fewer than about two
+// low-res columns ((W - 1) / (w - 1) >~ 128). Columns follow make_lerp: i0 is the truncation of the one rounded product
+// rx * x, identical on host and device. i0 is monotone in x, so strips s and s + 2 are the closest pair to check.
+static bool same_parity_strips_disjoint(int w, int W) {
+    const float rx = area_scale(w, W);
+    for (int s = 0; (s + 2) * kStrip < W; ++s) {
+        const float xl = (float)((s + 1) * kStrip - 1), xf = (float)((s + 2) * kStrip);
+        const int il = min((int)(rx * xl), w - 1), i_first = min((int)(rx * xf), w - 1);
+        const int hi = il + (il < w - 1 ? 1 : 0);   // i1 of strip s's last column
+        if (hi >= i_first) return false;
+    }
+    return true;
+}
+
+// Kernel choice of tsb_ohem_grad_up. The forward calls it too, so that it refuses every geometry the backward refuses.
+enum GradUpPath { kGradUpRefused, kGradUpGeneric, kGradUpExact };
+static GradUpPath grad_up_path(int C, int w, int W, size_t* smem) {
+    const int maxcols = band_maxcols(kStrip, w, W);
+    if (maxcols > kStrip) return kGradUpRefused;
+    if (C == 19 || C == 21) {
+        const size_t smx = sizeof(float) * (2 * (size_t)C * kPitch + 2 * (size_t)maxcols * C);
+        if (smx <= 72 * 1024 && same_parity_strips_disjoint(w, W)) {
+            *smem = smx;
+            return kGradUpExact;
+        }
+    }
+    const int cmax = C <= 20 ? 20 : 32;
+    *smem = sizeof(float) * (2 * (size_t)cmax * kPitch + 2 * (size_t)maxcols * cmax);
+    return *smem <= 96 * 1024 ? kGradUpGeneric : kGradUpRefused;
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -703,6 +736,9 @@ extern "C" int tsb_ohem_ptarget_up(const float* logits_lo, int cs, int h, int w,
     TSB_REQUIRE(N > 0 && C > 0 && C <= 32 && cs >= C && H > 0 && W > 0 && h > 0 && w > 0,
                 "tsb_ohem_ptarget_up: bad shape (C must be <= 32)");
     TSB_REQUIRE(N <= 65535 && h <= 65535, "tsb_ohem_ptarget_up: N and h must fit a grid dimension");
+    size_t grad_smem;
+    TSB_REQUIRE(grad_up_path(C, w, W, &grad_smem) != kGradUpRefused,
+                "tsb_ohem_ptarget_up: up-scale factor W/w too small for the gradient band kernel");
     const int maxcols = band_maxcols(kStrip, w, W);
     const dim3 grid((W + kStrip - 1) / kStrip, h, N);
     const cudaStream_t st = (cudaStream_t)stream;
@@ -777,24 +813,23 @@ extern "C" int tsb_ohem_grad_up(const float* logits_lo, int cs, int h, int w, co
     TSB_REQUIRE(N <= 65535 && h <= 65535, "tsb_ohem_grad_up: N and h must fit a grid dimension");
     const int maxcols = band_maxcols(kStrip, w, W);
     TSB_REQUIRE(maxcols <= kStrip, "tsb_ohem_grad_up: up-scale factor W/w too small for the band kernel");
+    size_t smem = 0;
+    const GradUpPath path = grad_up_path(C, w, W, &smem);
+    TSB_REQUIRE(path != kGradUpRefused, "tsb_ohem_grad_up: shared memory budget exceeded");
     const cudaStream_t st = (cudaStream_t)stream;
-    if (C == 19 || C == 21) {
-        const size_t smx = sizeof(float) * (2 * (size_t)C * kPitch + 2 * (size_t)maxcols * C);
-        if (smx <= 72 * 1024) {
-            const dim3 gridx(((W + kStrip - 1) / kStrip + 1) / 2, (h + 1) / 2, N);
-            auto kernel = C == 19 ? ohem_grad_up_x_kernel<19> : ohem_grad_up_x_kernel<21>;
-            int rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(kernel), smx);
-            if (rc) return rc;
-            for (int ph = 0; ph < 4; ++ph) {
-                kernel<<<gridx, kThreads, smx, st>>>(logits_lo, cs, h, w, labels, p, N, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols, ph);
-                TSB_CUDA_CHECK_LAUNCH("ohem_grad_up_x");
-            }
-            return TSB_OK;
+    if (path == kGradUpExact) {
+        const dim3 gridx(((W + kStrip - 1) / kStrip + 1) / 2, (h + 1) / 2, N);
+        auto kernel = C == 19 ? ohem_grad_up_x_kernel<19> : ohem_grad_up_x_kernel<21>;
+        int rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(kernel), smem);
+        if (rc) return rc;
+        for (int ph = 0; ph < 4; ++ph) {
+            kernel<<<gridx, kThreads, smem, st>>>(logits_lo, cs, h, w, labels, p, N, H, W, ignore_label, class_weight, state, gscale, dlogits_lo, maxcols, ph);
+            TSB_CUDA_CHECK_LAUNCH("ohem_grad_up_x");
         }
+        return TSB_OK;
     }
-    const int cmax = C <= 20 ? 20 : 32;
-    const size_t smem = sizeof(float) * (2 * (size_t)cmax * kPitch + 2 * (size_t)maxcols * cmax);
-    TSB_REQUIRE(smem <= 96 * 1024, "tsb_ohem_grad_up: shared memory budget exceeded");
+    // the generic kernel: bands add to the low-res gradient with atomics, so this path's rounding can differ from run to
+    // run (C = 19 / 21 land here when the shared memory or the strip geometry rules out the exact-class kernel)
     const dim3 grid((W + kStrip - 1) / kStrip, h, N);
     auto kernel = C <= 20 ? ohem_grad_up_kernel<20> : ohem_grad_up_kernel<32>;
     int rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(kernel), smem);

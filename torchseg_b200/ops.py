@@ -1146,7 +1146,8 @@ def _ohem_forward(pt_call, n, labels, ignore_label, thresh, min_kept, class_weig
 
 class OhemCEFn(torch.autograd.Function):
     """ProbOhemCrossEntropy2d.forward on MATERIALISED logits [N,C,H,W] (any strides, fp32/bf16) —
-    TorchSeg furnace/seg_opr/loss_opr.py:68-98."""
+    TorchSeg furnace/seg_opr/loss_opr.py:68-98. Labels lie in [0, C) or equal ignore_label (the kernels index the class
+    weights and the logits with them)."""
 
     @staticmethod
     def forward(ctx, pred, target, ignore_label, thresh, min_kept, class_weight):
@@ -1179,7 +1180,9 @@ class OhemCEFn(torch.autograd.Function):
 
 class OhemUpCEFn(torch.autograd.Function):
     """Fused head tail: bilinear x`scale` upsample (align_corners) of the LOW-res fp32 NHWC logits +
-    ProbOhemCrossEntropy2d; the full-resolution logits are never written (bisenet network.py:104-108,163-166)."""
+    ProbOhemCrossEntropy2d; the full-resolution logits are never written (bisenet network.py:104-108,163-166). Labels lie
+    in [0, C) or equal ignore_label (the kernels index shared memory with them). The forward refuses an up-scale the
+    backward cannot run."""
 
     @staticmethod
     def forward(ctx, lo, target, H, W, num_classes, ignore_label, thresh, min_kept, class_weight):
@@ -1213,7 +1216,8 @@ class OhemUpCEFn(torch.autograd.Function):
 class CEUpFn(torch.autograd.Function):
     """Fused head tail for MANY classes (ADE's 150): bilinear up-sampling (align_corners) of the LOW-res fp32 NHWC logits to
     H x W + CrossEntropyLoss(mean, ignore_index); the full-resolution [N,C,H,W] logits are never written
-    (pspnet network.py:46-57, psanet network.py:46-55). 1 <= C <= 152."""
+    (pspnet network.py:46-57, psanet network.py:46-55). 1 <= C <= 152. Labels lie in [0, C) or equal ignore_label (the
+    kernels index shared memory with them). The forward refuses an up-scale the backward cannot run."""
 
     @staticmethod
     def forward(ctx, lo, target, H, W, num_classes, ignore_label):
