@@ -307,21 +307,29 @@ int tsb_bias_grad(const void* dy, int dycs, long long npix, int K, float* db, fl
                   tsb_stream_t stream);
 
 /* ================================================================================================
- * Depthwise 3x3 convolution (groups = C, padding 1, dilation 1, stride 1 or 2) — replaces the `groups=in_channels`
- * nn.Conv2d of SeparableConvBnRelu (furnace/base_model/xception.py:14-16) and its cuDNN dgrad / wgrad.
- * x, y, dy, dx: bf16 NHWC with channel strides (multiples of 8, >= C; 16-byte aligned), so channel slices of wider
- * (e.g. 64-padded) buffers are read and written in place; C % 8 == 0, C <= 4096. H, W: INPUT size; the output is
- * P = (H - 1) / stride + 1 by Q = (W - 1) / stride + 1. w: the fp32 [C][3][3] master weight, rounded to bf16 on load.
- * All sums are fp32, taps in a fixed (r, s) order, rounded to bf16 once.
+ * Depthwise 3x3 convolution (groups = C) — replaces the `groups=in_channels` nn.Conv2d of SeparableConvBnRelu
+ * (furnace/base_model/xception.py:14-16; furnace/seg_opr/seg_oprs.py:76-94 with padding = dilation) and its cuDNN
+ * dgrad / wgrad. Geometry: stride 1 with padding = dilation >= 1, or stride 2 with padding 1 and dilation 1; anything
+ * else is an error. x, y, dy, dx: bf16 NHWC with channel strides (multiples of 8, >= C; 16-byte aligned), so channel
+ * slices of wider (e.g. 64-padded) buffers are read and written in place; C % 8 == 0, C <= 4096. H, W: INPUT size; the
+ * output is P = (H - 1) / stride + 1 by Q = (W - 1) / stride + 1. w: the fp32 [C][3][3] master weight, rounded to bf16
+ * on load. All sums are fp32, taps in a fixed (r, s) order, rounded to bf16 once; taps outside the map add nothing.
  * ============================================================================================== */
-/* y[n,p,q,c] = Σ_{r,s} x[n, p·stride−1+r, q·stride−1+s, c] · w[c,r,s] */
+/* y[n,p,q,c] = Σ_{r,s} x[n, p·stride+(r−1)·dilation, q·stride+(s−1)·dilation, c] · w[c,r,s] */
+int tsb_dwconv2d_fprop(const void* x, int xcs, const float* w, void* y, int ycs, int N, int H, int W, int C, int stride,
+                       int dilation, tsb_stream_t stream);
+/* dx = the gather-form transpose of fprop (no atomics); accumulate != 0: dx = bf16(dx + result) */
+int tsb_dwconv2d_dgrad(const void* dy, int dycs, const float* w, void* dx, int dxcs, int N, int H, int W, int C,
+                       int stride, int dilation, int accumulate, tsb_stream_t stream);
+/* dw[c,r,s] (fp32 [C][3][3]) += Σ_{n,p,q} dy[n,p,q,c] · x[n, p·stride+(r−1)·dilation, q·stride+(s−1)·dilation, c]: one
+ * [C·9] workspace slot per CTA, summed in slot order (a too-small workspace is an error) */
+int tsb_dwconv2d_wgrad(const void* x, int xcs, const void* dy, int dycs, float* dw, int N, int H, int W, int C,
+                       int stride, int dilation, float* ws, long long ws_floats, tsb_stream_t stream);
+/* the same three at dilation 1 (padding 1) */
 int tsb_dwconv_fprop(const void* x, int xcs, const float* w, void* y, int ycs, int N, int H, int W, int C, int stride,
                      tsb_stream_t stream);
-/* dx = the gather-form transpose of fprop (no atomics); accumulate != 0: dx = bf16(dx + result) */
 int tsb_dwconv_dgrad(const void* dy, int dycs, const float* w, void* dx, int dxcs, int N, int H, int W, int C, int stride,
                      int accumulate, tsb_stream_t stream);
-/* dw[c,r,s] (fp32 [C][3][3]) += Σ_{n,p,q} dy[n,p,q,c] · x[n, p·stride−1+r, q·stride−1+s, c]: one [C·9] workspace slot
- * per CTA, summed in slot order (a too-small workspace is an error) */
 int tsb_dwconv_wgrad(const void* x, int xcs, const void* dy, int dycs, float* dw, int N, int H, int W, int C, int stride,
                      float* ws, long long ws_floats, tsb_stream_t stream);
 

@@ -73,6 +73,9 @@ _SIGS = {
     "tsb_dwconv_fprop": [P, I, P, P, I, I, I, I, I, I, P],
     "tsb_dwconv_dgrad": [P, I, P, P, I, I, I, I, I, I, I, P],
     "tsb_dwconv_wgrad": [P, I, P, I, P, I, I, I, I, I, P, L, P],
+    "tsb_dwconv2d_fprop": [P, I, P, P, I, I, I, I, I, I, I, P],
+    "tsb_dwconv2d_dgrad": [P, I, P, P, I, I, I, I, I, I, I, I, P],
+    "tsb_dwconv2d_wgrad": [P, I, P, I, P, I, I, I, I, I, I, P, L, P],
     "tsb_sgd_flat": [P, P, P, L, P, P, P, I, F, F, I, P],
     "tsb_sgd_flat_pack": [P, P, P, L, P, P, P, I, F, F, I, P, P],
     "tsb_pack_wt_multi": [P, P, P, P, I, I, P],

@@ -3,3 +3,4 @@ from .fcn import FCN
 from .pspnet import PSPNet, PyramidPooling
 from .dfn import DFN, DFNHead
 from .psanet import PSANet, PointwiseSpatialAttention
+from .deeplabv3plus import DeepLabV3Plus, ASPP, Decoder

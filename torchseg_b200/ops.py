@@ -511,6 +511,59 @@ class GradShare(object):
         return out
 
 
+def _bn_forward(raw, stats, count, gamma, beta, residual, running_mean, running_var, relu, eps, momentum, training):
+    """the BatchNorm half of ConvBNActFn.forward: y = act(BN(raw) + residual) over the dense NHWC raw [N,K,P,Q]. Training
+    normalises with the batch statistics stats = [Σ; Σ²] (summed over the SyncBN group here) and updates the running
+    statistics; eval uses the running statistics. Returns (y, aux = [mean; invstd; scale; shift])."""
+    N, K, P, Q = raw.shape
+    aux = torch.empty((4, K), dtype=torch.float32, device=raw.device)  # mean, invstd, scale, shift
+    if training:
+        _allreduce_stats(stats)
+        call("tsb_bn_finalize", ptr(stats[0]), ptr(stats[1]), count, K, ptr(gamma), ptr(beta), eps, momentum,
+             ptr(aux[0]), ptr(aux[1]), ptr(aux[2]), ptr(aux[3]), ptr(running_mean), ptr(running_var), stream())
+    else:
+        # eval: scale/shift from the running statistics (sum := mean*1, sumsq := var + mean^2, count 1)
+        s = torch.stack([running_mean, running_var + running_mean * running_mean]).contiguous()
+        call("tsb_bn_finalize", ptr(s[0]), ptr(s[1]), 1.0, K, ptr(gamma), ptr(beta), eps, 0.0, ptr(aux[0]),
+             ptr(aux[1]), ptr(aux[2]), ptr(aux[3]), None, None, stream())
+    y = nhwc_empty(N, K, P, Q, device=raw.device)
+    call("tsb_bn_apply", ptr(raw), K, ptr(aux[2]), ptr(aux[3]), ptr(residual), cs_of(residual) if residual is not None else 0,
+         int(relu), ptr(y), K, N * P * Q, K, stream())
+    return y, aux
+
+
+def _bn_backward(dy, y, raw, aux, gamma, beta, count, relu, has_res, direct):
+    """the BatchNorm half of ConvBNActFn.backward: (draw, dres, dgamma, dbeta). direct: gamma / beta (and the caller's
+    weight) take their gradients in their flat .grad views, and dgamma / dbeta are returned as None."""
+    N, K, P, Q = raw.shape
+    dev = raw.device
+    npix = N * P * Q
+    if dy.dtype != _BF or dy.stride(1) != 1:
+        dy = to_nhwc(dy)
+    red = zero_arena.take((2, K), dev)
+    # ReLU mask: recomputed from raw*scale+shift when there is no residual (saves reading y in both passes)
+    y_mask = ptr(y) if (relu and has_res) else None
+    call("tsb_bn_bwd_reduce", ptr(dy), cs_of(dy), y_mask, K, ptr(raw), K, ptr(aux[0]), ptr(aux[1]), int(relu), npix, K,
+         ptr(red[0]), ptr(red[1]), ptr(aux[2]), ptr(aux[3]), *det_ws(), stream())
+    # dgamma = Σ dz·x̂, dbeta = Σ dz are LOCAL sums (the DDP all-reduce averages parameter grads);
+    # the dx formula needs the GLOBAL sums under SyncBN.
+    fold = direct and _sync["world"] == 1   # single GPU: the accumulation is folded into tsb_bn_bwd_apply
+    if direct:
+        dgamma = dbeta = None
+        # multi-GPU: the exchange kernel adds the LOCAL sums to gamma.grad / beta.grad before it reduces
+        _allreduce_stats(red, None if fold else gamma.grad, None if fold else beta.grad)
+    else:
+        dgamma = red[1].clone()
+        dbeta = red[0].clone()
+        _allreduce_stats(red)
+    draw = nhwc_empty(N, K, P, Q, device=dev)
+    dres = nhwc_empty(N, K, P, Q, device=dev) if has_res else None
+    call("tsb_bn_bwd_apply", ptr(dy), cs_of(dy), y_mask, K, ptr(raw), K, ptr(aux[0]), ptr(aux[1]), ptr(gamma), ptr(red[0]),
+         ptr(red[1]), count, int(relu), ptr(draw), K, ptr(dres), K if has_res else 0, npix, K,
+         ptr(gamma.grad) if fold else None, ptr(beta.grad) if fold else None, ptr(aux[2]), ptr(aux[3]), stream())
+    return draw, dres, dgamma, dbeta
+
+
 class ConvBNActFn(torch.autograd.Function):
     """y = act(BN_train(conv(x, w)) + residual).
 
@@ -555,19 +608,8 @@ class ConvBNActFn(torch.autograd.Function):
         else:
             wb, _ = pack_cache.get(w, False)
             conv_fprop(x, wb, K, R, stride, pad, dil, out=raw, stats=stats)
-        aux = torch.empty((4, K), dtype=torch.float32, device=dev)  # mean, invstd, scale, shift
-        if training:
-            _allreduce_stats(stats)
-            call("tsb_bn_finalize", ptr(stats[0]), ptr(stats[1]), count, K, ptr(gamma), ptr(beta), eps, momentum,
-                 ptr(aux[0]), ptr(aux[1]), ptr(aux[2]), ptr(aux[3]), ptr(running_mean), ptr(running_var), stream())
-        else:
-            # eval: scale/shift from the running statistics (sum := mean*1, sumsq := var + mean^2, count 1)
-            s = torch.stack([running_mean, running_var + running_mean * running_mean]).contiguous()
-            call("tsb_bn_finalize", ptr(s[0]), ptr(s[1]), 1.0, K, ptr(gamma), ptr(beta), eps, 0.0, ptr(aux[0]),
-                 ptr(aux[1]), ptr(aux[2]), ptr(aux[3]), None, None, stream())
-        y = nhwc_empty(N, K, P, Q, device=dev)
-        call("tsb_bn_apply", ptr(raw), K, ptr(aux[2]), ptr(aux[3]), ptr(residual), cs_of(residual) if residual is not None else 0,
-             int(relu), ptr(y), K, N * P * Q, K, stream())
+        y, aux = _bn_forward(raw, stats, count, gamma, beta, residual, running_mean, running_var, relu, eps, momentum,
+                             training)
         ctx.save_for_backward(x, w, gamma, raw, y, aux)
         ctx.beta_ref = beta
         ctx.cfg = (stride, pad, dil, relu, stem, residual is not None, count, training, transposed)
@@ -587,32 +629,9 @@ class ConvBNActFn(torch.autograd.Function):
         R = w.shape[2]
         N, _, P, Q = raw.shape
         dev = dy.device
-        npix = N * P * Q
-        if dy.dtype != _BF or dy.stride(1) != 1:
-            dy = to_nhwc(dy)
-        red = zero_arena.take((2, K), dev)
-        # ReLU mask: recomputed from raw*scale+shift when there is no residual (saves reading y in both passes)
-        y_mask = ptr(y) if (relu and has_res) else None
-        call("tsb_bn_bwd_reduce", ptr(dy), cs_of(dy), y_mask, K, ptr(raw), K, ptr(aux[0]), ptr(aux[1]), int(relu), npix, K,
-             ptr(red[0]), ptr(red[1]), ptr(aux[2]), ptr(aux[3]), *det_ws(), stream())
-        # dgamma = Σ dz·x̂, dbeta = Σ dz are LOCAL sums (the DDP all-reduce averages parameter grads);
-        # the dx formula needs the GLOBAL sums under SyncBN.
         beta = ctx.beta_ref
         direct = _direct_grad(w) and _direct_grad(gamma) and _direct_grad(beta)
-        fold = direct and _sync["world"] == 1   # single GPU: the accumulation is folded into tsb_bn_bwd_apply
-        if direct:
-            dgamma = dbeta = None
-            # multi-GPU: the exchange kernel adds the LOCAL sums to gamma.grad / beta.grad before it reduces
-            _allreduce_stats(red, None if fold else gamma.grad, None if fold else beta.grad)
-        else:
-            dgamma = red[1].clone()
-            dbeta = red[0].clone()
-            _allreduce_stats(red)
-        draw = nhwc_empty(N, K, P, Q, device=dev)
-        dres = nhwc_empty(N, K, P, Q, device=dev) if has_res else None
-        call("tsb_bn_bwd_apply", ptr(dy), cs_of(dy), y_mask, K, ptr(raw), K, ptr(aux[0]), ptr(aux[1]), ptr(gamma), ptr(red[0]),
-             ptr(red[1]), count, int(relu), ptr(draw), K, ptr(dres), K if has_res else 0, npix, K,
-             ptr(gamma.grad) if fold else None, ptr(beta.grad) if fold else None, ptr(aux[2]), ptr(aux[3]), stream())
+        draw, dres, dgamma, dbeta = _bn_backward(dy, y, raw, aux, gamma, beta, count, relu, has_res, direct)
         if direct:
             dw_view, dw = None, w.grad.permute(0, 2, 3, 1)   # KRSC view of the flat gradient buffer
         else:
@@ -837,8 +856,9 @@ class ConvTransposeFn(torch.autograd.Function):
 
 
 class DWConvFn(torch.autograd.Function):
-    """depthwise 3x3 convolution, padding 1, stride 1 or 2, no bias: the `groups=in_channels` conv of
-    SeparableConvBnRelu (TorchSeg furnace/base_model/xception.py:14-16), on tsb_dwconv_{fprop,dgrad,wgrad}.
+    """depthwise 3x3 convolution, no bias, stride 1 with padding = dilation `dil`, or stride 2 with padding 1: the
+    `groups=in_channels` conv of the SeparableConvBnRelu blocks (TorchSeg furnace/base_model/xception.py:14-16,
+    furnace/seg_opr/seg_oprs.py:76-94), on tsb_dwconv2d_{fprop,dgrad,wgrad}.
 
     x may carry more logical channels than the conv has (a 64-padded buffer whose channels [C, Cx) are zero): the
     kernels read its first C channels in place. The output has `ocs` >= C logical channels whose pads are exact zeros,
@@ -846,24 +866,24 @@ class DWConvFn(torch.autograd.Function):
     consumers in the same block and their input gradients are chained through one buffer (dgrad accumulate)."""
 
     @staticmethod
-    def forward(ctx, x, w, stride, ocs, share=None):
+    def forward(ctx, x, w, stride, ocs, share=None, dil=1):
         C = w.shape[0]
         assert w.shape[1:] == (1, 3, 3), "depthwise 3x3 weight [C,1,3,3] expected"
         N, Cx, H, W = x.shape
         assert Cx >= C
-        P, Q = conv_out_size(H, 3, stride, 1, 1), conv_out_size(W, 3, stride, 1, 1)
+        P, Q = conv_out_size(H, 3, stride, dil, dil), conv_out_size(W, 3, stride, dil, dil)
         ocs = C if ocs is None else ocs
         y = (nhwc_zeros if ocs > C else nhwc_empty)(N, ocs, P, Q, device=x.device)
-        call("tsb_dwconv_fprop", ptr(x), cs_of(x), ptr(w.detach().reshape(C, 9)), ptr(y), cs_of(y), N, H, W, C, stride,
-             stream())
+        call("tsb_dwconv2d_fprop", ptr(x), cs_of(x), ptr(w.detach().reshape(C, 9)), ptr(y), cs_of(y), N, H, W, C, stride,
+             dil, stream())
         ctx.save_for_backward(x, w)
-        ctx.stride, ctx.share = stride, share
+        ctx.stride, ctx.share, ctx.dil = stride, share, dil
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, w = ctx.saved_tensors
-        stride, share = ctx.stride, ctx.share
+        stride, share, dil = ctx.stride, ctx.share, ctx.dil
         C = w.shape[0]
         N, Cx, H, W = x.shape
         if dy.dtype != _BF or dy.stride(1) != 1:
@@ -874,21 +894,57 @@ class DWConvFn(torch.autograd.Function):
             dw_view, dw = None, w.grad
         else:
             dw_view = dw = torch.zeros_like(w, memory_format=torch.contiguous_format)
-        call("tsb_dwconv_wgrad", ptr(x), cs_of(x), ptr(dy), cs_of(dy), ptr(dw), N, H, W, C, stride, *det_ws(), stream())
+        call("tsb_dwconv2d_wgrad", ptr(x), cs_of(x), ptr(dy), cs_of(dy), ptr(dw), N, H, W, C, stride, dil, *det_ws(),
+             stream())
         dx = None
         if ctx.needs_input_grad[0]:
             if share is not None and share.stash is not None:
                 dx = share.stash
-                call("tsb_dwconv_dgrad", ptr(dy), cs_of(dy), ptr(w9), ptr(dx), cs_of(dx), N, H, W, C, stride, 1, stream())
+                call("tsb_dwconv2d_dgrad", ptr(dy), cs_of(dy), ptr(w9), ptr(dx), cs_of(dx), N, H, W, C, stride, dil, 1,
+                     stream())
                 dx = share.contribute(dx, accumulated=True)
             else:
                 dx = (nhwc_zeros if Cx > C else nhwc_empty)(N, Cx, H, W, device=dy.device)
-                call("tsb_dwconv_dgrad", ptr(dy), cs_of(dy), ptr(w9), ptr(dx), cs_of(dx), N, H, W, C, stride, 0, stream())
+                call("tsb_dwconv2d_dgrad", ptr(dy), cs_of(dy), ptr(w9), ptr(dx), cs_of(dx), N, H, W, C, stride, dil, 0,
+                     stream())
                 if share is not None:
                     dx = share.contribute(dx)
         if direct:
             _notify(w)
-        return dx, dw_view, None, None, None
+        return dx, dw_view, None, None, None, None
+
+
+class BNFn(torch.autograd.Function):
+    """y = BN(x) without an activation, on the BatchNorm half of ConvBNActFn: the `bn` between the depthwise and the
+    pointwise conv of SeparableConvBnRelu (TorchSeg furnace/seg_opr/seg_oprs.py:88,93). Training takes the batch
+    statistics with tsb_bn_stats (summed over the SyncBN group like every other BN) and updates the running statistics;
+    eval applies the running statistics. x: dense bf16 NHWC [N,C,H,W]."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, running_mean, running_var, eps, momentum, training):
+        N, C, H, W = x.shape
+        assert cs_of(x) == C
+        count = float(N * H * W) * _sync["world"]
+        stats = None
+        if training:
+            stats = zero_arena.take((2, C), x.device)
+            call("tsb_bn_stats", ptr(x), C, N * H * W, C, ptr(stats[0]), ptr(stats[1]), *det_ws(), stream())
+        y, aux = _bn_forward(x, stats, count, gamma, beta, None, running_mean, running_var, False, eps, momentum,
+                             training)
+        ctx.save_for_backward(x, gamma, aux)
+        ctx.beta_ref, ctx.count, ctx.training = beta, count, training
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, gamma, aux = ctx.saved_tensors
+        assert ctx.training, "backward through eval-mode BN is not supported"
+        beta = ctx.beta_ref
+        direct = _direct_grad(gamma) and _direct_grad(beta)
+        dx, _, dgamma, dbeta = _bn_backward(dy, None, x, aux, gamma, beta, ctx.count, False, False, direct)
+        if direct:
+            _notify(gamma, beta)
+        return dx, dgamma, dbeta, None, None, None, None, None
 
 
 # --------------------------------------------------------------------------------------------------

@@ -246,6 +246,49 @@ class DeConvBnRelu(nn.Module):
         return deconv_bn_act(x, self.conv, self.bn if self.has_bn else None, self.has_relu)
 
 
+class SeparableConvBnRelu(nn.Module):
+    """seg_oprs.py:76-94 — same ctor, children named conv1 (a genuine depthwise nn.Conv2d) / bn / point_wise_cbr: the
+    depthwise conv, BN (batch statistics in training, running statistics in eval; no ReLU), then the pointwise
+    ConvBnRelu. Runs the 3x3 depthwise conv at stride 1 with padding = dilation (the atrous separable conv of
+    DeepLabV3+), or at stride 2 with padding 1 and dilation 1, over a multiple of 8 channels; anything else raises
+    NotImplementedError."""
+
+    def __init__(self, in_channels, out_channels, kernel_size=1, stride=1, padding=0, dilation=1, has_relu=True,
+                 norm_layer=nn.BatchNorm2d):
+        super(SeparableConvBnRelu, self).__init__()
+        self.conv1 = nn.Conv2d(in_channels, in_channels, kernel_size, stride, padding, dilation, groups=in_channels,
+                               bias=False)
+        self.bn = norm_layer(in_channels)
+        self.point_wise_cbr = ConvBnRelu(in_channels, out_channels, 1, 1, 0, has_bn=True, norm_layer=norm_layer,
+                                         has_relu=has_relu, has_bias=False)
+
+    def _geometry(self):
+        """(stride, dilation) of the depthwise conv the dwconv kernels run (include/tsb.h)"""
+        c = self.conv1
+        k, st, pd, dl = c.kernel_size, c.stride, c.padding, c.dilation
+        if k != (3, 3):
+            raise NotImplementedError("SeparableConvBnRelu: only a 3x3 depthwise conv runs on libtsb (got %s)" % (k,))
+        if st[0] != st[1] or pd[0] != pd[1] or dl[0] != dl[1] or not isinstance(pd[0], int):
+            raise NotImplementedError("SeparableConvBnRelu: non-square stride, padding or dilation")
+        if pd[0] != dl[0]:
+            raise NotImplementedError("SeparableConvBnRelu: padding must equal the dilation (got %d, %d)" % (pd[0], dl[0]))
+        if st[0] not in (1, 2) or (st[0] == 2 and dl[0] != 1):
+            raise NotImplementedError("SeparableConvBnRelu: stride 1, or stride 2 at dilation 1 (got stride %d, "
+                                      "dilation %d)" % (st[0], dl[0]))
+        if c.in_channels % 8 != 0:
+            raise NotImplementedError("SeparableConvBnRelu: in_channels must be a multiple of 8 (got %d)" % c.in_channels)
+        return st[0], dl[0]
+
+    def forward(self, x):
+        stride, dil = self._geometry()
+        bn, pw = self.bn, self.point_wise_cbr
+        t = ops.DWConvFn.apply(_as_act(x), self.conv1.weight, stride, None, None, dil)
+        momentum = bn.momentum if bn.momentum is not None else 0.1
+        t = ops.BNFn.apply(t, bn.weight, bn.bias, bn.running_mean, bn.running_var, float(bn.eps), float(momentum),
+                           bool(bn.training))
+        return conv_bn_act(t, pw.conv, pw.bn, pw.has_relu)
+
+
 class ReluFn(torch.autograd.Function):
     """stand-alone ReLU on a small tensor (FFM squeeze branch [N,C,1,1], seg_oprs.py:224-226): expressed through
     tsb_bn_apply with scale 1 / shift 0 so it stays on the library path"""
