@@ -538,12 +538,22 @@ _KERNEL_RE = re.compile(r"(igemm_v2_kernel<\d+, (?:true|false)>|wgrad_(?:taps|ro
 
 
 def _kernels_of(fn):
+    """the conv kernels fn launches, by name. In a long process the profiler occasionally returns a trace without any
+    of the kernels the library launched inside its window (seen: one full-size case, all three ops, in a whole-suite
+    run); such a lost trace is told apart by the library's own launch counter and measured again, at most twice. A
+    call that launches nothing still reports nothing."""
     from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
+    from torchseg_b200 import _lib
+    for _ in range(3):
         torch.cuda.synchronize()
-    return {m.group(1) for m in (_KERNEL_RE.search(e.name) for e in prof.events()) if m}
+        n0 = _lib.launch_count()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        got = {m.group(1) for m in (_KERNEL_RE.search(e.name) for e in prof.events()) if m}
+        if got or _lib.launch_count() == n0:
+            return got
+    return got
 
 
 def test_conv_dispatch_coverage(cuda):

@@ -511,6 +511,13 @@ class GradShare(object):
         return out
 
 
+def _running_stats_written(running_mean, running_var):
+    """tsb_bn_finalize updated the running statistics through raw pointers, which autograd's version counters do not
+    see: bump them, so that what is keyed on those versions (the eval-mode fold cache) rebuilds from the new values. A
+    version bump changes no tensor data; inside a graph capture it happens once, and the replays bump pack_cache.step."""
+    torch.autograd.graph.increment_version((running_mean, running_var))
+
+
 def _bn_forward(raw, stats, count, gamma, beta, residual, running_mean, running_var, relu, eps, momentum, training):
     """the BatchNorm half of ConvBNActFn.forward: y = act(BN(raw) + residual) over the dense NHWC raw [N,K,P,Q]. Training
     normalises with the batch statistics stats = [Σ; Σ²] (summed over the SyncBN group here) and updates the running
@@ -521,6 +528,7 @@ def _bn_forward(raw, stats, count, gamma, beta, residual, running_mean, running_
         _allreduce_stats(stats)
         call("tsb_bn_finalize", ptr(stats[0]), ptr(stats[1]), count, K, ptr(gamma), ptr(beta), eps, momentum,
              ptr(aux[0]), ptr(aux[1]), ptr(aux[2]), ptr(aux[3]), ptr(running_mean), ptr(running_var), stream())
+        _running_stats_written(running_mean, running_var)
     else:
         # eval: scale/shift from the running statistics (sum := mean*1, sumsq := var + mean^2, count 1)
         s = torch.stack([running_mean, running_var + running_mean * running_mean]).contiguous()
@@ -700,6 +708,7 @@ class StemPairFn(torch.autograd.Function):
         for (off, Kh, g, b, rm, rv, eps, mom) in ((0, K1, g1, b1, rm1, rv1, eps1, mom1), (K1, K2, g2, b2, rm2, rv2, eps2, mom2)):
             call("tsb_bn_finalize", ptr(stats[0][off:]), ptr(stats[1][off:]), count, Kh, ptr(g), ptr(b), eps, mom,
                  ptr(aux[0][off:]), ptr(aux[1][off:]), ptr(aux[2][off:]), ptr(aux[3][off:]), ptr(rm), ptr(rv), stream())
+            _running_stats_written(rm, rv)
         y = nhwc_empty(N, K, P, Q, device=dev)
         call("tsb_bn_apply", ptr(raw), K, ptr(aux[2]), ptr(aux[3]), None, 0, 1, ptr(y), K, N * P * Q, K, stream())
         ctx.save_for_backward(xs, w1, g1, w2, g2, raw, aux)
