@@ -334,6 +334,37 @@ int tsb_dwconv_wgrad(const void* x, int xcs, const void* dy, int dycs, float* dw
                      float* ws, long long ws_floats, tsb_stream_t stream);
 
 /* ================================================================================================
+ * Context Encoding (EncNet's Encoding layer, Zhang et al., CVPR 2018) and the SE-loss. For the N pixels x_i (bf16 NHWC,
+ * channel stride xcs) of each of B images, K codewords c_k (fp32 [K][D]) and smoothing factors s_k (fp32 [K]):
+ *   d²_ik = ‖x_i − c_k‖² (direct differences), a_ik = softmax_k(s_k d²_ik), E_bk = Σ_i a_ik (x_i − c_k).
+ * K is a multiple of 8 and at most 32 (one warp lane per codeword), D a multiple of 64 and at most 1024 with K·D <= 16384
+ * (the codewords sit in shared memory); anything else is TSB_ERR_UNSUPPORTED. xcs, dxcs: multiples of 8, >= D; x, dx
+ * 16-byte aligned. Arithmetic is fp32. Each CTA sums its pixels into its own workspace slot (16 slots per image, so
+ * B·16·(K·D + K) floats forward and B·16·(K·D + 2K) backward, independent of N) and the slots are added in a fixed order.
+ * ============================================================================================== */
+/* E: bf16 [B·D rows][K channels] (row b·D + d), an NHWC tensor with C = K that the BN entry points normalise as is.
+ * a, d2: fp32 [B·N][K], saved for the backward (both NULL in inference). sum_a: fp32 [B][K] = Σ_i a_ik. */
+int tsb_encoding_fwd(const void* x, int xcs, int B, int N, int D, const float* codewords, const float* scale, int K,
+                     float* a, float* d2, float* sum_a, void* E, float* ws, long long ws_floats, tsb_stream_t stream);
+/* dE bf16 [B·D][K] like E. With t_ik = dE_k·(x_i − c_k) and g_ik = a_ik (t_ik − Σ_j a_ij t_ij):
+ *   dx_i = Σ_k a_ik dE_k + 2 Σ_k g_ik s_k (x_i − c_k)                        (bf16, written)
+ *   dcodewords_k += −Σ_b (Σ_i a_ik) dE_bk − 2 s_k Σ_b Σ_i g_ik (x_i − c_k)    (fp32 [K][D], accumulated)
+ *   dscale_k     += Σ_b Σ_i g_ik d²_ik                                        (fp32 [K], accumulated) */
+int tsb_encoding_bwd(const void* dE, const void* x, int xcs, int B, int N, int D, const float* codewords,
+                     const float* scale, int K, const float* a, const float* d2, const float* sum_a, void* dx, int dxcs,
+                     float* dcodewords, float* dscale, float* ws, long long ws_floats, tsb_stream_t stream);
+/* y[p] = (1/C) Σ_c x[p, c] summed in channel order (bf16 in, bf16 y[npix] out): EncNet's mean over the codewords.
+ * bwd: dx[p, c] = dy[p] / C (dy dense bf16 [npix], dx channel stride dxcs >= C). */
+int tsb_chan_mean_fwd(const void* x, int xcs, long long npix, int C, void* y, tsb_stream_t stream);
+int tsb_chan_mean_bwd(const void* dy, long long npix, int C, void* dx, int dxcs, tsb_stream_t stream);
+/* SE-loss: nn.BCELoss(sigmoid(z), presence) with presence[b, c] = any(labels[b] == c) for c in [0, C) (other label values
+ * count for nothing). labels int64 [B][HW]; z fp32 [B][C] with row stride zs. presence: uint32 [B][ceil(C/32)] bit words,
+ * written (per-CTA shared-memory bitmaps ORed together, so deterministic). *loss: the mean with torch's −100 clamp on
+ * the logs; dz_unit (row stride dzs): d loss / d z for a unit upstream gradient. C <= 4096. No host synchronisation. */
+int tsb_se_loss_fwd_bwd(const int64_t* labels, int B, long long HW, const float* z, int zs, int C, uint32_t* presence,
+                        float* loss, float* dz_unit, int dzs, tsb_stream_t stream);
+
+/* ================================================================================================
  * Optimiser — fused flat-buffer momentum SGD replacing torch.optim.SGD.step (train.py:86-89,142) with
  * the group semantics of furnace/utils/init_func.py:34-57 (decay / no-decay, 1x / 10x LR):
  *   g = grad*gscale + wd*p ; buf = first ? g : mom*buf + g ; p -= lr*buf      (torch SGD, dampening 0)

@@ -88,6 +88,11 @@ _SIGS = {
     "tsb_eval_windows": [P, I, I, I, D, I, I, I, I, P, I, P, I, I, I, I, P, P],
     "tsb_eval_accumulate": [P, P, P, I, I, I, I, P, I, I, P],
     "tsb_eval_resize_add": [P, I, I, I, L, L, P, I, I, P, P],
+    "tsb_encoding_fwd": [P, I, I, I, I, P, P, I, P, P, P, P, P, L, P],
+    "tsb_encoding_bwd": [P, P, I, I, I, I, P, P, I, P, P, P, P, I, P, P, P, L, P],
+    "tsb_chan_mean_fwd": [P, I, L, I, P, P],
+    "tsb_chan_mean_bwd": [P, L, I, P, I, P],
+    "tsb_se_loss_fwd_bwd": [P, I, L, P, I, I, P, P, P, I, P],
 }
 EXPORTS = sorted(list(_SIGS) + ["tsb_last_error", "tsb_version", "tsb_launch_count", "tsb_p2p_buffer_bytes", "tsb_edge_labels_workspace_bytes"])
 

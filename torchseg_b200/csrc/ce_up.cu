@@ -9,10 +9,12 @@
 // T[j][column][q] (consecutive lanes → consecutive words: conflict-free), staged once per band; a hi-res row then costs 2 LDS
 // + 3 flops per class for the value, and the 4 lanes of a pixel combine max / sum with two shuffles.
 //   forward : lse[pixel] = logsumexp_c v_c (kept for the backward), loss = mean over valid pixels of lse − v_target
-//   backward: d lo[i, j, c] += Σ_pixels w_y·w_x·(exp(v_c − lse) − [c = target])·g/count — the softmax part through per-thread
-//             register accumulators reduced per band in shared memory (phase 2: band.cuh col_sums, shared with the OHEM
-//             gradient kernels), the one-hot part through a low-resolution shared-memory tile (4 RED.shared per pixel) that
-//             phase 2 starts from
+//   backward: d lo[i, j, c] += Σ_pixels w_y·w_x·(exp(v_c − lse) − [c = target])·g/count through per-thread register
+//             accumulators (the lane that owns the target class subtracts the one-hot term in its own accumulator), reduced
+//             per band in shared memory in a fixed order (phase 2: band.cuh col_sums, shared with the OHEM gradient kernels).
+//             The bands run in launches by (row parity, strip phase), chosen so that no two bands of one launch touch the same
+//             low-res element; each element therefore receives its contributions one launch at a time, in launch order, and
+//             the gradient is the same on every run.
 #include "band.cuh"
 
 namespace {
@@ -113,8 +115,9 @@ __global__ void ce_up_finalize_kernel(uint32_t* state, float* loss_out) {
 __global__ void __launch_bounds__(kT, 2)
 ce_up_bwd_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64_t* __restrict__ labels,
                  const float* __restrict__ lse_in, int C, int H, int W, int ignore_label, const uint32_t* __restrict__ state,
-                 const float* __restrict__ gscale, float* __restrict__ dlo, int maxcols) {
-    extern __shared__ float s_dyn[];       // sT0 / G0 | sT1 / G1 | s_lo0 | s_lo1 | s_oh[2][maxcols][C]
+                 const float* __restrict__ gscale, float* __restrict__ dlo, int maxcols, int row_phase, int strip_phase,
+                 int strip_step) {
+    extern __shared__ float s_dyn[];       // sT0 / G0 | sT1 / G1 | s_lo0 | s_lo1
     __shared__ float s_l0[kXS], s_l1[kXS];
     __shared__ short s_seg[kXS + 8];
     const int J = (C + 3) >> 2;
@@ -122,14 +125,15 @@ ce_up_bwd_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64
     float* sT1 = s_dyn + J * kTQ;
     float* s_lo0 = s_dyn + 2 * J * kTQ;
     float* s_lo1 = s_lo0 + maxcols * C;
-    float* s_oh = s_lo1 + maxcols * C;
     const float wgt = __uint_as_float(state[4]) * (gscale ? *gscale : 1.f);
     const float ry = area_scale(h, H), rx = area_scale(w, W);
-    const int n = blockIdx.z, ci = blockIdx.y, x0 = blockIdx.x * kXS, x1 = min(W, x0 + kXS);
+    const int n = blockIdx.z, ci = 2 * blockIdx.y + row_phase, x0 = (blockIdx.x * strip_step + strip_phase) * kXS;
+    if (ci >= h || x0 >= W) return;
+    const int x1 = min(W, x0 + kXS);
     const int nx = x1 - x0;
     const BandGeom g = band_geom(ry, rx, ci, x0, x1, h, H, w);
     if (g.ncols > maxcols) __trap();
-    stage_rows<kT, true>(lo, cs, h, w, n, ci, g, C, C, s_lo0, s_lo1, s_oh);   // and clear the one-hot tile
+    stage_rows<kT>(lo, cs, h, w, n, ci, g, C, C, s_lo0, s_lo1);
     const int xloc = threadIdx.x >> 2, qd = threadIdx.x & 3;
     const int x = x0 + xloc;
     const bool xin = x < x1;
@@ -160,23 +164,16 @@ ce_up_bwd_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64
         const Lerp ly = make_lerp(ry, y, h);
         if (ly.i0 != ci || !xin) continue;
         if (lab == (long long)ignore_label) continue;
+        const int t = (int)lab;
 #pragma unroll
         for (int j = 0; j < kJMax; ++j) {
             const int c = 4 * j + qd;
             if (c < C) {
                 const float v = lerp_v(ly, sT0[t_index(c, xloc)], sT1[t_index(c, xloc)]);
-                const float p = __expf(v - lse) * wgt;
+                const float p = __expf(v - lse) * wgt - (c == t ? wgt : 0.f);
                 G0[j] = fmaf(ly.l0, p, G0[j]);
                 G1[j] = fmaf(ly.l1, p, G1[j]);
             }
-        }
-        if (qd == 0) {
-            const int t = (int)lab;
-            const float a0 = -wgt * ly.l0, a1 = -wgt * ly.l1;
-            atomicAdd(s_oh + j0 * C + t, a0 * lx.l0);
-            atomicAdd(s_oh + j1 * C + t, a0 * lx.l1);
-            atomicAdd(s_oh + (g.ncols + j0) * C + t, a1 * lx.l0);
-            atomicAdd(s_oh + (g.ncols + j1) * C + t, a1 * lx.l1);
         }
     }
     // hand-over in place: entry (c, xloc) of sT0 / sT1 was only ever read by this thread (and its quad for the target class
@@ -187,14 +184,17 @@ ce_up_bwd_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64
         if (c < C) { sT0[t_index(c, xloc)] = G0[j]; sT1[t_index(c, xloc)] = G1[j]; }
     }
     __syncthreads();
-    // phase 2, starting from the one-hot tile
+    // phase 2. No other band of this launch touches these elements (rows ci, i1 belong to this band's row pair; columns
+    // [jbase, jbase + ncols) to this strip of the strip phase), so the read-modify-write needs no atomics; when the band
+    // is one row (i1 == ci) the bottom sum is added after the top one.
     const int npairs = g.ncols * C;
     for (int q = threadIdx.x; q < npairs; q += kT) {
         const int j = q / C, c = q - j * C;
-        const float2 s = col_sums(sT0, sT1, [&](int xx) { return t_index(c, xx); }, s_seg, s_l0, s_l1, g, w, j,
-                                  s_oh[j * C + c], s_oh[(g.ncols + j) * C + c]);
-        if (s.x != 0.f) atomicAdd(dlo + (((long long)n * h + ci) * w + g.jbase + j) * cs + c, s.x);
-        if (s.y != 0.f) atomicAdd(dlo + (((long long)n * h + g.i1) * w + g.jbase + j) * cs + c, s.y);
+        const float2 s = col_sums(sT0, sT1, [&](int xx) { return t_index(c, xx); }, s_seg, s_l0, s_l1, g, w, j, 0.f, 0.f);
+        float* top = dlo + (((long long)n * h + ci) * w + g.jbase + j) * cs + c;
+        float* bot = dlo + (((long long)n * h + g.i1) * w + g.jbase + j) * cs + c;
+        if (s.x != 0.f) *top += s.x;
+        if (s.y != 0.f) *bot += s.y;
     }
 }
 
@@ -202,8 +202,11 @@ ce_up_bwd_kernel(const float* __restrict__ lo, int cs, int h, int w, const int64
 // geometries too, so that a loss it accepts can always be differentiated.
 static size_t bwd_smem(int C, int w, int W) {
     const int maxcols = band_maxcols(kXS, w, W);
-    const size_t smem = sizeof(float) * (2 * (size_t)((C + 3) / 4) * kTQ + 4 * (size_t)maxcols * C);
-    return maxcols <= kXS && smem <= 110 * 1024 ? smem : 0;
+    // the geometries accepted keep the bound 4·(2·J·kTQ + 4·maxcols·C) <= 110 KB that the forward's refusals and the band
+    // geometry tables rely on; the kernel itself uses the sT arrays and the two staged rows
+    const size_t bound = sizeof(float) * (2 * (size_t)((C + 3) / 4) * kTQ + 4 * (size_t)maxcols * C);
+    const size_t smem = sizeof(float) * (2 * (size_t)((C + 3) / 4) * kTQ + 2 * (size_t)maxcols * C);
+    return maxcols <= kXS && bound <= 110 * 1024 ? smem : 0;
 }
 
 }  // namespace
@@ -241,7 +244,21 @@ extern "C" int tsb_ce_up_bwd(const float* logits_lo, int cs, int h, int w, const
     TSB_REQUIRE(smem != 0, "tsb_ce_up_bwd: shared memory budget exceeded");
     int rc = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(ce_up_bwd_kernel), smem);
     if (rc) return rc;
-    ce_up_bwd_kernel<<<dim3((W + kXS - 1) / kXS, h, N), kT, smem, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, lse, C, H, W, ignore_label, state, gscale, dlogits_lo, maxcols);
-    TSB_CUDA_CHECK_LAUNCH("ce_up_bwd");
+    // strips s and s + P touch disjoint low-res columns once ((P − 1)·kXS + 1)·rx >= 2 (the last column of strip s is at
+    // most floor((x0 + kXS − 1)·rx) + 1, the first of strip s + P floor((x0 + P·kXS)·rx)); the margin covers the float
+    // rounding of the stencil positions. rx = 0 (one low-res column, or one output column): every strip has its own launch.
+    const int nstrips = (W + kXS - 1) / kXS;
+    const float rx = area_scale(w, W);
+    int P = rx > 0.f ? 1 + (int)ceilf(2.5f / ((float)kXS * rx)) : nstrips;
+    P = P < 2 ? 2 : P;
+    P = P > nstrips ? nstrips : P;
+    for (int rp = 0; rp < 2 && rp < h; ++rp)
+        for (int sp = 0; sp < P; ++sp) {
+            const dim3 grid((nstrips - sp + P - 1) / P, (h - rp + 1) / 2, N);
+            ce_up_bwd_kernel<<<grid, kT, smem, (cudaStream_t)stream>>>(logits_lo, cs, h, w, labels, lse, C, H, W,
+                                                                       ignore_label, state, gscale, dlogits_lo, maxcols,
+                                                                       rp, sp, P);
+            TSB_CUDA_CHECK_LAUNCH("ce_up_bwd");
+        }
     return TSB_OK;
 }

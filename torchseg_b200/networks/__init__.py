@@ -4,3 +4,4 @@ from .pspnet import PSPNet, PyramidPooling
 from .dfn import DFN, DFNHead
 from .psanet import PSANet, PointwiseSpatialAttention
 from .deeplabv3plus import DeepLabV3Plus, ASPP, Decoder
+from .encnet import EncNet, EncModule, EncHead

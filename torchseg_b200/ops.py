@@ -924,13 +924,13 @@ class DWConvFn(torch.autograd.Function):
 
 
 class BNFn(torch.autograd.Function):
-    """y = BN(x) without an activation, on the BatchNorm half of ConvBNActFn: the `bn` between the depthwise and the
-    pointwise conv of SeparableConvBnRelu (TorchSeg furnace/seg_opr/seg_oprs.py:88,93). Training takes the batch
-    statistics with tsb_bn_stats (summed over the SyncBN group like every other BN) and updates the running statistics;
-    eval applies the running statistics. x: dense bf16 NHWC [N,C,H,W]."""
+    """y = BN(x), followed by a ReLU when `relu`, on the BatchNorm half of ConvBNActFn: the `bn` between the depthwise and
+    the pointwise conv of SeparableConvBnRelu (TorchSeg furnace/seg_opr/seg_oprs.py:88,93), and EncNet's BN + ReLU over
+    the codewords. Training takes the batch statistics with tsb_bn_stats (summed over the SyncBN group like every other
+    BN) and updates the running statistics; eval applies the running statistics. x: dense bf16 NHWC [N,C,H,W]."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, running_mean, running_var, eps, momentum, training):
+    def forward(ctx, x, gamma, beta, running_mean, running_var, eps, momentum, training, relu=False):
         N, C, H, W = x.shape
         assert cs_of(x) == C
         count = float(N * H * W) * _sync["world"]
@@ -938,10 +938,10 @@ class BNFn(torch.autograd.Function):
         if training:
             stats = zero_arena.take((2, C), x.device)
             call("tsb_bn_stats", ptr(x), C, N * H * W, C, ptr(stats[0]), ptr(stats[1]), *det_ws(), stream())
-        y, aux = _bn_forward(x, stats, count, gamma, beta, None, running_mean, running_var, False, eps, momentum,
+        y, aux = _bn_forward(x, stats, count, gamma, beta, None, running_mean, running_var, relu, eps, momentum,
                              training)
         ctx.save_for_backward(x, gamma, aux)
-        ctx.beta_ref, ctx.count, ctx.training = beta, count, training
+        ctx.beta_ref, ctx.count, ctx.training, ctx.relu = beta, count, training, relu
         return y
 
     @staticmethod
@@ -950,10 +950,120 @@ class BNFn(torch.autograd.Function):
         assert ctx.training, "backward through eval-mode BN is not supported"
         beta = ctx.beta_ref
         direct = _direct_grad(gamma) and _direct_grad(beta)
-        dx, _, dgamma, dbeta = _bn_backward(dy, None, x, aux, gamma, beta, ctx.count, False, False, direct)
+        # without a residual the ReLU mask is recomputed from x, scale and shift (no read of y)
+        dx, _, dgamma, dbeta = _bn_backward(dy, None, x, aux, gamma, beta, ctx.count, ctx.relu, False, direct)
         if direct:
             _notify(gamma, beta)
-        return dx, dgamma, dbeta, None, None, None, None, None
+        return dx, dgamma, dbeta, None, None, None, None, None, None
+
+
+# --------------------------------------------------------------------------------------------------
+# EncNet: Context Encoding, mean over the codewords, SE-loss
+# --------------------------------------------------------------------------------------------------
+def _encoding_args(x, codewords, scale):
+    N, D, H, W = x.shape
+    K = codewords.shape[0]
+    assert codewords.shape == (K, D) and scale.shape == (K,), "codewords [K, D] and scale [K] expected"
+    assert codewords.is_contiguous() and scale.is_contiguous()
+    return N, D, H * W, K
+
+
+def encoding_infer(x, codewords, scale):
+    """the Encoding forward without the saved soft-assignments (inference): E as bf16 NHWC [B, K, D, 1]"""
+    B, D, HW, K = _encoding_args(x, codewords, scale)
+    E = nhwc_empty(B, K, D, 1, device=x.device)
+    sum_a = torch.empty((B, K), dtype=torch.float32, device=x.device)
+    call("tsb_encoding_fwd", ptr(x), cs_of(x), B, HW, D, ptr(codewords), ptr(scale), K, None, None, ptr(sum_a), ptr(E),
+         *det_ws(), stream())
+    return E
+
+
+class EncodingFn(torch.autograd.Function):
+    """EncNet's Encoding layer: E_bk = Σ_i softmax_k(s_k ‖x_i − c_k‖²) (x_i − c_k) over the pixels of image b, on
+    tsb_encoding_{fwd,bwd}; the [B, HW, K, D] residuals are never formed. x: bf16 NHWC [B, D, h, w]. E comes back as the
+    bf16 NHWC tensor [B, K, D, 1] (row b·D + d, channel k), so the codeword BN runs on it as on any activation."""
+
+    @staticmethod
+    def forward(ctx, x, codewords, scale):
+        B, D, HW, K = _encoding_args(x, codewords, scale)
+        dev = x.device
+        a = torch.empty((B * HW, K), dtype=torch.float32, device=dev)
+        d2 = torch.empty((B * HW, K), dtype=torch.float32, device=dev)
+        sum_a = torch.empty((B, K), dtype=torch.float32, device=dev)
+        E = nhwc_empty(B, K, D, 1, device=dev)
+        call("tsb_encoding_fwd", ptr(x), cs_of(x), B, HW, D, ptr(codewords), ptr(scale), K, ptr(a), ptr(d2), ptr(sum_a),
+             ptr(E), *det_ws(), stream())
+        ctx.save_for_backward(x, codewords, scale, a, d2, sum_a)
+        return E
+
+    @staticmethod
+    def backward(ctx, dE):
+        x, codewords, scale, a, d2, sum_a = ctx.saved_tensors
+        B, D, H, W = x.shape
+        K = codewords.shape[0]
+        if dE.dtype != _BF or dE.stride(1) != 1 or cs_of(dE) != K:
+            dE = to_nhwc(dE)
+        direct = _direct_grad(codewords) and _direct_grad(scale)
+        if direct:
+            dc, ds = codewords.grad, scale.grad
+        else:
+            dc, ds = torch.zeros_like(codewords), torch.zeros_like(scale)
+        dx = nhwc_empty(B, D, H, W, device=x.device)
+        call("tsb_encoding_bwd", ptr(dE), ptr(x), cs_of(x), B, H * W, D, ptr(codewords), ptr(scale), K, ptr(a), ptr(d2),
+             ptr(sum_a), ptr(dx), D, ptr(dc), ptr(ds), *det_ws(), stream())
+        if direct:
+            _notify(codewords, scale)
+            return dx, None, None
+        return dx, dc, ds
+
+
+class ChanMeanFn(torch.autograd.Function):
+    """mean over the C channels of each pixel: [N, C, H, W] → [N·H·W] values, returned as the bf16 NHWC [N, H·W, 1, 1]
+    (EncNet's mean over the K codewords of E [B, K, D, 1] gives en [B, D, 1, 1])"""
+
+    @staticmethod
+    def forward(ctx, x):
+        N, C, H, W = x.shape
+        y = nhwc_empty(N, H * W, 1, 1, device=x.device)
+        call("tsb_chan_mean_fwd", ptr(x), cs_of(x), N * H * W, C, ptr(y), stream())
+        ctx.shape = (N, C, H, W)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        N, C, H, W = ctx.shape
+        if dy.dtype != _BF or not dy.is_contiguous():
+            dy = dy.to(_BF).contiguous()   # [N, H·W, 1, 1]: contiguous is the dense NHWC layout
+        dx = nhwc_empty(N, C, H, W, device=dy.device)
+        call("tsb_chan_mean_bwd", ptr(dy), N * H * W, C, ptr(dx), C, stream())
+        return dx
+
+
+class SELossFn(torch.autograd.Function):
+    """EncNet's SE-loss: nn.BCELoss(sigmoid(z), presence(label)) with presence[b, c] = any(label[b] == c), c in [0, C),
+    built on the device (tsb_se_loss_fwd_bwd): no host synchronisation, so the step stays one graph replay. z: fp32 NHWC
+    [B, C, 1, 1] logits (any channel stride); label: int64 [B, H, W]."""
+
+    @staticmethod
+    def forward(ctx, z, label, num_classes):
+        B = z.shape[0]
+        C = int(num_classes)
+        assert z.dtype == torch.float32 and z.shape[1] == C and z.shape[0] == label.shape[0]
+        label = label.contiguous()
+        zs = cs_of(z)
+        dev = z.device
+        presence = torch.empty((B, (C + 31) // 32), dtype=torch.int32, device=dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        dz = nhwc_zeros(B, C, 1, 1, dtype=torch.float32, device=dev, cs=zs)
+        call("tsb_se_loss_fwd_bwd", ptr(label), B, label[0].numel(), ptr(z), zs, C, ptr(presence), ptr(loss), ptr(dz),
+             zs, stream())
+        ctx.save_for_backward(dz)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        (dz,) = ctx.saved_tensors
+        return dz * g.to(dz.dtype), None, None
 
 
 # --------------------------------------------------------------------------------------------------

@@ -289,6 +289,31 @@ class SeparableConvBnRelu(nn.Module):
         return conv_bn_act(t, pw.conv, pw.bn, pw.has_relu)
 
 
+class Encoding(nn.Module):
+    """EncNet's Context Encoding layer (Zhang et al., CVPR 2018): K codewords c_k ([K, D], `codewords`) with smoothing
+    factors s_k ([K], `scale`); E_bk = Σ_i a_ik (x_i − c_k) over the pixels x_i of image b with a_ik = softmax_k(s_k
+    ‖x_i − c_k‖²). Input [B, D, h, w]; output the bf16 NHWC [B, K, D, 1]. Runs on tsb_encoding_{fwd,bwd}: K a multiple
+    of 8 and at most 32, D a multiple of 64 (include/tsb.h); under no_grad nothing is saved for a backward."""
+
+    def __init__(self, D, K):
+        super(Encoding, self).__init__()
+        self.D, self.K = D, K
+        self.codewords = nn.Parameter(torch.empty(K, D, dtype=torch.float))
+        self.scale = nn.Parameter(torch.empty(K, dtype=torch.float))
+        self.reset_params()
+
+    def reset_params(self):
+        std = 1.0 / (self.K * self.D) ** 0.5
+        self.codewords.data.uniform_(-std, std)
+        self.scale.data.uniform_(-1, 0)
+
+    def forward(self, x):
+        x = _as_act(x)
+        if torch.is_grad_enabled():
+            return ops.EncodingFn.apply(x, self.codewords, self.scale)
+        return ops.encoding_infer(x, self.codewords, self.scale)
+
+
 class ReluFn(torch.autograd.Function):
     """stand-alone ReLU on a small tensor (FFM squeeze branch [N,C,1,1], seg_oprs.py:224-226): expressed through
     tsb_bn_apply with scale 1 / shift 0 so it stays on the library path"""
