@@ -2,8 +2,9 @@
 
 A training-mode forward updates the BN running statistics inside tsb_bn_finalize, through raw pointers that autograd's
 version counters do not see. The fake finalize below writes them the same way (through `.data`, which shares the storage
-but not the version counter), so these tests check that the two finalize call sites (ops._bn_forward and the BiSeNet
-stem pair) make the next eval-mode fold rebuild from the new statistics, for the plain, stem and transposed folds."""
+but not the version counter), so these tests check that the finalize step (ops._bn_finalize, reached through
+ops._bn_forward and the BiSeNet stem pair) makes the next eval-mode fold rebuild from the new statistics, for the plain,
+stem and transposed folds."""
 import pytest
 import torch
 import torch.nn as nn

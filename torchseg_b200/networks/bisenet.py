@@ -13,7 +13,8 @@ import torch.nn as nn
 
 from .. import ops
 from ..base_model import resnet18
-from ..seg_opr.seg_oprs import ConvBnRelu, AttentionRefinement, FeatureFusion, conv_plain, upsample_bilinear, _as_act
+from ..seg_opr.seg_oprs import (ConvBnRelu, AttentionRefinement, FeatureFusion, conv_plain, upsample_bilinear, _as_act,
+                                _bn_momentum, _packed_image)
 
 
 class _Cfg(object):
@@ -78,13 +79,11 @@ class BiSeNetBody(nn.Module):
         # shared space-to-depth image. Otherwise each stem reads the (cached) space-to-depth image on its own.
         if (data.shape[1] == 3 and isinstance(getattr(cp, "conv1", None), nn.Conv2d) and sp.conv_7x7.bn.training
                 and cp.bn1.training):
-            from ..seg_opr.seg_oprs import _packed_image
             bs, bc = sp.conv_7x7.bn, cp.bn1
             s_stem, c_stem = ops.StemPairFn.apply(
                 _packed_image(data), sp.conv_7x7.conv.weight, bs.weight, bs.bias, bs.running_mean, bs.running_var,
                 cp.conv1.weight, bc.weight, bc.bias, bc.running_mean, bc.running_var,
-                float(bs.eps), float(bs.momentum if bs.momentum is not None else 0.1),
-                float(bc.eps), float(bc.momentum if bc.momentum is not None else 0.1))
+                float(bs.eps), _bn_momentum(bs), float(bc.eps), _bn_momentum(bc))
             spatial_out = sp.forward_from_stem(s_stem)
             context_blocks = cp.forward_from_stem(c_stem)
         else:
@@ -177,33 +176,6 @@ class BiSeNetHead(nn.Module):
     def forward(self, x):
         lo = self.lowres_logits(x)
         if self.scale > 1:
-            return _UpsampleLogitsFn.apply(lo, lo.shape[2] * self.scale, lo.shape[3] * self.scale)
+            return ops.UpsampleLogitsFn.apply(lo, lo.shape[2] * self.scale, lo.shape[3] * self.scale)
         return lo
 
-
-class _UpsampleLogitsFn(torch.autograd.Function):
-    """reference-boundary form of the head tail: NCHW fp32 [N,C,H,W] logits, bilinear align_corners=True to an explicit
-    output size (network.py:164-166 use scale_factor; with align_corners the source coordinate is (in-1)/(out-1)·dst
-    either way, so size = in·scale is the same op — and sizes like 713 / 473 that are not a multiple of 8 work too)"""
-
-    @staticmethod
-    def forward(ctx, lo, H, W):
-        N, C, h, w = lo.shape
-        H, W = int(H), int(W)
-        out = torch.empty((N, C, H, W), dtype=torch.float32, device=lo.device)
-        ops.call("tsb_bilinear_fwd_nhwc_to_nchw", ops.ptr(lo), ops._lib.dt(lo), ops.cs_of(lo), ops.ptr(out), N, C, h, w,
-                 H, W, ops.stream())
-        ctx.shape = (N, C, h, w, H, W, ops.cs_of(lo))
-        return out
-
-    @staticmethod
-    def backward(ctx, g):
-        N, C, h, w, H, W, cs = ctx.shape
-        # gather-form transpose needs NHWC with C % 8 == 0: pad the class dimension into a 32-wide buffer
-        Cp = (C + 7) // 8 * 8
-        gp = ops.nhwc_zeros(N, Cp, H, W, dtype=torch.float32, device=g.device)
-        gp[:, :C].copy_(g)
-        d = ops.nhwc_zeros(N, Cp, h, w, dtype=torch.float32, device=g.device, cs=max(cs, Cp))
-        ops.call("tsb_bilinear_bwd", ops.ptr(gp), ops.F32, Cp, ops.ptr(d), ops.F32, ops.cs_of(d), N, Cp, h, w, H, W, 0,
-                 ops.stream())
-        return d[:, :C], None, None

@@ -23,7 +23,6 @@ import torch.nn as nn
 from .. import ops
 from ..base_model import resnet101
 from ..seg_opr.seg_oprs import ConvBnRelu, SeparableConvBnRelu, conv_plain, upsample_bilinear, _as_act
-from .bisenet import _UpsampleLogitsFn
 from .pspnet import PSPNet, _config, _dropout2d
 
 
@@ -46,11 +45,11 @@ class DeepLabV3Plus(nn.Module):
         lo = self.decoder(self.aspp(blocks[-1]), blocks[0])
         if label is None:
             H, W = int(data.shape[2]), int(data.shape[3])
-            return torch.log_softmax(_UpsampleLogitsFn.apply(lo, H, W), dim=1)
+            return torch.log_softmax(ops.UpsampleLogitsFn.apply(lo, H, W), dim=1)
         crit = self.criterion
         if hasattr(crit, "forward_lowres"):
             return crit.forward_lowres(lo, label, self.out_planes)
-        return crit(_UpsampleLogitsFn.apply(lo, label.shape[-2], label.shape[-1]), label)
+        return crit(ops.UpsampleLogitsFn.apply(lo, label.shape[-2], label.shape[-1]), label)
 
 
 class ASPP(nn.Module):

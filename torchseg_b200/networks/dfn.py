@@ -16,7 +16,6 @@ import torch.nn as nn
 from .. import ops
 from ..base_model import resnet101
 from ..seg_opr.seg_oprs import ConvBnRelu, RefineResidual, ChannelAttention, conv_plain, upsample_bilinear, _as_act
-from .bisenet import _UpsampleLogitsFn
 from .pspnet import _ignore_index_of
 
 
@@ -139,7 +138,8 @@ class DFN(nn.Module):
                 raise ValueError("DFN: label size must be scale x the head resolution")
             li = self._smooth_loss(lo, label)
             if li is None:
-                li = self.criterion(_UpsampleLogitsFn.apply(lo, lo.shape[2] * head.scale, lo.shape[3] * head.scale), label)
+                up = ops.UpsampleLogitsFn.apply(lo, lo.shape[2] * head.scale, lo.shape[3] * head.scale)
+                li = self.criterion(up, label)
             loss = li if loss is None else loss + li
         aux_loss = None
         for fm, head in zip(border, self.border_heads):
@@ -166,5 +166,5 @@ class DFNHead(nn.Module):
     def forward(self, x):
         lo = self.lowres_logits(x)
         if self.scale > 1:
-            return _UpsampleLogitsFn.apply(lo, lo.shape[2] * self.scale, lo.shape[3] * self.scale)
+            return ops.UpsampleLogitsFn.apply(lo, lo.shape[2] * self.scale, lo.shape[3] * self.scale)
         return lo

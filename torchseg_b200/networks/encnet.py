@@ -19,8 +19,7 @@ import torch.nn as nn
 
 from .. import ops
 from ..base_model import resnet101
-from ..seg_opr.seg_oprs import ConvBnRelu, Encoding, SELayer, conv_plain, _as_act
-from .bisenet import _UpsampleLogitsFn
+from ..seg_opr.seg_oprs import ConvBnRelu, Encoding, SELayer, conv_plain, _as_act, _bn_momentum
 from .pspnet import PSPNet, _config, _dropout2d, _ignore_index_of, head_loss
 
 
@@ -51,7 +50,7 @@ class EncNet(nn.Module):
         H, W = int(data.shape[2]), int(data.shape[3])
         lo, se = self.head(blocks[-1], with_se=label is not None)
         if label is None:
-            return torch.log_softmax(_UpsampleLogitsFn.apply(lo, H, W), dim=1)
+            return torch.log_softmax(ops.UpsampleLogitsFn.apply(lo, H, W), dim=1)
         ign = _ignore_index_of(self.criterion)
         loss = head_loss(lo, label, H, W, self.out_planes, ign)
         aux_loss = head_loss(self._aux_logits(blocks[-2]), label, H, W, self.out_planes, ign)
@@ -76,8 +75,7 @@ class EncModule(nn.Module):
         f = _as_act(f)
         E = self.encoding(self.conv(f))                 # [B, K, D, 1]: rows b·D + d, channel k
         bn = self.bn
-        momentum = bn.momentum if bn.momentum is not None else 0.1
-        e = ops.BNFn.apply(E, bn.weight, bn.bias, bn.running_mean, bn.running_var, float(bn.eps), float(momentum),
+        e = ops.BNFn.apply(E, bn.weight, bn.bias, bn.running_mean, bn.running_var, float(bn.eps), _bn_momentum(bn),
                            bool(bn.training), True)
         en = ops.ChanMeanFn.apply(e)                     # [B, D, 1, 1]
         # relu(f + f·γ) is f·(1 + γ): f is a ReLU output and 1 + γ > 0, so the relu is the identity, and its backward

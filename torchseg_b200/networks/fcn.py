@@ -37,8 +37,7 @@ class FCN(nn.Module):
         blocks = self.backbone(data)
         lo = self.head.lowres_logits(blocks[-1])
         if label is None:
-            from .bisenet import _UpsampleLogitsFn
-            return _UpsampleLogitsFn.apply(lo, lo.shape[2] * 32, lo.shape[3] * 32)
+            return ops.UpsampleLogitsFn.apply(lo, lo.shape[2] * 32, lo.shape[3] * 32)
         lo_aux = self.aux_head.lowres_logits(blocks[-2])
         H, W = label.shape[-2:]
         K = self.out_planes

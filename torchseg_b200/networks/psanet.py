@@ -15,7 +15,6 @@ import torch.nn as nn
 from .. import ops
 from ..base_model import resnet50, resnet101
 from ..seg_opr.seg_oprs import ConvBnRelu, conv_plain, _as_act
-from .bisenet import _UpsampleLogitsFn
 from .pspnet import _ignore_index_of, _dropout2d, _config, head_loss, PSPNet as _PSPNetBase
 
 
@@ -50,7 +49,7 @@ class PSANet(nn.Module):
         H, W = int(data.shape[2]), int(data.shape[3])
         psa_lo = self.psa_layer(blocks[-1])
         if label is None:
-            return torch.log_softmax(_UpsampleLogitsFn.apply(psa_lo, H, W), dim=1)   # network.py:46-51
+            return torch.log_softmax(ops.UpsampleLogitsFn.apply(psa_lo, H, W), dim=1)   # network.py:46-51
         ign = _ignore_index_of(self.criterion)
         loss = head_loss(psa_lo, label, H, W, self.out_planes, ign)
         aux_loss = head_loss(self._aux_logits(blocks[-2]), label, H, W, self.out_planes, ign)

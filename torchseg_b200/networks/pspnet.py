@@ -14,7 +14,6 @@ import torch.nn as nn
 from .. import ops
 from ..base_model import resnet50, resnet101
 from ..seg_opr.seg_oprs import ConvBnRelu, conv_plain, upsample_bilinear, _as_act
-from .bisenet import _UpsampleLogitsFn
 
 
 class _Cfg(object):
@@ -41,7 +40,7 @@ def head_loss(lo, label, H, W, num_classes, ignore_index):
     logits go through the OHEM kernels with min_kept = 0, which is exactly CrossEntropyLoss."""
     if FUSED_CE and num_classes <= ops.FUSED_CE_MAX_CLASSES:
         return ops.CEUpFn.apply(lo, label, H, W, num_classes, ignore_index)
-    return ops.OhemCEFn.apply(_UpsampleLogitsFn.apply(lo, H, W), label, ignore_index, 1.0, 0, None)
+    return ops.OhemCEFn.apply(ops.UpsampleLogitsFn.apply(lo, H, W), label, ignore_index, 1.0, 0, None)
 
 
 def _dropout2d(x, p, training):
@@ -87,7 +86,7 @@ class PSPNet(nn.Module):
         H, W = int(data.shape[2]), int(data.shape[3])
         psp_lo = self.psp_layer(blocks[-1])
         if label is None:
-            return torch.log_softmax(_UpsampleLogitsFn.apply(psp_lo, H, W), dim=1)   # network.py:46-51
+            return torch.log_softmax(ops.UpsampleLogitsFn.apply(psp_lo, H, W), dim=1)   # network.py:46-51
         ign = _ignore_index_of(self.criterion)
         loss = head_loss(psp_lo, label, H, W, self.out_planes, ign)
         aux_loss = head_loss(self._aux_logits(blocks[-2]), label, H, W, self.out_planes, ign)

@@ -60,6 +60,12 @@ def to_nhwc(t, dtype=_BF):
     return out
 
 
+def as_nhwc_bf16(t):
+    """t itself when it is a bf16 tensor with unit channel stride (an incoming gradient usually is), else a dense bf16
+    NHWC copy"""
+    return t if t.dtype == _BF and t.stride(1) == 1 else to_nhwc(t)
+
+
 def _krsc_ptr(w):
     """pointer to a dense [K,R,S,C] fp32 buffer for conv weight w ([K,C,R,S] logical)"""
     wp = w.permute(0, 2, 3, 1)
@@ -206,10 +212,40 @@ def _direct_grad(p):
     return getattr(p, "_tsb_direct", False) and p.grad is not None
 
 
-def _notify(*params):
-    if grad_ready_hook is not None:
-        for p in params:
-            grad_ready_hook(p)
+class _ParamGrads(object):
+    """The parameter gradients of one op (None entries: an absent bias). `direct` when every parameter's .grad is a
+    persistent flat-buffer view: the kernels then accumulate into the live .grad, autograd receives None and the DDP
+    hook (`grad_ready_hook`) is told in `result`. Otherwise each gradient is a fresh tensor that goes back to autograd.
+    A buffer handed to a kernel is therefore either the live accumulating .grad or zeros, because the wgrad, bias-grad
+    and encoding kernels add into it (a wgrad with one split adds in place)."""
+
+    def __init__(self, *params):
+        self.params = params
+        self.direct = all(_direct_grad(p) for p in params if p is not None)
+        self.grads = {}
+
+    def buffer(self, p, krsc=False):
+        """the tensor the kernel accumulates p's gradient into; krsc: p is a conv weight, written as its dense KRSC
+        storage"""
+        if self.direct:
+            return p.grad.permute(0, 2, 3, 1) if krsc else p.grad
+        if krsc:
+            self.grads[id(p)], g = _new_wgrad(p)
+            return g
+        g = self.grads[id(p)] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+        return g
+
+    def set(self, p, g):
+        """autograd receives g for p (not direct: a gradient computed outside `buffer`)"""
+        self.grads[id(p)] = g
+
+    def result(self):
+        """what autograd receives, one entry per parameter"""
+        if self.direct and grad_ready_hook is not None:
+            for p in self.params:
+                if p is not None:
+                    grad_ready_hook(p)
+        return tuple(self.grads.get(id(p)) for p in self.params)
 
 # process group for SyncBN statistics (set by apex_shim.parallel.SyncBatchNorm / DistributedDataParallel)
 _sync = {"group": None, "world": 1, "p2p": None, "p2p_tried": False}
@@ -316,16 +352,14 @@ class _ConvProf(object):
     def disable(self):
         self.on = False
 
-    def begin(self):
+    def launch(self, flops, name, *args):
+        """call(name, *args), bracketed by CUDA events while enabled"""
         if not self.on:
-            return None
-        e = torch.cuda.Event(enable_timing=True)
-        e.record()
-        return e
-
-    def end(self, e0, flops):
-        if e0 is None:
+            call(name, *args)
             return
+        e0 = torch.cuda.Event(enable_timing=True)
+        e0.record()
+        call(name, *args)
         e1 = torch.cuda.Event(enable_timing=True)
         e1.record()
         self.recs.append((e0, e1, flops))
@@ -355,10 +389,8 @@ def conv_fprop(x, wb, K, R, stride, pad, dil, bias=None, out_dtype=_BF, out=None
     s1 = s2 = None
     if stats is not None:
         s1, s2 = stats[0], stats[1]
-    ev = conv_prof.begin()
-    call("tsb_conv2d_fprop", ctypes.byref(shp), ptr(x), cs_of(x), ptr(wb), ptr(bias), ptr(out), _lib.dt(out), cs_of(out),
-         ptr(s1), ptr(s2), *det_ws(), stream())
-    conv_prof.end(ev, _conv_flops(shp))
+    conv_prof.launch(_conv_flops(shp), "tsb_conv2d_fprop", ctypes.byref(shp), ptr(x), cs_of(x), ptr(wb), ptr(bias), ptr(out),
+                     _lib.dt(out), cs_of(out), ptr(s1), ptr(s2), *det_ws(), stream())
     return out
 
 
@@ -371,10 +403,8 @@ def conv_transpose_fprop(x, wt, Co, R, stride, pad, dil, out_pad, bias=None, rel
     if out is None:
         out = nhwc_empty(N, Co, shp.H, shp.W, dtype=out_dtype, device=x.device)
     s1, s2 = (None, None) if stats is None else (stats[0], stats[1])
-    ev = conv_prof.begin()
-    call("tsb_conv_transpose2d_fprop", ctypes.byref(shp), ptr(x), cs_of(x), ptr(wt), ptr(bias), int(relu), ptr(out),
-         _lib.dt(out), cs_of(out), ptr(s1), ptr(s2), *det_ws(), stream())
-    conv_prof.end(ev, _conv_flops(shp))
+    conv_prof.launch(_conv_flops(shp), "tsb_conv_transpose2d_fprop", ctypes.byref(shp), ptr(x), cs_of(x), ptr(wt), ptr(bias),
+                     int(relu), ptr(out), _lib.dt(out), cs_of(out), ptr(s1), ptr(s2), *det_ws(), stream())
     return out
 
 
@@ -387,10 +417,8 @@ def conv_fprop_fused(x, wb, K, R, stride, pad, dil, bias, res=None, relu=False):
     if res is not None and (res.dtype != _BF or res.stride(1) != 1 or cs_of(res) != cs_of(out)):
         res = to_nhwc(res) if cs_of(out) == K else None
         assert res is not None, "residual layout must match the output"
-    ev = conv_prof.begin()
-    call("tsb_conv2d_fprop_fused", ctypes.byref(shp), ptr(x), cs_of(x), ptr(wb), ptr(bias), ptr(res),
-         cs_of(res) if res is not None else 0, int(relu), ptr(out), BF16, cs_of(out), stream())
-    conv_prof.end(ev, _conv_flops(shp))
+    conv_prof.launch(_conv_flops(shp), "tsb_conv2d_fprop_fused", ctypes.byref(shp), ptr(x), cs_of(x), ptr(wb), ptr(bias),
+                     ptr(res), cs_of(res) if res is not None else 0, int(relu), ptr(out), BF16, cs_of(out), stream())
     return out
 
 
@@ -399,9 +427,8 @@ def conv_stem_fprop_fused(xs2d, wp, K, bias, relu=True):
     N, _, H2, WP = xs2d.shape
     H, W = H2 * 2, (WP - 4) * 2
     out = nhwc_empty(N, K, H2, WP - 4, device=xs2d.device)
-    ev = conv_prof.begin()
-    call("tsb_conv_stem_fprop_fused", ptr(xs2d), N, H, W, ptr(wp), K, ptr(bias), int(relu), ptr(out), K, stream())
-    conv_prof.end(ev, 2.0 * N * H2 * (WP - 4) * K * 147)
+    conv_prof.launch(2.0 * N * H2 * (WP - 4) * K * 147, "tsb_conv_stem_fprop_fused", ptr(xs2d), N, H, W, ptr(wp), K,
+                     ptr(bias), int(relu), ptr(out), K, stream())
     return out
 
 
@@ -454,22 +481,20 @@ def conv_dgrad(dy, wt, xshape, K, R, stride, pad, dil, out=None, accumulate=Fals
     shp = make_shape(N, H, W, C, K, R, stride, pad, dil)
     if out is None:
         out = nhwc_empty(N, C, H, W, device=dy.device)
-    ev = conv_prof.begin()
     try:
-        call("tsb_conv2d_dgrad", ctypes.byref(shp), ptr(dy), cs_of(dy), ptr(wt), ptr(out), cs_of(out), int(accumulate), stream())
+        conv_prof.launch(_conv_flops(shp), "tsb_conv2d_dgrad", ctypes.byref(shp), ptr(dy), cs_of(dy), ptr(wt), ptr(out),
+                         cs_of(out), int(accumulate), stream())
     except RuntimeError as e:
         raise RuntimeError("%s [dgrad shape N=%d H=%d W=%d C=%d K=%d R=%d stride=%d pad=%d dil=%d]" % (
             e, N, H, W, C, K, R, stride, pad, dil)) from None
-    conv_prof.end(ev, _conv_flops(shp))
     return out
 
 
 def conv_wgrad(x, dy, K, R, stride, pad, dil, dw_krsc):
     N, C, H, W = x.shape
     shp = make_shape(N, H, W, C, K, R, stride, pad, dil)
-    ev = conv_prof.begin()
-    call("tsb_conv2d_wgrad", ctypes.byref(shp), ptr(x), cs_of(x), ptr(dy), cs_of(dy), ptr(dw_krsc), *det_ws(), stream())
-    conv_prof.end(ev, _conv_flops(shp))
+    conv_prof.launch(_conv_flops(shp), "tsb_conv2d_wgrad", ctypes.byref(shp), ptr(x), cs_of(x), ptr(dy), cs_of(dy),
+                     ptr(dw_krsc), *det_ws(), stream())
 
 
 def _new_wgrad(w):
@@ -511,6 +536,16 @@ class GradShare(object):
         return out
 
 
+def _dgrad_into(share, dgrad):
+    """the input gradient of one consumer at a GradShare fork (share None: no fork). dgrad(out, accumulate) runs the
+    consumer's dgrad into `out` (None: a fresh buffer it allocates) and returns that buffer: into the stash, adding,
+    when an earlier consumer started it, else into a fresh buffer that starts it. Returns what autograd receives."""
+    if share is not None and share.stash is not None:
+        return share.contribute(dgrad(share.stash, True), accumulated=True)
+    dx = dgrad(None, False)
+    return dx if share is None else share.contribute(dx)
+
+
 def _running_stats_written(running_mean, running_var):
     """tsb_bn_finalize updated the running statistics through raw pointers, which autograd's version counters do not
     see: bump them, so that what is keyed on those versions (the eval-mode fold cache) rebuilds from the new values. A
@@ -518,58 +553,71 @@ def _running_stats_written(running_mean, running_var):
     torch.autograd.graph.increment_version((running_mean, running_var))
 
 
+def _bn_finalize(aux, stats, count, gamma, beta, running_mean, running_var, eps, momentum, training):
+    """scale / shift of a BatchNorm into aux = [mean; invstd; scale; shift] (a channel slice of a wider aux). Training:
+    from the batch statistics stats = [Σ; Σ²] over `count` pixels (already summed over the SyncBN group), updating the
+    running statistics; eval: from the running statistics."""
+    if not training:
+        # sum := mean*1, sumsq := var + mean^2, count 1, no running-statistics update
+        stats = torch.stack([running_mean, running_var + running_mean * running_mean]).contiguous()
+        count, momentum, running_mean, running_var = 1.0, 0.0, None, None
+    call("tsb_bn_finalize", ptr(stats[0]), ptr(stats[1]), count, aux.shape[1], ptr(gamma), ptr(beta), eps, momentum,
+         ptr(aux[0]), ptr(aux[1]), ptr(aux[2]), ptr(aux[3]), ptr(running_mean), ptr(running_var), stream())
+    if training:
+        _running_stats_written(running_mean, running_var)
+
+
+def _bn_apply(raw, aux, residual, relu):
+    """y = act(raw * scale + shift + residual) over the dense NHWC raw [N,K,P,Q]"""
+    N, K, P, Q = raw.shape
+    y = nhwc_empty(N, K, P, Q, device=raw.device)
+    call("tsb_bn_apply", ptr(raw), K, ptr(aux[2]), ptr(aux[3]), ptr(residual), cs_of(residual) if residual is not None else 0,
+         int(relu), ptr(y), K, N * P * Q, K, stream())
+    return y
+
+
 def _bn_forward(raw, stats, count, gamma, beta, residual, running_mean, running_var, relu, eps, momentum, training):
     """the BatchNorm half of ConvBNActFn.forward: y = act(BN(raw) + residual) over the dense NHWC raw [N,K,P,Q]. Training
     normalises with the batch statistics stats = [Σ; Σ²] (summed over the SyncBN group here) and updates the running
     statistics; eval uses the running statistics. Returns (y, aux = [mean; invstd; scale; shift])."""
-    N, K, P, Q = raw.shape
-    aux = torch.empty((4, K), dtype=torch.float32, device=raw.device)  # mean, invstd, scale, shift
+    aux = torch.empty((4, raw.shape[1]), dtype=torch.float32, device=raw.device)
     if training:
         _allreduce_stats(stats)
-        call("tsb_bn_finalize", ptr(stats[0]), ptr(stats[1]), count, K, ptr(gamma), ptr(beta), eps, momentum,
-             ptr(aux[0]), ptr(aux[1]), ptr(aux[2]), ptr(aux[3]), ptr(running_mean), ptr(running_var), stream())
-        _running_stats_written(running_mean, running_var)
-    else:
-        # eval: scale/shift from the running statistics (sum := mean*1, sumsq := var + mean^2, count 1)
-        s = torch.stack([running_mean, running_var + running_mean * running_mean]).contiguous()
-        call("tsb_bn_finalize", ptr(s[0]), ptr(s[1]), 1.0, K, ptr(gamma), ptr(beta), eps, 0.0, ptr(aux[0]),
-             ptr(aux[1]), ptr(aux[2]), ptr(aux[3]), None, None, stream())
-    y = nhwc_empty(N, K, P, Q, device=raw.device)
-    call("tsb_bn_apply", ptr(raw), K, ptr(aux[2]), ptr(aux[3]), ptr(residual), cs_of(residual) if residual is not None else 0,
-         int(relu), ptr(y), K, N * P * Q, K, stream())
-    return y, aux
+    _bn_finalize(aux, stats, count, gamma, beta, running_mean, running_var, eps, momentum, training)
+    return _bn_apply(raw, aux, residual, relu), aux
 
 
-def _bn_backward(dy, y, raw, aux, gamma, beta, count, relu, has_res, direct):
-    """the BatchNorm half of ConvBNActFn.backward: (draw, dres, dgamma, dbeta). direct: gamma / beta (and the caller's
-    weight) take their gradients in their flat .grad views, and dgamma / dbeta are returned as None."""
+def _bn_backward(dy, y, raw, aux, gamma, beta, count, relu, has_res, grads, draw=None):
+    """the BatchNorm half of ConvBNActFn.backward: (draw, dres). raw / draw may be channel slices of wider NHWC buffers
+    (draw None: a fresh dense one), aux the matching [4, K] slice. gamma / beta take their gradients through `grads`
+    (_ParamGrads): accumulated into their flat .grad views when direct, else handed to autograd."""
     N, K, P, Q = raw.shape
     dev = raw.device
     npix = N * P * Q
-    if dy.dtype != _BF or dy.stride(1) != 1:
-        dy = to_nhwc(dy)
+    dy = as_nhwc_bf16(dy)
     red = zero_arena.take((2, K), dev)
     # ReLU mask: recomputed from raw*scale+shift when there is no residual (saves reading y in both passes)
     y_mask = ptr(y) if (relu and has_res) else None
-    call("tsb_bn_bwd_reduce", ptr(dy), cs_of(dy), y_mask, K, ptr(raw), K, ptr(aux[0]), ptr(aux[1]), int(relu), npix, K,
-         ptr(red[0]), ptr(red[1]), ptr(aux[2]), ptr(aux[3]), *det_ws(), stream())
+    ycs = cs_of(y) if y_mask is not None else (K if draw is None else 0)   # unread without y_mask
+    call("tsb_bn_bwd_reduce", ptr(dy), cs_of(dy), y_mask, ycs, ptr(raw), cs_of(raw), ptr(aux[0]), ptr(aux[1]), int(relu),
+         npix, K, ptr(red[0]), ptr(red[1]), ptr(aux[2]), ptr(aux[3]), *det_ws(), stream())
     # dgamma = Σ dz·x̂, dbeta = Σ dz are LOCAL sums (the DDP all-reduce averages parameter grads);
     # the dx formula needs the GLOBAL sums under SyncBN.
-    fold = direct and _sync["world"] == 1   # single GPU: the accumulation is folded into tsb_bn_bwd_apply
-    if direct:
-        dgamma = dbeta = None
+    fold = grads.direct and _sync["world"] == 1   # single GPU: the accumulation is folded into tsb_bn_bwd_apply
+    if grads.direct:
         # multi-GPU: the exchange kernel adds the LOCAL sums to gamma.grad / beta.grad before it reduces
         _allreduce_stats(red, None if fold else gamma.grad, None if fold else beta.grad)
     else:
-        dgamma = red[1].clone()
-        dbeta = red[0].clone()
+        grads.set(gamma, red[1].clone())
+        grads.set(beta, red[0].clone())
         _allreduce_stats(red)
-    draw = nhwc_empty(N, K, P, Q, device=dev)
+    if draw is None:
+        draw = nhwc_empty(N, K, P, Q, device=dev)
     dres = nhwc_empty(N, K, P, Q, device=dev) if has_res else None
-    call("tsb_bn_bwd_apply", ptr(dy), cs_of(dy), y_mask, K, ptr(raw), K, ptr(aux[0]), ptr(aux[1]), ptr(gamma), ptr(red[0]),
-         ptr(red[1]), count, int(relu), ptr(draw), K, ptr(dres), K if has_res else 0, npix, K,
+    call("tsb_bn_bwd_apply", ptr(dy), cs_of(dy), y_mask, ycs, ptr(raw), cs_of(raw), ptr(aux[0]), ptr(aux[1]), ptr(gamma),
+         ptr(red[0]), ptr(red[1]), count, int(relu), ptr(draw), cs_of(draw), ptr(dres), K if has_res else 0, npix, K,
          ptr(gamma.grad) if fold else None, ptr(beta.grad) if fold else None, ptr(aux[2]), ptr(aux[3]), stream())
-    return draw, dres, dgamma, dbeta
+    return draw, dres
 
 
 class ConvBNActFn(torch.autograd.Function):
@@ -606,10 +654,8 @@ class ConvBNActFn(torch.autograd.Function):
         raw = nhwc_empty(N, K, P, Q, device=dev)
         if stem:
             wp, _ = pack_cache.get(w, False, stem=True)
-            ev = conv_prof.begin()
-            call("tsb_conv_stem_fprop", ptr(x), N, H, W, ptr(wp), K, ptr(raw), K, ptr(stats[0]) if training else None,
-                 ptr(stats[1]) if training else None, *det_ws(), stream())
-            conv_prof.end(ev, 2.0 * N * P * Q * K * 147)
+            conv_prof.launch(2.0 * N * P * Q * K * 147, "tsb_conv_stem_fprop", ptr(x), N, H, W, ptr(wp), K, ptr(raw), K,
+                             ptr(stats[0]) if training else None, ptr(stats[1]) if training else None, *det_ws(), stream())
         elif transposed:
             _, wt = pack_cache.get(w, True)
             conv_transpose_fprop(x, wt, K, R, stride, pad, dil, out_pad, out=raw, stats=stats)
@@ -638,19 +684,15 @@ class ConvBNActFn(torch.autograd.Function):
         N, _, P, Q = raw.shape
         dev = dy.device
         beta = ctx.beta_ref
-        direct = _direct_grad(w) and _direct_grad(gamma) and _direct_grad(beta)
-        draw, dres, dgamma, dbeta = _bn_backward(dy, y, raw, aux, gamma, beta, count, relu, has_res, direct)
-        if direct:
-            dw_view, dw = None, w.grad.permute(0, 2, 3, 1)   # KRSC view of the flat gradient buffer
-        else:
-            dw_view, dw = _new_wgrad(w)
+        grads = _ParamGrads(w, gamma, beta)
+        draw, dres = _bn_backward(dy, y, raw, aux, gamma, beta, count, relu, has_res, grads)
+        dw = grads.buffer(w, krsc=True)
         dx = None
         if stem:
             H, W = P * 2, Q * 2
             dwp = zero_arena.take((K, 4, 64), dev)
-            ev = conv_prof.begin()
-            call("tsb_conv_stem_wgrad", ptr(x), N, H, W, ptr(draw), K, K, ptr(dwp), *det_ws(), stream())
-            conv_prof.end(ev, 2.0 * N * P * Q * K * 147)
+            conv_prof.launch(2.0 * N * P * Q * K * 147, "tsb_conv_stem_wgrad", ptr(x), N, H, W, ptr(draw), K, K, ptr(dwp),
+                             *det_ws(), stream())
             call("tsb_unpack_stem_wgrad", ptr(dwp), K, R, ptr(dw), stream())
         elif transposed:
             Ci = w.shape[0]
@@ -662,18 +704,11 @@ class ConvBNActFn(torch.autograd.Function):
             conv_wgrad(x, draw, K, R, stride, pad, dil, dw)
             if ctx.needs_input_grad[0]:
                 _, wt = pack_cache.get(w, True)
-                share = ctx.in_share
-                if share is not None and share.stash is not None:
-                    dx = conv_dgrad(draw, wt, x.shape, K, R, stride, pad, dil, out=share.stash, accumulate=True)
-                    dx = share.contribute(dx, accumulated=True)
-                else:
-                    dx = conv_dgrad(draw, wt, x.shape, K, R, stride, pad, dil)
-                    if share is not None:
-                        dx = share.contribute(dx)
+                dx = _dgrad_into(ctx.in_share, lambda out, acc: conv_dgrad(draw, wt, x.shape, K, R, stride, pad, dil,
+                                                                           out=out, accumulate=acc))
         if has_res and ctx.res_share is not None and ctx.needs_input_grad[4]:
             dres = ctx.res_share.contribute(dres)
-        if direct:
-            _notify(w, gamma, beta)
+        dw_view, dgamma, dbeta = grads.result()
         return dx, dw_view, dgamma, dbeta, dres, None, None, None, None, None, None, None, None, None, None, None, None, None
 
 
@@ -698,19 +733,15 @@ class StemPairFn(torch.autograd.Function):
         # two N=64 launches into the channel halves of one buffer: this layer is bound by the epilogue's stores and the
         # 64-column epilogue (one chunk per warp, register running sums) is the faster one; the wgrad below is fused
         for off, Kh in ((0, K1), (K1, K2)):
-            ev = conv_prof.begin()
-            call("tsb_conv_stem_fprop", ptr(xs), N, H, W, ptr(wp[off:]), Kh, ptr(raw[:, off:]), K, ptr(stats[0][off:]),
-                 ptr(stats[1][off:]), *det_ws(), stream())
-            conv_prof.end(ev, 2.0 * N * P * Q * Kh * 147)
+            conv_prof.launch(2.0 * N * P * Q * Kh * 147, "tsb_conv_stem_fprop", ptr(xs), N, H, W, ptr(wp[off:]), Kh,
+                             ptr(raw[:, off:]), K, ptr(stats[0][off:]), ptr(stats[1][off:]), *det_ws(), stream())
         _allreduce_stats(stats)
         count = float(N * P * Q) * _sync["world"]
         aux = torch.empty((4, K), dtype=torch.float32, device=dev)
-        for (off, Kh, g, b, rm, rv, eps, mom) in ((0, K1, g1, b1, rm1, rv1, eps1, mom1), (K1, K2, g2, b2, rm2, rv2, eps2, mom2)):
-            call("tsb_bn_finalize", ptr(stats[0][off:]), ptr(stats[1][off:]), count, Kh, ptr(g), ptr(b), eps, mom,
-                 ptr(aux[0][off:]), ptr(aux[1][off:]), ptr(aux[2][off:]), ptr(aux[3][off:]), ptr(rm), ptr(rv), stream())
-            _running_stats_written(rm, rv)
-        y = nhwc_empty(N, K, P, Q, device=dev)
-        call("tsb_bn_apply", ptr(raw), K, ptr(aux[2]), ptr(aux[3]), None, 0, 1, ptr(y), K, N * P * Q, K, stream())
+        for (h, g, b, rm, rv, eps, mom) in ((slice(0, K1), g1, b1, rm1, rv1, eps1, mom1),
+                                            (slice(K1, K), g2, b2, rm2, rv2, eps2, mom2)):
+            _bn_finalize(aux[:, h], stats[:, h], count, g, b, rm, rv, eps, mom, True)
+        y = _bn_apply(raw, aux, None, True)
         ctx.save_for_backward(xs, w1, g1, w2, g2, raw, aux)
         ctx.refs = (b1, b2)
         ctx.count = count
@@ -723,43 +754,29 @@ class StemPairFn(torch.autograd.Function):
         N, K, P, Q = raw.shape
         K1 = w1.shape[0]
         dev = raw.device
-        npix = N * P * Q
         draw = nhwc_empty(N, K, P, Q, device=dev)
-        grads = []
-        for (off, w, g, b, dy) in ((0, w1, g1, b1, dy1), (K1, w2, g2, b2, dy2)):
-            Kh = w.shape[0]
-            if dy.dtype != _BF or dy.stride(1) != 1:
-                dy = to_nhwc(dy)
-            red = zero_arena.take((2, Kh), dev)
-            xr = raw[:, off:off + Kh]
-            call("tsb_bn_bwd_reduce", ptr(dy), cs_of(dy), None, 0, ptr(xr), K, ptr(aux[0][off:]), ptr(aux[1][off:]), 1, npix, Kh,
-                 ptr(red[0]), ptr(red[1]), ptr(aux[2][off:]), ptr(aux[3][off:]), *det_ws(), stream())
-            direct = _direct_grad(w) and _direct_grad(g) and _direct_grad(b)
-            fold = direct and _sync["world"] == 1
-            dg, db = (None, None) if direct else (red[1].clone(), red[0].clone())
-            _allreduce_stats(red, g.grad if (direct and not fold) else None, b.grad if (direct and not fold) else None)
-            call("tsb_bn_bwd_apply", ptr(dy), cs_of(dy), None, 0, ptr(xr), K, ptr(aux[0][off:]), ptr(aux[1][off:]), ptr(g),
-                 ptr(red[0]), ptr(red[1]), ctx.count, 1, ptr(draw[:, off:off + Kh]), K, None, 0, npix, Kh,
-                 ptr(g.grad) if fold else None, ptr(b.grad) if fold else None, ptr(aux[2][off:]), ptr(aux[3][off:]), stream())
-            grads.append((direct, dg, db))
+        halves = []
+        for (h, w, g, b, dy) in ((slice(0, K1), w1, g1, b1, dy1), (slice(K1, K), w2, g2, b2, dy2)):
+            grads = _ParamGrads(w, g, b)
+            _bn_backward(dy, None, raw[:, h], aux[:, h], g, b, ctx.count, True, False, grads, draw=draw[:, h])
+            halves.append((h, w, grads))
         H, W = P * 2, Q * 2
         dwp = zero_arena.take((K, 4, 64), dev)
-        ev = conv_prof.begin()
-        call("tsb_conv_stem_wgrad", ptr(xs), N, H, W, ptr(draw), K, K, ptr(dwp), *det_ws(), stream())
-        conv_prof.end(ev, 2.0 * N * P * Q * K * 147)
+        conv_prof.launch(2.0 * N * P * Q * K * 147, "tsb_conv_stem_wgrad", ptr(xs), N, H, W, ptr(draw), K, K, ptr(dwp),
+                         *det_ws(), stream())
         outs = []
-        for (off, w, g, b), (direct, dg, db) in zip(((0, w1, g1, b1), (K1, w2, g2, b2)), grads):
-            Kh = w.shape[0]
-            if direct:
-                dwv, dw = None, w.grad.permute(0, 2, 3, 1)
-            else:
-                dwv, dw = _new_wgrad(w)
-            call("tsb_unpack_stem_wgrad", ptr(dwp[off:]), Kh, w.shape[2], ptr(dw), stream())
-            if direct:
-                _notify(w, g, b)
-            outs.append((dwv, dg, db))
+        for h, w, grads in halves:
+            call("tsb_unpack_stem_wgrad", ptr(dwp[h.start:]), w.shape[0], w.shape[2], ptr(grads.buffer(w, krsc=True)),
+                 stream())
+            outs.append(grads.result())
         (dw1, dg1, db1), (dw2, dg2, db2) = outs
         return None, dw1, dg1, db1, None, None, dw2, dg2, db2, None, None, None, None, None, None
+
+
+def _bias_grad(grads, bias, dy, dycs, npix, K):
+    """Σ dy over the pixels into the bias gradient (tsb_bias_grad), for a bias that is not None"""
+    if bias is not None:
+        call("tsb_bias_grad", ptr(dy), dycs, npix, K, ptr(grads.buffer(bias)), *det_ws(), stream())
 
 
 class ConvFn(torch.autograd.Function):
@@ -773,13 +790,13 @@ class ConvFn(torch.autograd.Function):
         y = conv_fprop(x, wb, K, R, stride, pad, dil, bias=bias, out_dtype=torch.float32 if out_f32 else _BF, ocs=ocs)
         ctx.save_for_backward(x, w)
         ctx.bias_ref = bias
-        ctx.cfg = (stride, pad, dil, bias is not None)
+        ctx.cfg = (stride, pad, dil)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, w = ctx.saved_tensors
-        stride, pad, dil, has_bias = ctx.cfg
+        stride, pad, dil = ctx.cfg
         K, C, R, _ = w.shape
         N, _, P, Q = dy.shape
         dev = dy.device
@@ -794,25 +811,14 @@ class ConvFn(torch.autograd.Function):
             else:
                 dyb = nhwc_zeros(N, Kp, P, Q, device=dev)
                 dyb[:, :K].copy_(dy)
-        direct = _direct_grad(w) and (not has_bias or _direct_grad(ctx.bias_ref))
-        if direct:
-            dw_view, dw = None, w.grad.permute(0, 2, 3, 1)
-        else:
-            dw_view, dw = _new_wgrad(w)
-        conv_wgrad(x, dyb[:, :K], K, R, stride, pad, dil, dw)
-        db = None
-        if has_bias:
-            db = ctx.bias_ref.grad if direct else torch.zeros((K,), dtype=torch.float32, device=dev)
-            call("tsb_bias_grad", ptr(dyb), Kp, N * P * Q, K, ptr(db), *det_ws(), stream())
-            if direct:
-                db = None
+        grads = _ParamGrads(w, ctx.bias_ref)
+        conv_wgrad(x, dyb[:, :K], K, R, stride, pad, dil, grads.buffer(w, krsc=True))
+        _bias_grad(grads, ctx.bias_ref, dyb, Kp, N * P * Q, K)
         dx = None
         if ctx.needs_input_grad[0]:
             _, wt = pack_cache.get(w, True, pad_k=Kp)
             dx = conv_dgrad(dyb, wt, x.shape, Kp, R, stride, pad, dil)
-        if direct:
-            _notify(*([w, ctx.bias_ref] if has_bias else [w]))
-        return dx, dw_view, db, None, None, None, None, None
+        return (dx,) + grads.result() + (None,) * 5
 
 
 class ConvTransposeFn(torch.autograd.Function):
@@ -827,41 +833,29 @@ class ConvTransposeFn(torch.autograd.Function):
         y = conv_transpose_fprop(x, wt, Co, R, stride, pad, dil, out_pad, bias=bias, relu=relu)
         ctx.save_for_backward(x, w, y if relu else None)
         ctx.bias_ref = bias
-        ctx.cfg = (stride, pad, dil, relu, bias is not None)
+        ctx.cfg = (stride, pad, dil, relu)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, w, y = ctx.saved_tensors
-        stride, pad, dil, relu, has_bias = ctx.cfg
+        stride, pad, dil, relu = ctx.cfg
         Ci, Co, R, _ = w.shape
         N, _, P, Q = dy.shape
         dev = dy.device
-        if dy.dtype != _BF or dy.stride(1) != 1:
-            dy = to_nhwc(dy)
+        dy = as_nhwc_bf16(dy)
         if relu:
             dz = nhwc_empty(N, Co, P, Q, device=dev)
             call("tsb_relu_bwd", ptr(dy), cs_of(dy), ptr(y), cs_of(y), ptr(dz), Co, N * P * Q, Co, stream())
             dy = dz
-        direct = _direct_grad(w) and (not has_bias or _direct_grad(ctx.bias_ref))
-        if direct:
-            dw_view, dw = None, w.grad.permute(0, 2, 3, 1)
-        else:
-            dw_view, dw = _new_wgrad(w)
-        conv_wgrad(dy, x, Ci, R, stride, pad, dil, dw)
-        db = None
-        if has_bias:
-            db = ctx.bias_ref.grad if direct else torch.zeros((Co,), dtype=torch.float32, device=dev)
-            call("tsb_bias_grad", ptr(dy), cs_of(dy), N * P * Q, Co, ptr(db), *det_ws(), stream())
-            if direct:
-                db = None
+        grads = _ParamGrads(w, ctx.bias_ref)
+        conv_wgrad(dy, x, Ci, R, stride, pad, dil, grads.buffer(w, krsc=True))
+        _bias_grad(grads, ctx.bias_ref, dy, cs_of(dy), N * P * Q, Co)
         dx = None
         if ctx.needs_input_grad[0]:
             wb, _ = pack_cache.get(w, False)
             dx = conv_fprop(dy, wb, Ci, R, stride, pad, dil)
-        if direct:
-            _notify(*([w, ctx.bias_ref] if has_bias else [w]))
-        return dx, dw_view, db, None, None, None, None, None
+        return (dx,) + grads.result() + (None,) * 5
 
 
 class DWConvFn(torch.autograd.Function):
@@ -892,35 +886,24 @@ class DWConvFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x, w = ctx.saved_tensors
-        stride, share, dil = ctx.stride, ctx.share, ctx.dil
+        stride, dil = ctx.stride, ctx.dil
         C = w.shape[0]
         N, Cx, H, W = x.shape
-        if dy.dtype != _BF or dy.stride(1) != 1:
-            dy = to_nhwc(dy)
+        dy = as_nhwc_bf16(dy)
         w9 = w.detach().reshape(C, 9)
-        direct = _direct_grad(w)
-        if direct:
-            dw_view, dw = None, w.grad
-        else:
-            dw_view = dw = torch.zeros_like(w, memory_format=torch.contiguous_format)
-        call("tsb_dwconv2d_wgrad", ptr(x), cs_of(x), ptr(dy), cs_of(dy), ptr(dw), N, H, W, C, stride, dil, *det_ws(),
-             stream())
+        grads = _ParamGrads(w)
+        call("tsb_dwconv2d_wgrad", ptr(x), cs_of(x), ptr(dy), cs_of(dy), ptr(grads.buffer(w)), N, H, W, C, stride, dil,
+             *det_ws(), stream())
         dx = None
         if ctx.needs_input_grad[0]:
-            if share is not None and share.stash is not None:
-                dx = share.stash
-                call("tsb_dwconv2d_dgrad", ptr(dy), cs_of(dy), ptr(w9), ptr(dx), cs_of(dx), N, H, W, C, stride, dil, 1,
-                     stream())
-                dx = share.contribute(dx, accumulated=True)
-            else:
-                dx = (nhwc_zeros if Cx > C else nhwc_empty)(N, Cx, H, W, device=dy.device)
-                call("tsb_dwconv2d_dgrad", ptr(dy), cs_of(dy), ptr(w9), ptr(dx), cs_of(dx), N, H, W, C, stride, dil, 0,
-                     stream())
-                if share is not None:
-                    dx = share.contribute(dx)
-        if direct:
-            _notify(w)
-        return dx, dw_view, None, None, None, None
+            def dgrad(out, accumulate):
+                if out is None:
+                    out = (nhwc_zeros if Cx > C else nhwc_empty)(N, Cx, H, W, device=dy.device)
+                call("tsb_dwconv2d_dgrad", ptr(dy), cs_of(dy), ptr(w9), ptr(out), cs_of(out), N, H, W, C, stride, dil,
+                     int(accumulate), stream())
+                return out
+            dx = _dgrad_into(ctx.share, dgrad)
+        return (dx,) + grads.result() + (None,) * 4
 
 
 class BNFn(torch.autograd.Function):
@@ -949,12 +932,10 @@ class BNFn(torch.autograd.Function):
         x, gamma, aux = ctx.saved_tensors
         assert ctx.training, "backward through eval-mode BN is not supported"
         beta = ctx.beta_ref
-        direct = _direct_grad(gamma) and _direct_grad(beta)
+        grads = _ParamGrads(gamma, beta)
         # without a residual the ReLU mask is recomputed from x, scale and shift (no read of y)
-        dx, _, dgamma, dbeta = _bn_backward(dy, None, x, aux, gamma, beta, ctx.count, ctx.relu, False, direct)
-        if direct:
-            _notify(gamma, beta)
-        return dx, dgamma, dbeta, None, None, None, None, None, None
+        dx, _ = _bn_backward(dy, None, x, aux, gamma, beta, ctx.count, ctx.relu, False, grads)
+        return (dx,) + grads.result() + (None,) * 6
 
 
 # --------------------------------------------------------------------------------------------------
@@ -1003,18 +984,12 @@ class EncodingFn(torch.autograd.Function):
         K = codewords.shape[0]
         if dE.dtype != _BF or dE.stride(1) != 1 or cs_of(dE) != K:
             dE = to_nhwc(dE)
-        direct = _direct_grad(codewords) and _direct_grad(scale)
-        if direct:
-            dc, ds = codewords.grad, scale.grad
-        else:
-            dc, ds = torch.zeros_like(codewords), torch.zeros_like(scale)
+        grads = _ParamGrads(codewords, scale)
+        dc, ds = grads.buffer(codewords), grads.buffer(scale)
         dx = nhwc_empty(B, D, H, W, device=x.device)
         call("tsb_encoding_bwd", ptr(dE), ptr(x), cs_of(x), B, H * W, D, ptr(codewords), ptr(scale), K, ptr(a), ptr(d2),
              ptr(sum_a), ptr(dx), D, ptr(dc), ptr(ds), *det_ws(), stream())
-        if direct:
-            _notify(codewords, scale)
-            return dx, None, None
-        return dx, dc, ds
+        return (dx,) + grads.result()
 
 
 class ChanMeanFn(torch.autograd.Function):
@@ -1087,8 +1062,7 @@ class MaxPool3x3S2Fn(torch.autograd.Function):
     def backward(ctx, dy):
         (idx,) = ctx.saved_tensors
         N, C, H, W = ctx.shape
-        if dy.dtype != _BF or dy.stride(1) != 1:
-            dy = to_nhwc(dy)
+        dy = as_nhwc_bf16(dy)
         dx = nhwc_empty(N, C, H, W, device=dy.device)
         call("tsb_maxpool3x3s2_bwd", ptr(idx), ptr(dy), cs_of(dy), ptr(dx), C, N, C, H, W, stream())
         return dx
@@ -1147,8 +1121,7 @@ class BilinearFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         N, C, Hi, Wi, Ho, Wo = ctx.shape
-        if dy.dtype != _BF or dy.stride(1) != 1:
-            dy = to_nhwc(dy)
+        dy = as_nhwc_bf16(dy)
         dx = nhwc_empty(N, C, Hi, Wi, device=dy.device)
         if Hi == 1 and Wi == 1:
             # broadcast forward (1x1 → HxW, bisenet network.py:82-84) ⇒ the backward is a plain spatial sum: reuse the
@@ -1159,6 +1132,33 @@ class BilinearFn(torch.autograd.Function):
         else:
             call("tsb_bilinear_bwd", ptr(dy), BF16, cs_of(dy), ptr(dx), BF16, C, N, C, Hi, Wi, Ho, Wo, 0, stream())
         return dx, None, None
+
+
+class UpsampleLogitsFn(torch.autograd.Function):
+    """reference-boundary form of the head tail: NCHW fp32 [N,C,H,W] logits, bilinear align_corners=True to an explicit
+    output size (bisenet network.py:164-166 use scale_factor; with align_corners the source coordinate is
+    (in-1)/(out-1)·dst either way, so size = in·scale is the same op — and sizes like 713 / 473 that are not a multiple
+    of 8 work too)"""
+
+    @staticmethod
+    def forward(ctx, lo, H, W):
+        N, C, h, w = lo.shape
+        H, W = int(H), int(W)
+        out = torch.empty((N, C, H, W), dtype=torch.float32, device=lo.device)
+        call("tsb_bilinear_fwd_nhwc_to_nchw", ptr(lo), _lib.dt(lo), cs_of(lo), ptr(out), N, C, h, w, H, W, stream())
+        ctx.shape = (N, C, h, w, H, W, cs_of(lo))
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        N, C, h, w, H, W, cs = ctx.shape
+        # gather-form transpose needs NHWC with C % 8 == 0: pad the class dimension into a 32-wide buffer
+        Cp = (C + 7) // 8 * 8
+        gp = nhwc_zeros(N, Cp, H, W, dtype=torch.float32, device=g.device)
+        gp[:, :C].copy_(g)
+        d = nhwc_zeros(N, Cp, h, w, dtype=torch.float32, device=g.device, cs=max(cs, Cp))
+        call("tsb_bilinear_bwd", ptr(gp), F32, Cp, ptr(d), F32, cs_of(d), N, Cp, h, w, H, W, 0, stream())
+        return d[:, :C], None, None
 
 
 class ChanScaleFn(torch.autograd.Function):
@@ -1182,8 +1182,7 @@ class ChanScaleFn(torch.autograd.Function):
         x, a32 = ctx.saved_tensors
         base, has_add = ctx.cfg
         N, C, H, W = x.shape
-        if dy.dtype != _BF or dy.stride(1) != 1:
-            dy = to_nhwc(dy)
+        dy = as_nhwc_bf16(dy)
         dx = nhwc_empty(N, C, H, W, device=x.device)
         da32 = torch.zeros((N, C), dtype=torch.float32, device=x.device)
         call("tsb_chan_scale_bwd", ptr(dy), cs_of(dy), ptr(x), cs_of(x), ptr(a32), float(base), ptr(dx), C, ptr(da32), N,
@@ -1213,8 +1212,7 @@ class ConcatFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy):
-        if dy.dtype != _BF or dy.stride(1) != 1:
-            dy = to_nhwc(dy)
+        dy = as_nhwc_bf16(dy)
         outs, off = [], 0
         for c in ctx.chans:
             outs.append(dy[:, off:off + c])
@@ -1271,8 +1269,7 @@ class PSABmmFn(torch.autograd.Function):
         Lp = S.shape[1]
         L = h * w
         dev = x.device
-        if dout.dtype != _BF or dout.stride(1) != 1:
-            dout = to_nhwc(dout)
+        dout = as_nhwc_bf16(dout)
         dS = nhwc_empty(b, L, h, w, device=dev, cs=Lp)
         dx = nhwc_empty(b, c, h, w, device=dev)
         dxt = torch.empty((c, Lp), dtype=torch.float32, device=dev)

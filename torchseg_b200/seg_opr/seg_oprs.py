@@ -72,6 +72,39 @@ def _ragged(conv, x):
     return conv.in_channels != x.shape[1] or conv.in_channels % 64 != 0
 
 
+def _pad_layer(x, w, Cp, Kp, b=None, transposed=False):
+    """a layer's operands in the 64-padded channel domain: x with Cp channels (its first C, the weight's input channels,
+    copied into zero pads unless it has Cp already), the weight [K][C] ([C][K] when transposed) zero-padded to Kp output
+    and Cp input channels, the bias (None stays None) to Kp"""
+    C = w.shape[0] if transposed else w.shape[1]
+    if x.shape[1] != Cp:
+        x = _pad_act(x[:, :C], Cp)
+    w = _pad_weight(w, Cp, Kp) if transposed else _pad_weight(w, Kp, Cp)
+    return x, w, (None if b is None else _pad_vec(b, Kp))
+
+
+def _bn_momentum(bn):
+    return float(bn.momentum if bn.momentum is not None else 0.1)
+
+
+def _conv_bn_act_fn(x, w, bn, Kp, residual, stride, pad, dil, relu, stem=False, in_share=None, res_share=None,
+                    out_pad=None):
+    """ops.ConvBNActFn with bn's γ, β and running statistics padded to the Kp output channels of w (γ and the running
+    variance with ones, β and the running mean with zeros). A training forward updates the padded running statistics;
+    they are copied back into bn."""
+    gamma, beta = _pad_vec(bn.weight, Kp, 1.0), _pad_vec(bn.bias, Kp)
+    with torch.no_grad():
+        rm, rv = _pad_vec(bn.running_mean, Kp), _pad_vec(bn.running_var, Kp, 1.0)
+    y = ops.ConvBNActFn.apply(x, w, gamma, beta, residual, rm, rv, stride, pad, dil, bool(relu), float(bn.eps),
+                              _bn_momentum(bn), bool(bn.training), stem, in_share, res_share, out_pad)
+    if bn.training and rm is not bn.running_mean:
+        with torch.no_grad():
+            K = bn.running_mean.shape[0]
+            bn.running_mean.copy_(rm[:K])
+            bn.running_var.copy_(rv[:K])
+    return y
+
+
 EVAL_FOLD_BN = True   # eval mode: fold the BatchNorm into the conv weights, bias (+ residual) + ReLU in the conv epilogue
 
 
@@ -88,18 +121,12 @@ def conv_bn_act(x, conv, bn, relu, residual=None, in_share=None, res_share=None)
         xin = _as_act(x)
     if residual is not None:
         residual = _as_act(residual)
-    momentum = bn.momentum if bn.momentum is not None else 0.1
-    w, gamma, beta, rm, rv = conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var
-    K = conv.out_channels
+    w = conv.weight
+    K = Kp = conv.out_channels
     padded = (not stem) and (_ragged(conv, xin) or K % 64 != 0)
     if padded:
-        Cp, Kp = _ceil_to(xin.shape[1], 64), _ceil_to(K, 64)
-        if xin.shape[1] != Cp:
-            xin = _pad_act(xin, Cp)
-        w = _pad_weight(w, Kp, Cp)
-        gamma, beta = _pad_vec(gamma, Kp, 1.0), _pad_vec(beta, Kp)
-        with torch.no_grad():
-            rm, rv = _pad_vec(rm, Kp), _pad_vec(rv, Kp, 1.0)
+        Kp = _ceil_to(K, 64)
+        xin, w, _ = _pad_layer(xin, w, _ceil_to(xin.shape[1], 64), Kp)
     if stem or not bn.training:
         in_share = res_share = None
     elif padded:
@@ -115,14 +142,8 @@ def conv_bn_act(x, conv, bn, relu, residual=None, in_share=None, res_share=None)
             return ops.conv_stem_fprop_fused(xin, wb, K, bias, relu=bool(relu))
         return ops.conv_fprop_fused(xin, wb, K, ks, conv.stride[0], conv.padding[0], conv.dilation[0], bias,
                                     res=residual, relu=bool(relu))
-    y = ops.ConvBNActFn.apply(xin, w, gamma, beta, residual, rm, rv,
-                              conv.stride[0], conv.padding[0], conv.dilation[0], bool(relu), float(bn.eps),
-                              float(momentum), bool(bn.training), stem, in_share, res_share)
-    if padded and bn.training and rm is not bn.running_mean:
-        with torch.no_grad():
-            bn.running_mean.copy_(rm[:K])
-            bn.running_var.copy_(rv[:K])
-    return y
+    return _conv_bn_act_fn(xin, w, bn, Kp, residual, conv.stride[0], conv.padding[0], conv.dilation[0], relu, stem,
+                           in_share, res_share)
 
 
 def conv_plain(x, conv, out_f32=False, ocs=None, pad_out=False):
@@ -132,13 +153,7 @@ def conv_plain(x, conv, out_f32=False, ocs=None, pad_out=False):
     w, b = conv.weight, conv.bias
     K = conv.out_channels
     if _ragged(conv, xin) or (pad_out and K % 64 != 0):
-        Cp = _ceil_to(xin.shape[1], 64)
-        Kp = _ceil_to(K, 64) if pad_out else K
-        if xin.shape[1] != Cp:
-            xin = _pad_act(xin, Cp)
-        w = _pad_weight(w, Kp, Cp)
-        if b is not None:
-            b = _pad_vec(b, Kp)
+        xin, w, b = _pad_layer(xin, w, _ceil_to(xin.shape[1], 64), _ceil_to(K, 64) if pad_out else K, b)
     return ops.ConvFn.apply(xin, w, b, conv.stride[0], conv.padding[0], conv.dilation[0], bool(out_f32), ocs)
 
 
@@ -197,32 +212,17 @@ def deconv_bn_act(x, conv, bn, relu):
     Cp, Kp = _ceil_to(Ci, 64), _ceil_to(Co, 64)
     padded = Cp != Ci or Kp != Co or xin.shape[1] != Ci
     if padded:
-        if xin.shape[1] != Cp:
-            xin = _pad_act(xin[:, :Ci], Cp)
-        w = _pad_weight(w, Cp, Kp)   # [Ci][Co] → [Cp][Kp]: the same zero-padding of both leading dims
+        xin, w, b = _pad_layer(xin, w, Cp, Kp, b, transposed=True)
     if bn is None:
-        if b is not None and padded:
-            b = _pad_vec(b, Kp)
         y = ops.ConvTransposeFn.apply(xin, w, b, stride, pad, dil, op, bool(relu))
-        return y[:, :Co] if Kp != Co else y
-    if b is not None:
+    elif b is not None:
         raise NotImplementedError("DeConvBnRelu with both bias and BN is not on the accelerated path")
-    momentum = bn.momentum if bn.momentum is not None else 0.1
-    gamma, beta, rm, rv = bn.weight, bn.bias, bn.running_mean, bn.running_var
-    if (not bn.training) and EVAL_FOLD_BN and not padded and not torch.is_grad_enabled():
+    elif (not bn.training) and EVAL_FOLD_BN and not padded and not torch.is_grad_enabled():
         # inference: W' = W·γ/σ along Co, b' = β − μ·γ/σ, epilogue = + b' → ReLU
         wt, bias = ops.fold_cache.get(conv.weight, bn, False, transposed=True)
         return ops.conv_transpose_fprop(xin, wt, Co, k, stride, pad, dil, op, bias=bias, relu=bool(relu))
-    if padded:
-        gamma, beta = _pad_vec(gamma, Kp, 1.0), _pad_vec(beta, Kp)
-        with torch.no_grad():
-            rm, rv = _pad_vec(rm, Kp), _pad_vec(rv, Kp, 1.0)
-    y = ops.ConvBNActFn.apply(xin, w, gamma, beta, None, rm, rv, stride, pad, dil, bool(relu), float(bn.eps),
-                              float(momentum), bool(bn.training), False, None, None, op)
-    if padded and bn.training and rm is not bn.running_mean:
-        with torch.no_grad():
-            bn.running_mean.copy_(rm[:Co])
-            bn.running_var.copy_(rv[:Co])
+    else:
+        y = _conv_bn_act_fn(xin, w, bn, Kp, None, stride, pad, dil, relu, out_pad=op)
     return y[:, :Co] if Kp != Co else y
 
 
@@ -283,8 +283,7 @@ class SeparableConvBnRelu(nn.Module):
         stride, dil = self._geometry()
         bn, pw = self.bn, self.point_wise_cbr
         t = ops.DWConvFn.apply(_as_act(x), self.conv1.weight, stride, None, None, dil)
-        momentum = bn.momentum if bn.momentum is not None else 0.1
-        t = ops.BNFn.apply(t, bn.weight, bn.bias, bn.running_mean, bn.running_var, float(bn.eps), float(momentum),
+        t = ops.BNFn.apply(t, bn.weight, bn.bias, bn.running_mean, bn.running_var, float(bn.eps), _bn_momentum(bn),
                            bool(bn.training))
         return conv_bn_act(t, pw.conv, pw.bn, pw.has_relu)
 
@@ -395,8 +394,7 @@ class AddReluFn(torch.autograd.Function):
     def backward(ctx, dy):
         (y,) = ctx.saved_tensors
         N, C, H, W = y.shape
-        if dy.dtype != torch.bfloat16 or dy.stride(1) != 1:
-            dy = ops.to_nhwc(dy)
+        dy = ops.as_nhwc_bf16(dy)
         dx = ops.nhwc_empty(N, C, H, W, device=y.device)
         ops.call("tsb_relu_bwd", ops.ptr(dy), ops.cs_of(dy), ops.ptr(y), C, ops.ptr(dx), C, N * H * W, C, ops.stream())
         return dx, dx
