@@ -173,6 +173,10 @@ int tsb_bn_bwd_apply(const void* dy, int dycs, const void* y, int ycs, const voi
                      double count, int relu, void* dx, int dxcs, void* dres, int drcs, long long npix, int C,
                      float* dgamma_acc, float* dbeta_acc, const float* scale, const float* shift,
                      tsb_stream_t stream);
+/* out/argmax = tsb_maxpool3x3s2_fwd of tsb_bn_apply(x, scale, shift, no residual, relu = 1), bit for bit and in the
+ * same layouts, in one pass that never writes the normalised map (the context stem of BiSeNet-R18). */
+int tsb_bn_apply_maxpool3x3s2(const void* x, int xcs, const float* scale, const float* shift, void* out, int ocs,
+                              void* argmax, int N, int C, int H, int W, tsb_stream_t stream);
 
 /* ================================================================================================
  * Channel-attention fusions — AttentionRefinement.forward seg_oprs.py:207-212 (fm*sigmoid(se) and the

@@ -47,6 +47,7 @@ _SIGS = {
     "tsb_bn_apply": [P, I, P, P, P, I, I, P, I, L, I, P],
     "tsb_bn_bwd_reduce": [P, I, P, I, P, I, P, P, I, L, I, P, P, P, P, P, L, P],
     "tsb_bn_bwd_apply": [P, I, P, I, P, I, P, P, P, P, P, D, I, P, I, P, I, L, I, P, P, P, P, P],
+    "tsb_bn_apply_maxpool3x3s2": [P, I, P, P, P, I, P, I, I, I, I, P],
     "tsb_chan_scale_fwd": [P, I, P, F, P, I, P, I, I, I, I, P],
     "tsb_chan_scale_bwd": [P, I, P, I, P, F, P, I, P, I, I, I, P, L, P],
     "tsb_pack_image_s2d": [P, I, I, I, P, P],

@@ -130,10 +130,12 @@ class ResNet(nn.Module):
             return self.forward_from_stem(conv_bn_act(x, c[6], self.bn1, True))
         return self.forward_from_stem(conv_bn_act(x, self.conv1, self.bn1, True))
 
-    def forward_from_stem(self, x):
-        """stages after conv1 → bn1 → relu (the stem may be computed elsewhere, fused with a sibling stem)"""
+    def forward_from_stem(self, x, pooled=False):
+        """stages after conv1 → bn1 → relu (the stem may be computed elsewhere, fused with a sibling stem); pooled: x is
+        already past the max pool (ops.StemPairFn pools the context stem itself)"""
         _release_packed_image()   # every stem of this forward has consumed the space-to-depth image by now
-        x = ops.MaxPool3x3S2Fn.apply(x)
+        if not pooled:
+            x = ops.MaxPool3x3S2Fn.apply(x)
         blocks = []
         x = self.layer1(x)
         blocks.append(x)

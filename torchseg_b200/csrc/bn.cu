@@ -136,18 +136,9 @@ bn_apply_kernel(const __nv_bfloat16* __restrict__ x, int xcs, const float* __res
                 ldg8f(scale + c8s[u] * 8, sc);
                 ldg8f(shift + c8s[u] * 8, sh);
             }
-#pragma unroll
-            for (int k = 0; k < 8; ++k) v[k] = fmaf(v[k], sc[k], sh[k]);
-            if (kRes) {
-                float r[8];
-                unpack8(rq[u], r);
-#pragma unroll
-                for (int k = 0; k < 8; ++k) v[k] += r[k];
-            }
-            if (kRelu) {
-#pragma unroll
-                for (int k = 0; k < 8; ++k) v[k] = fmaxf(v[k], 0.f);
-            }
+            float r[8];
+            if (kRes) unpack8(rq[u], r);
+            bn_act8<kRelu, kRes>(v, sc, sh, r);
             if (ok[u]) Vec8<__nv_bfloat16>::store(y + off_y[u], v);
         }
     }

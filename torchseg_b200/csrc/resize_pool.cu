@@ -249,42 +249,76 @@ adaptive_avgpool_bwd_kernel(const float* __restrict__ dout, int N, int C8, int H
 }
 
 // ---------------------------------------------------------------- max pool 3x3 stride 2 pad 1
-// forward also records the arg-max window position r*3+s (first maximum in scan order, strict '>' — ATen
-// max_pool2d semantics) as one byte per output element, so the backward is a pure gather.
+// One 8-channel output vector (n, p, q, c8) of the pool over the H x W input that load(pixel, c8, v) reads. Records the
+// arg-max window position r*3+s (first maximum in scan order, strict '>' — ATen max_pool2d semantics) as one byte per
+// output element, so the backward is a pure gather.
+template <typename Load>
+__device__ __forceinline__ void maxpool3x3s2_vec(const Load& load, __nv_bfloat16* __restrict__ out, int ocs,
+                                                 uint8_t* __restrict__ idx, long long pix, int c8, int C8, int H,
+                                                 int W, int P, int Q) {
+    int q, p, n;
+    split_pix(pix, Q, P, q, p, n);
+    float m[8];
+    uint32_t am[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { m[k] = -INFINITY; am[k] = 0; }
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        int h = 2 * p - 1 + r;
+        if (h < 0 || h >= H) continue;
+#pragma unroll
+        for (int s = 0; s < 3; ++s) {
+            int w = 2 * q - 1 + s;
+            if (w < 0 || w >= W) continue;
+            float v[8];
+            load(((long long)n * H + h) * W + w, c8, v);
+#pragma unroll
+            for (int k = 0; k < 8; ++k)
+                if (v[k] > m[k]) { m[k] = v[k]; am[k] = r * 3 + s; }
+        }
+    }
+    Vec8<__nv_bfloat16>::store(out + pix * ocs + c8 * 8, m);
+    if (idx) {
+        uint2 pk;
+        pk.x = am[0] | (am[1] << 8) | (am[2] << 16) | (am[3] << 24);
+        pk.y = am[4] | (am[5] << 8) | (am[6] << 16) | (am[7] << 24);
+        *reinterpret_cast<uint2*>(idx + pix * (long long)(C8 * 8) + c8 * 8) = pk;
+    }
+}
+
 __global__ void __launch_bounds__(kThreads)
 maxpool_fwd_kernel(const __nv_bfloat16* __restrict__ in, int ics, __nv_bfloat16* __restrict__ out, int ocs,
                    uint8_t* __restrict__ idx, int N, int C8, int H, int W, int P, int Q) {
     const long long total = (long long)N * P * Q * C8;
-    for_each_vec(total, C8, [&](long long pix, int c8) {
-        int q, p, n;
-        split_pix(pix, Q, P, q, p, n);
-        float m[8];
-        uint32_t am[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) { m[k] = -INFINITY; am[k] = 0; }
-#pragma unroll
-        for (int r = 0; r < 3; ++r) {
-            int h = 2 * p - 1 + r;
-            if (h < 0 || h >= H) continue;
-#pragma unroll
-            for (int s = 0; s < 3; ++s) {
-                int w = 2 * q - 1 + s;
-                if (w < 0 || w >= W) continue;
-                float v[8];
-                Vec8<__nv_bfloat16>::load(in + (((long long)n * H + h) * W + w) * ics + c8 * 8, v);
-#pragma unroll
-                for (int k = 0; k < 8; ++k)
-                    if (v[k] > m[k]) { m[k] = v[k]; am[k] = r * 3 + s; }
-            }
+    auto load = [&](long long pix, int c8, float (&v)[8]) { Vec8<__nv_bfloat16>::load(in + pix * ics + c8 * 8, v); };
+    for_each_vec(total, C8, [&](long long pix, int c8) { maxpool3x3s2_vec(load, out, ocs, idx, pix, c8, C8, H, W, P, Q); });
+}
+
+// The pool of act(x·scale + shift) with act = ReLU, normalised on the fly (the normalised map is never written). Each
+// vector is rounded to bf16 before the comparison, as tsb_bn_apply stores it, so the pooled map and the argmax are bit
+// for bit those of tsb_bn_apply followed by tsb_maxpool3x3s2_fwd.
+__global__ void __launch_bounds__(kThreads)
+bn_relu_maxpool_fwd_kernel(const __nv_bfloat16* __restrict__ x, int xcs, const float* __restrict__ scale,
+                           const float* __restrict__ shift, __nv_bfloat16* __restrict__ out, int ocs,
+                           uint8_t* __restrict__ idx, int N, int C8, int H, int W, int P, int Q) {
+    const long long total = (long long)N * P * Q * C8;
+    // the walk keeps one channel group per thread when C8 divides kThreads (bn_apply_kernel): parameters loaded once
+    const bool hoist = (kThreads % C8) == 0;
+    float sc[8], sh[8];
+    if (hoist) {
+        ldg8f(scale + (threadIdx.x % C8) * 8, sc);
+        ldg8f(shift + (threadIdx.x % C8) * 8, sh);
+    }
+    auto load = [&](long long pix, int c8, float (&v)[8]) {
+        unpack8(*reinterpret_cast<const uint4*>(x + pix * xcs + c8 * 8), v);
+        if (!hoist) {
+            ldg8f(scale + c8 * 8, sc);
+            ldg8f(shift + c8 * 8, sh);
         }
-        Vec8<__nv_bfloat16>::store(out + pix * ocs + c8 * 8, m);
-        if (idx) {
-            uint2 pk;
-            pk.x = am[0] | (am[1] << 8) | (am[2] << 16) | (am[3] << 24);
-            pk.y = am[4] | (am[5] << 8) | (am[6] << 16) | (am[7] << 24);
-            *reinterpret_cast<uint2*>(idx + pix * (long long)(C8 * 8) + c8 * 8) = pk;
-        }
-    });
+        bn_act8<true, false>(v, sc, sh, nullptr);
+        unpack8(pack8(v), v);
+    };
+    for_each_vec(total, C8, [&](long long pix, int c8) { maxpool3x3s2_vec(load, out, ocs, idx, pix, c8, C8, H, W, P, Q); });
 }
 
 // backward, gather form. One thread owns a 2x2 block of input pixels (h = 2a+dh, w = 2b+dw) x 8 channels: the
@@ -468,6 +502,20 @@ extern "C" int tsb_maxpool3x3s2_fwd(const void* in, int ics, void* out, int ocs,
     int grid = tsb_grid_for(total, kThreads, 8);
     maxpool_fwd_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)in, ics, (__nv_bfloat16*)out, ocs, (uint8_t*)argmax, N, C / 8, H, W, P, Q);
     TSB_CUDA_CHECK_LAUNCH("maxpool_fwd");
+    return TSB_OK;
+}
+
+extern "C" int tsb_bn_apply_maxpool3x3s2(const void* x, int xcs, const float* scale, const float* shift, void* out,
+                                         int ocs, void* argmax, int N, int C, int H, int W, tsb_stream_t stream) {
+    TSB_REQUIRE(x && scale && shift && out && argmax && N > 0 && H > 0 && W > 0, "tsb_bn_apply_maxpool3x3s2: bad args");
+    TSB_REQUIRE(TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, ocs, out) && tsb_aligned8(argmax),
+                "tsb_bn_apply_maxpool3x3s2: C, strides must be multiples of 8, strides >= C, x/out 16B and argmax 8B aligned");
+    TSB_REQUIRE(tsb_aligned16(scale) && tsb_aligned16(shift), "tsb_bn_apply_maxpool3x3s2: scale and shift must be 16B aligned");
+    const int P = (H + 2 - 3) / 2 + 1, Q = (W + 2 - 3) / 2 + 1;
+    long long total = (long long)N * P * Q * (C / 8);
+    int grid = tsb_grid_for(total, kThreads, 8);
+    bn_relu_maxpool_fwd_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, xcs, scale, shift, (__nv_bfloat16*)out, ocs, (uint8_t*)argmax, N, C / 8, H, W, P, Q);
+    TSB_CUDA_CHECK_LAUNCH("bn_relu_maxpool_fwd");
     return TSB_OK;
 }
 

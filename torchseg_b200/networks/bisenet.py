@@ -80,12 +80,12 @@ class BiSeNetBody(nn.Module):
         if (data.shape[1] == 3 and isinstance(getattr(cp, "conv1", None), nn.Conv2d) and sp.conv_7x7.bn.training
                 and cp.bn1.training):
             bs, bc = sp.conv_7x7.bn, cp.bn1
-            s_stem, c_stem = ops.StemPairFn.apply(
+            s_stem, c_pooled = ops.StemPairFn.apply(
                 _packed_image(data), sp.conv_7x7.conv.weight, bs.weight, bs.bias, bs.running_mean, bs.running_var,
                 cp.conv1.weight, bc.weight, bc.bias, bc.running_mean, bc.running_var,
                 float(bs.eps), _bn_momentum(bs), float(bc.eps), _bn_momentum(bc))
             spatial_out = sp.forward_from_stem(s_stem)
-            context_blocks = cp.forward_from_stem(c_stem)
+            context_blocks = cp.forward_from_stem(c_pooled, pooled=True)
         else:
             spatial_out = sp(data)
             context_blocks = cp(data)

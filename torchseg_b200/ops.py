@@ -568,11 +568,11 @@ def _bn_finalize(aux, stats, count, gamma, beta, running_mean, running_var, eps,
 
 
 def _bn_apply(raw, aux, residual, relu):
-    """y = act(raw * scale + shift + residual) over the dense NHWC raw [N,K,P,Q]"""
+    """y = act(raw * scale + shift + residual) over the NHWC raw [N,K,P,Q] (possibly a channel slice), into a dense y"""
     N, K, P, Q = raw.shape
     y = nhwc_empty(N, K, P, Q, device=raw.device)
-    call("tsb_bn_apply", ptr(raw), K, ptr(aux[2]), ptr(aux[3]), ptr(residual), cs_of(residual) if residual is not None else 0,
-         int(relu), ptr(y), K, N * P * Q, K, stream())
+    call("tsb_bn_apply", ptr(raw), cs_of(raw), ptr(aux[2]), ptr(aux[3]), ptr(residual),
+         cs_of(residual) if residual is not None else 0, int(relu), ptr(y), K, N * P * Q, K, stream())
     return y
 
 
@@ -715,8 +715,9 @@ class ConvBNActFn(torch.autograd.Function):
 class StemPairFn(torch.autograd.Function):
     """The TWO 7x7/2 stems of BiSeNet (spatial_path.conv_7x7, bisenet network.py:118, and context_path.conv1,
     resnet.py:126) read the same image: one conv launch computes both (K = 64 + 64 output channels, N = 128 MMA
-    tiles), one BN-apply pass normalises both, one wgrad launch produces both weight gradients. Returns the two
-    64-channel halves as channel-slice views of one NHWC buffer."""
+    tiles), one wgrad launch produces both weight gradients. Returns the spatial stem's output and the context stem's
+    output after the context path's 3x3/2 max pool (resnet.py:132): that half is normalised, ReLU'd and pooled in one
+    pass (tsb_bn_apply_maxpool3x3s2), so its full-resolution output is never stored."""
 
     @staticmethod
     def forward(ctx, xs, w1, g1, b1, rm1, rv1, w2, g2, b2, rm2, rv2, eps1, mom1, eps2, mom2):
@@ -741,19 +742,28 @@ class StemPairFn(torch.autograd.Function):
         for (h, g, b, rm, rv, eps, mom) in ((slice(0, K1), g1, b1, rm1, rv1, eps1, mom1),
                                             (slice(K1, K), g2, b2, rm2, rv2, eps2, mom2)):
             _bn_finalize(aux[:, h], stats[:, h], count, g, b, rm, rv, eps, mom, True)
-        y = _bn_apply(raw, aux, None, True)
-        ctx.save_for_backward(xs, w1, g1, w2, g2, raw, aux)
+        y = _bn_apply(raw[:, :K1], aux[:, :K1], None, True)
+        P2, Q2 = (P - 1) // 2 + 1, (Q - 1) // 2 + 1
+        pooled = nhwc_empty(N, K2, P2, Q2, device=dev)
+        argmax = torch.empty((N, P2, Q2, K2), dtype=torch.uint8, device=dev)
+        call("tsb_bn_apply_maxpool3x3s2", ptr(raw[:, K1:]), K, ptr(aux[2, K1:]), ptr(aux[3, K1:]), ptr(pooled), K2,
+             ptr(argmax), N, K2, P, Q, stream())
+        ctx.save_for_backward(xs, w1, g1, w2, g2, raw, aux, argmax)
         ctx.refs = (b1, b2)
         ctx.count = count
-        return y[:, :K1], y[:, K1:]
+        return y, pooled
 
     @staticmethod
-    def backward(ctx, dy1, dy2):
-        xs, w1, g1, w2, g2, raw, aux = ctx.saved_tensors
+    def backward(ctx, dy1, dpooled):
+        xs, w1, g1, w2, g2, raw, aux, argmax = ctx.saved_tensors
         b1, b2 = ctx.refs
         N, K, P, Q = raw.shape
         K1 = w1.shape[0]
         dev = raw.device
+        dpooled = as_nhwc_bf16(dpooled)
+        dy2 = nhwc_empty(N, K - K1, P, Q, device=dev)
+        call("tsb_maxpool3x3s2_bwd", ptr(argmax), ptr(dpooled), cs_of(dpooled), ptr(dy2), K - K1, N, K - K1, P, Q,
+             stream())
         draw = nhwc_empty(N, K, P, Q, device=dev)
         halves = []
         for (h, w, g, b, dy) in ((slice(0, K1), w1, g1, b1, dy1), (slice(K1, K), w2, g2, b2, dy2)):
