@@ -368,6 +368,23 @@ int tsb_chan_mean_bwd(const void* dy, long long npix, int C, void* dx, int dxcs,
 int tsb_se_loss_fwd_bwd(const int64_t* labels, int B, long long HW, const float* z, int zs, int C, uint32_t* presence,
                         float* loss, float* dz_unit, int dzs, tsb_stream_t stream);
 
+/* ---- OCNet: fused self-attention over the pixels of each image ------------------------------------------------------
+ *   o[b,i,:] = Σ_j softmax_j(scale · q[b,i,:]·k[b,j,:]) · v[b,j,:]     b < B, i, j < N
+ * q, k, v, o, dout and the gradients are bf16 rows [B·N][d] (row b·N + i) with channel stride *cs: multiples of 8 and
+ * >= d, every pointer 16-byte aligned. Only d_k = d_v = 256 is implemented (anything else is TSB_ERR_UNSUPPORTED);
+ * B·N < 2^31, B <= 65535, 0 < scale < inf. S = q·kᵀ and its softmax are never written to global memory; every output
+ * element has one writer, so results are bit-identical from run to run. */
+/* lse: fp32 [B·N], m_i + log Σ_j exp(scale·s_ij − m_i) per query row (the softmax normaliser), or NULL (inference). */
+int tsb_attention_fwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, void* o, int ocs, float* lse,
+                      int B, int N, int dim_k, int dim_v, float scale, tsb_stream_t stream);
+/* The gradient from the forward's o and lse. delta_ws: fp32 [B·N] scratch (δ_i = Σ_c dout_ic·o_ic). dk and dv are
+ * written; dq is written, or, with dq_accumulate, added to (dq += dQ, rounded once): with dq == dk the shared query/key
+ * gradient dQ + dK comes out of one call, since dK is finished before dQ is added. */
+int tsb_attention_bwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, const void* o, int ocs,
+                      const void* dout, int docs, const float* lse, float* delta_ws, void* dq, int dqcs, void* dk,
+                      int dkcs, void* dv, int dvcs, int dq_accumulate, int B, int N, int dim_k, int dim_v, float scale,
+                      tsb_stream_t stream);
+
 /* ================================================================================================
  * Optimiser — fused flat-buffer momentum SGD replacing torch.optim.SGD.step (train.py:86-89,142) with
  * the group semantics of furnace/utils/init_func.py:34-57 (decay / no-decay, 1x / 10x LR):

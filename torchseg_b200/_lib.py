@@ -94,6 +94,8 @@ _SIGS = {
     "tsb_chan_mean_fwd": [P, I, L, I, P, P],
     "tsb_chan_mean_bwd": [P, L, I, P, I, P],
     "tsb_se_loss_fwd_bwd": [P, I, L, P, I, I, P, P, P, I, P],
+    "tsb_attention_fwd": [P, I, P, I, P, I, P, I, P, I, I, I, I, F, P],
+    "tsb_attention_bwd": [P, I, P, I, P, I, P, I, P, I, P, P, P, I, P, I, P, I, I, I, I, I, I, F, P],
 }
 EXPORTS = sorted(list(_SIGS) + ["tsb_last_error", "tsb_version", "tsb_launch_count", "tsb_p2p_buffer_bytes", "tsb_edge_labels_workspace_bytes"])
 

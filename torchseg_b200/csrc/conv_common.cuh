@@ -61,6 +61,24 @@ static inline int encode_4d(CUtensorMap* m, const void* base, uint64_t d0, uint6
                  (unsigned long long)s1, (unsigned long long)s2, (unsigned long long)s3, b0, b1, b2, b3);
     return TSB_OK;
 }
+// rank-3 bf16 map; strides in BYTES for dims 1..2; zero OOB fill; 128B swizzle
+static inline int encode_3d(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1,
+                            uint64_t s2, uint32_t b0, uint32_t b1, uint32_t b2) {
+    PFN_encodeTiled enc = get_encode();
+    if (!enc) TSB_FAIL(TSB_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+    cuuint64_t dims[3] = {d0, d1, d2};
+    cuuint64_t strides[2] = {s1, s2};
+    cuuint32_t box[3] = {b0, b1, b2};
+    cuuint32_t es[3] = {1, 1, 1};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS)
+        TSB_FAIL(TSB_ERR_CUDA, "cuTensorMapEncodeTiled(3d) failed: %d dims=(%llu,%llu,%llu) strides=(%llu,%llu) box=(%u,%u,%u)",
+                 (int)r, (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, (unsigned long long)s1,
+                 (unsigned long long)s2, b0, b1, b2);
+    return TSB_OK;
+}
 static inline int encode_2d(CUtensorMap* m, const void* base, uint64_t d0, uint64_t d1, uint64_t s1, uint32_t b0, uint32_t b1) {
     PFN_encodeTiled enc = get_encode();
     if (!enc) TSB_FAIL(TSB_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");

@@ -53,6 +53,13 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* map, uin
         "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* map, uint64_t* bar, int c0, int c1, int c2) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
+            smem_u32(smem_dst)),
+        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const void* map, uint64_t* bar, int c0, int c1, int c2,
                                             int c3) {
     asm volatile(
@@ -65,6 +72,9 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const void* map, uin
 // ------------------------------------------------------------------ wgmma (warpgroup MMA)
 // Registers written by ordinary instructions must be fenced before a wgmma reads them as accumulators.
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+// Shared memory written by ordinary stores must be fenced (by every writing thread, before the barrier that orders it)
+// before a wgmma reads it as an operand: wgmma reads through the async proxy.
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }

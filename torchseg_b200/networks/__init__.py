@@ -5,3 +5,4 @@ from .dfn import DFN, DFNHead
 from .psanet import PSANet, PointwiseSpatialAttention
 from .deeplabv3plus import DeepLabV3Plus, ASPP, Decoder
 from .encnet import EncNet, EncModule, EncHead
+from .ocnet import OCNet

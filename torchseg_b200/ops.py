@@ -1052,6 +1052,50 @@ class SELossFn(torch.autograd.Function):
 
 
 # --------------------------------------------------------------------------------------------------
+# OCNet: dense self-attention over the pixels of each image
+# --------------------------------------------------------------------------------------------------
+class AttentionFn(torch.autograd.Function):
+    """o = softmax(scale · q kᵀ) v over the h·w pixels of each image (OCNet's object context), fused on
+    tsb_attention_{fwd,bwd}: the [N, N] scores never reach memory, and the backward recomputes them from the saved
+    q, k, v, o and the per-row log-sum-exp (O(N·d) saved, not O(N²)). q, k, v: bf16 NHWC [B, 256, h, w] (channel slices
+    allowed). k = None means k is q (OCNet's shared f_key): the backward then returns dQ + dK as q's gradient, formed by
+    the kernels in one buffer. Without any input needing a gradient the forward skips the log-sum-exp."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, scale):
+        shared = k is None
+        k = q if shared else k
+        B, dk, h, w = q.shape
+        dv = v.shape[1]
+        assert k.shape == q.shape and v.shape[0] == B and v.shape[2:] == q.shape[2:], "attention: shape mismatch"
+        need = any(ctx.needs_input_grad)
+        o = nhwc_empty(B, dv, h, w, device=q.device)
+        lse = torch.empty((B, h * w), dtype=torch.float32, device=q.device) if need else None
+        call("tsb_attention_fwd", ptr(q), cs_of(q), ptr(k), cs_of(k), ptr(v), cs_of(v), ptr(o), dv, ptr(lse), B, h * w,
+             dk, dv, float(scale), stream())
+        if need:
+            ctx.save_for_backward(q, k, v, o, lse)
+            ctx.cfg = (shared, float(scale))
+        return o
+
+    @staticmethod
+    def backward(ctx, do):
+        q, k, v, o, lse = ctx.saved_tensors
+        shared, scale = ctx.cfg
+        B, dk, h, w = q.shape
+        dv = v.shape[1]
+        do = as_nhwc_bf16(do)
+        dq = nhwc_empty(B, dk, h, w, device=q.device)
+        dkt = dq if shared else nhwc_empty(B, dk, h, w, device=q.device)
+        dvt = nhwc_empty(B, dv, h, w, device=q.device)
+        delta = torch.empty((B, h * w), dtype=torch.float32, device=q.device)
+        call("tsb_attention_bwd", ptr(q), cs_of(q), ptr(k), cs_of(k), ptr(v), cs_of(v), ptr(o), cs_of(o), ptr(do),
+             cs_of(do), ptr(lse), ptr(delta), ptr(dq), dk, ptr(dkt), dk, ptr(dvt), dv, int(shared), B, h * w, dk, dv,
+             scale, stream())
+        return dq, (None if shared else dkt), dvt, None
+
+
+# --------------------------------------------------------------------------------------------------
 # pooling / resize / attention scale
 # --------------------------------------------------------------------------------------------------
 class MaxPool3x3S2Fn(torch.autograd.Function):

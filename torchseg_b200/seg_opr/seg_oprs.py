@@ -313,6 +313,62 @@ class Encoding(nn.Module):
         return ops.encoding_infer(x, self.codewords, self.scale)
 
 
+class SelfAttentionBlock(nn.Module):
+    """OCNet's object-context self-attention (Yuan & Wang, OCNet, `_SelfAttentionBlock` at scale 1): f_key, a 1x1
+    ConvBnRelu, gives both the queries and the keys (one child, so its parameters appear once), f_value a 1x1 conv with
+    bias, and W a 1x1 conv with bias, zero-initialised as in OCNet. forward(x) = W(softmax(k kᵀ / √key_channels) v) with
+    k = f_key(x), v = f_value(x), the attention over the h·w pixels of each image on ops.AttentionFn (key_channels =
+    value_channels = 256). f_key runs once per forward, so its BatchNorm running statistics get one update."""
+
+    def __init__(self, in_channels, key_channels, value_channels, out_channels=None, scale=1,
+                 norm_layer=nn.BatchNorm2d):
+        super(SelfAttentionBlock, self).__init__()
+        if scale > 1:
+            raise NotImplementedError("SelfAttentionBlock: scale > 1 (the pooled variants of OCNet) is not implemented")
+        self.scale = scale
+        self.in_channels = in_channels
+        self.key_channels = key_channels
+        self.value_channels = value_channels
+        self.out_channels = in_channels if out_channels is None else out_channels
+        self.f_key = ConvBnRelu(in_channels, key_channels, 1, 1, 0, has_bn=True, has_relu=True, has_bias=False,
+                                norm_layer=norm_layer)
+        self.f_value = nn.Conv2d(in_channels, value_channels, kernel_size=1)
+        self.W = nn.Conv2d(value_channels, self.out_channels, kernel_size=1)
+        nn.init.constant_(self.W.weight, 0)
+        nn.init.constant_(self.W.bias, 0)
+
+    def forward(self, x):
+        x = _as_act(x)
+        key = self.f_key(x)
+        value = conv_plain(x, self.f_value)
+        context = ops.AttentionFn.apply(key, None, value, self.key_channels ** -0.5)
+        return conv_plain(context, self.W)
+
+
+class BaseOCModule(nn.Module):
+    """OCNet's Base-OC module (`BaseOC_Module`): the sum of the `stages` (SelfAttentionBlock) concatenated in front of
+    the input, then `conv_bn_dropout` = 1x1 ConvBnRelu(2·in → out) and Dropout2d"""
+
+    def __init__(self, in_channels, out_channels, key_channels, value_channels, dropout, sizes=(1,),
+                 norm_layer=nn.BatchNorm2d):
+        super(BaseOCModule, self).__init__()
+        self.stages = nn.ModuleList([SelfAttentionBlock(in_channels, key_channels, value_channels, out_channels, size,
+                                                        norm_layer) for size in sizes])
+        self.conv_bn_dropout = nn.Sequential(
+            ConvBnRelu(2 * in_channels, out_channels, 1, 1, 0, has_bn=True, has_relu=True, has_bias=False,
+                       norm_layer=norm_layer),
+            nn.Dropout2d(dropout))
+
+    def forward(self, feats):
+        from ..networks.pspnet import _dropout2d
+        feats = _as_act(feats)
+        context = self.stages[0](feats)
+        for stage in self.stages[1:]:
+            context = ops.AddFn.apply(context, stage(feats))
+        out = self.conv_bn_dropout[0](ops.ConcatFn.apply(context, feats))
+        return _dropout2d(out, self.conv_bn_dropout[1].p, self.training)
+
+
 class ReluFn(torch.autograd.Function):
     """stand-alone ReLU on a small tensor (FFM squeeze branch [N,C,1,1], seg_oprs.py:224-226): expressed through
     tsb_bn_apply with scale 1 / shift 0 so it stays on the library path"""
