@@ -173,6 +173,15 @@ int tsb_bn_bwd_apply(const void* dy, int dycs, const void* y, int ycs, const voi
                      double count, int relu, void* dx, int dxcs, void* dres, int drcs, long long npix, int C,
                      float* dgamma_acc, float* dbeta_acc, const float* scale, const float* shift,
                      tsb_stream_t stream);
+/* tsb_bn_bwd_apply, ADDING into dx: dx = bf16(float(dx) + r), rounded once, with r the fp32 value tsb_bn_bwd_apply
+ * would round and store (same arguments, same dgamma_acc / dbeta_acc folding and mask rules). The input gradients of
+ * several BatchNorms over channel slices of one concatenated tensor (DenseASPP's pre-activation blocks) land in one
+ * gradient buffer this way. */
+int tsb_bn_bwd_apply_add(const void* dy, int dycs, const void* y, int ycs, const void* x, int xcs, const float* mean,
+                         const float* invstd, const float* gamma, const float* sum_dz, const float* sum_dz_xhat,
+                         double count, int relu, void* dx, int dxcs, void* dres, int drcs, long long npix, int C,
+                         float* dgamma_acc, float* dbeta_acc, const float* scale, const float* shift,
+                         tsb_stream_t stream);
 /* out/argmax = tsb_maxpool3x3s2_fwd of tsb_bn_apply(x, scale, shift, no residual, relu = 1), bit for bit and in the
  * same layouts, in one pass that never writes the normalised map (the context stem of BiSeNet-R18). */
 int tsb_bn_apply_maxpool3x3s2(const void* x, int xcs, const float* scale, const float* shift, void* out, int ocs,
@@ -297,6 +306,22 @@ int tsb_conv_transpose2d_fprop(const tsb_conv_shape* s, const void* x, int xcs, 
  * workspace large enough for two splits the kernel adds into dw in place. */
 int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs, const void* dy, int dycs, float* dw, float* ws,
                      long long ws_floats, tsb_stream_t stream);
+/* 1x1 convolution of a pre-activation input (BatchNorm → ReLU → 1x1 conv, DenseASPP's blocks): the conv reads
+ *   x̂ = bf16(relu(fmaf(x, in_scale[c], in_shift[c])))
+ * (the arithmetic of tsb_bn_apply with relu, rounded once) instead of x. The kernels normalise each landed activation
+ * tile in shared memory between the TMA load and the wgmma, so x̂ never reaches HBM; rows past the last pixel stay
+ * zero. R = S = 1, stride 1, pad 0 only (anything else: TSB_ERR_UNSUPPORTED); C % 64 == 0; in_scale / in_shift fp32 [C],
+ * 16-byte aligned.
+ * fprop: y = relu?(conv(x̂, w) + bias), the rest as tsb_conv2d_fprop: training passes sum/sumsq (the BN-statistics
+ *        epilogue over the rounded output) and no ReLU; eval passes the next BatchNorm folded into w / bias, relu = 1.
+ *        Bit for bit tsb_bn_apply(relu) followed by tsb_conv2d_fprop (tsb_conv2d_fprop_fused in eval form).
+ * wgrad: dw += Σ_pixels dy ⊗ x̂, the split plan and workspace rules of tsb_conv2d_wgrad; bit for bit tsb_bn_apply(relu)
+ *        followed by tsb_conv2d_wgrad. */
+int tsb_conv1x1_bnrelu_fprop(const tsb_conv_shape* s, const void* x, int xcs, const float* in_scale, const float* in_shift,
+                             const void* w, const float* bias, int relu, void* y, int ydtype, int ycs, float* sum,
+                             float* sumsq, float* ws, long long ws_floats, tsb_stream_t stream);
+int tsb_conv1x1_bnrelu_wgrad(const tsb_conv_shape* s, const void* x, int xcs, const float* in_scale, const float* in_shift,
+                             const void* dy, int dycs, float* dw, float* ws, long long ws_floats, tsb_stream_t stream);
 /* stride-2 C_in=3 stem (7x7 pad 3 or 3x3 pad 1, same packed weight format) on the s2d-packed image (tsb_pack_image_s2d / tsb_pack_stem_weight):
  * xs2d [N,H/2,W/2+4,16] bf16, wp [K,4,4,16] bf16 → y [N,H/2,W/2,K] (K % 8 == 0, channel stride ycs >= K, exactly K
  * channels written). wgrad: dy with channel stride dycs >= K → dwp [K,4,64] fp32 (+=; tsb_unpack_stem_wgrad). */

@@ -47,6 +47,7 @@ _SIGS = {
     "tsb_bn_apply": [P, I, P, P, P, I, I, P, I, L, I, P],
     "tsb_bn_bwd_reduce": [P, I, P, I, P, I, P, P, I, L, I, P, P, P, P, P, L, P],
     "tsb_bn_bwd_apply": [P, I, P, I, P, I, P, P, P, P, P, D, I, P, I, P, I, L, I, P, P, P, P, P],
+    "tsb_bn_bwd_apply_add": [P, I, P, I, P, I, P, P, P, P, P, D, I, P, I, P, I, L, I, P, P, P, P, P],
     "tsb_bn_apply_maxpool3x3s2": [P, I, P, P, P, I, P, I, I, I, I, P],
     "tsb_chan_scale_fwd": [P, I, P, F, P, I, P, I, I, I, I, P],
     "tsb_chan_scale_bwd": [P, I, P, I, P, F, P, I, P, I, I, I, P, L, P],
@@ -65,6 +66,8 @@ _SIGS = {
     "tsb_conv2d_fprop": [P, P, I, P, P, P, I, I, P, P, P, L, P],
     "tsb_conv2d_fprop_fused": [P, P, I, P, P, P, I, I, P, I, I, P],
     "tsb_conv_stem_fprop_fused": [P, I, I, I, P, I, P, I, P, I, P],
+    "tsb_conv1x1_bnrelu_fprop": [P, P, I, P, P, P, P, I, P, I, I, P, P, P, L, P],
+    "tsb_conv1x1_bnrelu_wgrad": [P, P, I, P, P, P, I, P, P, L, P],
     "tsb_conv2d_dgrad": [P, P, I, P, P, I, I, P],
     "tsb_conv2d_wgrad": [P, P, I, P, I, P, P, L, P],
     "tsb_conv_transpose2d_fprop": [P, P, I, P, P, I, P, I, I, P, P, P, L, P],

@@ -248,15 +248,16 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_
     }
 }
 
-template <int kRelu, bool kDres>
-__global__ void __launch_bounds__(kThreads, 3)
-bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_bfloat16* __restrict__ y, int ycs,
-                    const __nv_bfloat16* __restrict__ x, int xcs, const float* __restrict__ mean,
-                    const float* __restrict__ invstd, const float* __restrict__ gamma,
-                    const float* __restrict__ sum_dz, const float* __restrict__ sum_dz_xhat, float inv_count,
-                    __nv_bfloat16* __restrict__ dx, int dxcs, __nv_bfloat16* __restrict__ dres, int drcs,
-                    long long npix, int C8, float* dgamma_acc, float* dbeta_acc, const float* __restrict__ scale,
-                    const float* __restrict__ shift) {
+// kAdd: dx = bf16(float(dx) + r) with r the fp32 value stored without it (tsb_bn_bwd_apply_add)
+template <int kRelu, bool kDres, bool kAdd>
+__device__ __forceinline__ void
+bn_bwd_apply_body(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_bfloat16* __restrict__ y, int ycs,
+                  const __nv_bfloat16* __restrict__ x, int xcs, const float* __restrict__ mean,
+                  const float* __restrict__ invstd, const float* __restrict__ gamma,
+                  const float* __restrict__ sum_dz, const float* __restrict__ sum_dz_xhat, float inv_count,
+                  __nv_bfloat16* __restrict__ dx, int dxcs, __nv_bfloat16* __restrict__ dres, int drcs,
+                  long long npix, int C8, float* dgamma_acc, float* dbeta_acc, const float* __restrict__ scale,
+                  const float* __restrict__ shift) {
     if (dgamma_acc != nullptr && blockIdx.x == 0) {  // fold the parameter-gradient accumulation into this pass
         for (int c = threadIdx.x; c < C8 * 8; c += kThreads) {
             dgamma_acc[c] += sum_dz_xhat[c];
@@ -288,7 +289,7 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_b
     const long long start = (long long)blockIdx.x * kThreads + threadIdx.x;
     VecWalk wk(C8, start, stride);
     for (long long i0 = start; i0 < total; i0 += kU * stride) {
-        uint4 gq[kU], xq[kU], yq[kU];
+        uint4 gq[kU], xq[kU], yq[kU], dq[kU];
         long long pix[kU];
         int c8s[kU];
         bool ok[kU];
@@ -302,8 +303,9 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_b
                 gq[u] = *reinterpret_cast<const uint4*>(dy + pix[u] * dycs + c8s[u] * 8);
                 xq[u] = *reinterpret_cast<const uint4*>(x + pix[u] * xcs + c8s[u] * 8);
                 if (kRelu == 1) yq[u] = *reinterpret_cast<const uint4*>(y + pix[u] * ycs + c8s[u] * 8);
+                if (kAdd) dq[u] = *reinterpret_cast<const uint4*>(dx + pix[u] * dxcs + c8s[u] * 8);
             } else {
-                gq[u] = xq[u] = yq[u] = make_uint4(0u, 0u, 0u, 0u);
+                gq[u] = xq[u] = yq[u] = dq[u] = make_uint4(0u, 0u, 0u, 0u);
             }
         }
 #pragma unroll
@@ -323,6 +325,12 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_b
             }
 #pragma unroll
             for (int k = 0; k < 8; ++k) o[k] = fmaf(A[k], g[k], fmaf(B[k], xv[k], Cc[k]));
+            if (kAdd) {
+                float d[8];
+                unpack8(dq[u], d);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) o[k] = d[k] + o[k];
+            }
             if (ok[u]) {
                 Vec8<__nv_bfloat16>::store(dx + pix[u] * dxcs + c8s[u] * 8, o);
                 if (kDres) Vec8<__nv_bfloat16>::store(dres + pix[u] * drcs + c8s[u] * 8, g);
@@ -330,6 +338,27 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_b
         }
     }
 }
+
+#define TSB_BN_BWD_APPLY_ARGS                                                                                          \
+    const __nv_bfloat16* __restrict__ dy, int dycs, const __nv_bfloat16* __restrict__ y, int ycs,                      \
+        const __nv_bfloat16* __restrict__ x, int xcs, const float* __restrict__ mean, const float* __restrict__ invstd, \
+        const float* __restrict__ gamma, const float* __restrict__ sum_dz, const float* __restrict__ sum_dz_xhat,      \
+        float inv_count, __nv_bfloat16* __restrict__ dx, int dxcs, __nv_bfloat16* __restrict__ dres, int drcs,         \
+        long long npix, int C8, float *dgamma_acc, float *dbeta_acc, const float *__restrict__ scale,                  \
+        const float *__restrict__ shift
+#define TSB_BN_BWD_APPLY_PASS \
+    dy, dycs, y, ycs, x, xcs, mean, invstd, gamma, sum_dz, sum_dz_xhat, inv_count, dx, dxcs, dres, drcs, npix, C8, \
+        dgamma_acc, dbeta_acc, scale, shift
+template <int kRelu, bool kDres>
+__global__ void __launch_bounds__(kThreads, 3) bn_bwd_apply_kernel(TSB_BN_BWD_APPLY_ARGS) {
+    bn_bwd_apply_body<kRelu, kDres, false>(TSB_BN_BWD_APPLY_PASS);
+}
+template <int kRelu, bool kDres>   // the read of dx costs registers: two CTAs per SM keep it free of spills
+__global__ void __launch_bounds__(kThreads, 2) bn_bwd_apply_add_kernel(TSB_BN_BWD_APPLY_ARGS) {
+    bn_bwd_apply_body<kRelu, kDres, true>(TSB_BN_BWD_APPLY_PASS);
+}
+#undef TSB_BN_BWD_APPLY_ARGS
+#undef TSB_BN_BWD_APPLY_PASS
 
 // ---------------------------------------------------------------- channel attention scale (ARM / FFM)
 template <bool kAdd>
@@ -472,31 +501,54 @@ extern "C" int tsb_bn_bwd_reduce(const void* dy, int dycs, const void* y, int yc
     return rc ? rc : tsb_det_reduce(sum_dz_xhat, ws + C, grid, C, 2LL * C, st);
 }
 
+template <bool kAdd>
+static int bn_bwd_apply_impl(const void* dy, int dycs, const void* y, int ycs, const void* x, int xcs,
+                             const float* mean, const float* invstd, const float* gamma, const float* sum_dz,
+                             const float* sum_dz_xhat, double count, int relu, void* dx, int dxcs, void* dres,
+                             int drcs, long long npix, int C, float* dgamma_acc, float* dbeta_acc,
+                             const float* scale, const float* shift, tsb_stream_t stream, const char* who) {
+    TSB_REQUIRE(dy && x && mean && invstd && gamma && sum_dz && sum_dz_xhat && dx && npix > 0 && count > 0, "%s: bad args", who);
+    TSB_REQUIRE((dgamma_acc == nullptr) == (dbeta_acc == nullptr), "%s: dgamma_acc and dbeta_acc go together", who);
+    const int mode = !relu ? 0 : (y ? 1 : 2);
+    TSB_REQUIRE(mode != 2 || (scale && shift), "%s: relu without y needs scale and shift", who);
+    TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, dxcs, dx) &&
+                (mode != 1 || TSB_VEC_OK(C, ycs, y)) && (!dres || TSB_VEC_OK(C, drcs, dres)), "%s: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned", who);
+    TSB_REQUIRE(tsb_aligned16(mean) && tsb_aligned16(invstd) && tsb_aligned16(gamma) && tsb_aligned16(sum_dz) &&
+                tsb_aligned16(sum_dz_xhat) && (mode != 2 || (tsb_aligned16(scale) && tsb_aligned16(shift))),
+                "%s: per-channel vectors must be 16B aligned", who);
+    int C8 = C / 8;
+    int grid = tsb_grid_for(npix * C8, kThreads, 8);
+    cudaStream_t st = (cudaStream_t)stream;
+    float inv_count = (float)(1.0 / count);
+#define K_(R, D) (kAdd ? bn_bwd_apply_add_kernel<R, D> : bn_bwd_apply_kernel<R, D>)
+#define L(R, D) K_(R, D)<<<grid, kThreads, 0, st>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)y, ycs, (const __nv_bfloat16*)x, xcs, mean, invstd, gamma, sum_dz, sum_dz_xhat, inv_count, (__nv_bfloat16*)dx, dxcs, (__nv_bfloat16*)dres, drcs, npix, C8, dgamma_acc, dbeta_acc, scale, shift)
+    if (mode == 0) { if (dres) L(0, true); else L(0, false); }
+    else if (mode == 1) { if (dres) L(1, true); else L(1, false); }
+    else { if (dres) L(2, true); else L(2, false); }
+#undef L
+#undef K_
+    TSB_CUDA_CHECK_LAUNCH(kAdd ? "bn_bwd_apply_add" : "bn_bwd_apply");
+    return TSB_OK;
+}
+
 extern "C" int tsb_bn_bwd_apply(const void* dy, int dycs, const void* y, int ycs, const void* x, int xcs,
                                 const float* mean, const float* invstd, const float* gamma, const float* sum_dz,
                                 const float* sum_dz_xhat, double count, int relu, void* dx, int dxcs, void* dres,
                                 int drcs, long long npix, int C, float* dgamma_acc, float* dbeta_acc,
                                 const float* scale, const float* shift, tsb_stream_t stream) {
-    TSB_REQUIRE(dy && x && mean && invstd && gamma && sum_dz && sum_dz_xhat && dx && npix > 0 && count > 0, "tsb_bn_bwd_apply: bad args");
-    TSB_REQUIRE((dgamma_acc == nullptr) == (dbeta_acc == nullptr), "tsb_bn_bwd_apply: dgamma_acc and dbeta_acc go together");
-    const int mode = !relu ? 0 : (y ? 1 : 2);
-    TSB_REQUIRE(mode != 2 || (scale && shift), "tsb_bn_bwd_apply: relu without y needs scale and shift");
-    TSB_REQUIRE(TSB_VEC_OK(C, dycs, dy) && TSB_VEC_OK(C, xcs, x) && TSB_VEC_OK(C, dxcs, dx) &&
-                (mode != 1 || TSB_VEC_OK(C, ycs, y)) && (!dres || TSB_VEC_OK(C, drcs, dres)), "tsb_bn_bwd_apply: C and channel strides must be multiples of 8, strides >= C, pointers 16B aligned");
-    TSB_REQUIRE(tsb_aligned16(mean) && tsb_aligned16(invstd) && tsb_aligned16(gamma) && tsb_aligned16(sum_dz) &&
-                tsb_aligned16(sum_dz_xhat) && (mode != 2 || (tsb_aligned16(scale) && tsb_aligned16(shift))),
-                "tsb_bn_bwd_apply: per-channel vectors must be 16B aligned");
-    int C8 = C / 8;
-    int grid = tsb_grid_for(npix * C8, kThreads, 8);
-    cudaStream_t st = (cudaStream_t)stream;
-    float inv_count = (float)(1.0 / count);
-#define L(R, D) bn_bwd_apply_kernel<R, D><<<grid, kThreads, 0, st>>>((const __nv_bfloat16*)dy, dycs, (const __nv_bfloat16*)y, ycs, (const __nv_bfloat16*)x, xcs, mean, invstd, gamma, sum_dz, sum_dz_xhat, inv_count, (__nv_bfloat16*)dx, dxcs, (__nv_bfloat16*)dres, drcs, npix, C8, dgamma_acc, dbeta_acc, scale, shift)
-    if (mode == 0) { if (dres) L(0, true); else L(0, false); }
-    else if (mode == 1) { if (dres) L(1, true); else L(1, false); }
-    else { if (dres) L(2, true); else L(2, false); }
-#undef L
-    TSB_CUDA_CHECK_LAUNCH("bn_bwd_apply");
-    return TSB_OK;
+    return bn_bwd_apply_impl<false>(dy, dycs, y, ycs, x, xcs, mean, invstd, gamma, sum_dz, sum_dz_xhat, count, relu, dx,
+                                    dxcs, dres, drcs, npix, C, dgamma_acc, dbeta_acc, scale, shift, stream,
+                                    "tsb_bn_bwd_apply");
+}
+
+extern "C" int tsb_bn_bwd_apply_add(const void* dy, int dycs, const void* y, int ycs, const void* x, int xcs,
+                                    const float* mean, const float* invstd, const float* gamma, const float* sum_dz,
+                                    const float* sum_dz_xhat, double count, int relu, void* dx, int dxcs, void* dres,
+                                    int drcs, long long npix, int C, float* dgamma_acc, float* dbeta_acc,
+                                    const float* scale, const float* shift, tsb_stream_t stream) {
+    return bn_bwd_apply_impl<true>(dy, dycs, y, ycs, x, xcs, mean, invstd, gamma, sum_dz, sum_dz_xhat, count, relu, dx,
+                                   dxcs, dres, drcs, npix, C, dgamma_acc, dbeta_acc, scale, shift, stream,
+                                   "tsb_bn_bwd_apply_add");
 }
 
 extern "C" int tsb_chan_scale_fwd(const void* x, int xcs, const float* a, float base, const void* add, int acs, void* y,

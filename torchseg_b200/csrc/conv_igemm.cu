@@ -31,6 +31,10 @@ struct alignas(64) WgParams {
     float* dw;                // dW-shaped slice per split (workspace), part_stride apart; or dW itself when `add`
     long long part_stride;
     int add;                  // one split: add in place
+    // input prologue (flat 1x1 only): X = bf16(relu(x·in_scale[c] + in_shift[c])) over the pro_q pixels
+    const float* in_scale;
+    const float* in_shift;
+    int pro_q;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -45,7 +49,11 @@ constexpr int kWgStageBytes = 2 * kWgBoxBytes + 4 * kWgBoxBytes;  // A (2 boxes)
 constexpr int kWgBarOff = kWgStages * kWgStageBytes;
 constexpr int kWgSmemTotal = kWgBarOff + 256 + 1024;
 
-__global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __grid_constant__ WgParams p) {
+// PRO: the input prologue of tsb_conv1x1_bnrelu_wgrad (flat launches only). Both consumer warpgroups read every X box
+// of a stage, so the 256 consumer threads normalise the landed boxes together (bnrelu_box), fence them into the async
+// proxy and meet at named barrier 1 before the wgmmas.
+template <bool PRO>
+__device__ __forceinline__ void wgrad_mnmajor_body(const WgParams& p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kWgBarOff);
@@ -107,6 +115,16 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __gr
         for (int j = 0; j < 4; ++j) fence_operands(acc[j]);
         for (int it = 0; it < total_iters; ++it) {
             ring.wait_full();
+            if constexpr (PRO) {
+                const int rows = min(64, p.pro_q - (t_begin + it) * 64);   // flat: tile t holds pixels [64 t, 64 t + 64)
+                uint8_t* b_s = smem + ring.slot * kWgStageBytes + 2 * kWgBoxBytes;
+                for (int j = 0; j < nb; ++j) {   // one tap: box b holds channel chunk b
+                    bnrelu_box<64, kWgConsumers * 128>(b_s + j * kWgBoxBytes, rows, threadIdx.x, p.in_scale + (box0 + j) * 64,
+                                                       p.in_shift + (box0 + j) * 64);
+                }
+                fence_proxy_async();
+                asm volatile("bar.sync 1, %0;" ::"n"(kWgConsumers * 128) : "memory");
+            }
             const uint32_t a_lo = base_lo + (uint32_t)(ring.slot * (kWgStageBytes >> 4)) + (uint32_t)c * (kWgBoxBytes >> 4);
             const uint32_t b_lo = base_lo + (uint32_t)(ring.slot * (kWgStageBytes >> 4)) + ((2 * kWgBoxBytes) >> 4);
 #pragma unroll
@@ -140,9 +158,19 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __gr
     }
 }
 
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_kernel(const __grid_constant__ WgParams p) {
+    wgrad_mnmajor_body<false>(p);
+}
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_mnmajor_bnrelu_kernel(const __grid_constant__ WgParams p) {
+    wgrad_mnmajor_body<true>(p);
+}
+
 int launch_wg(const WgParams& prm, int splits, int co_tiles, int groups, cudaStream_t st) {
-    { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(wgrad_mnmajor_kernel), kWgSmemTotal); if (rc_) return rc_; }
-    wgrad_mnmajor_kernel<<<dim3(splits, co_tiles, groups), kWgThreads, kWgSmemTotal, st>>>(prm);
+    const void* k = prm.in_scale ? reinterpret_cast<const void*>(wgrad_mnmajor_bnrelu_kernel)
+                                 : reinterpret_cast<const void*>(wgrad_mnmajor_kernel);
+    { int rc_ = tsb_ensure_dyn_smem(k, kWgSmemTotal); if (rc_) return rc_; }
+    if (prm.in_scale) wgrad_mnmajor_bnrelu_kernel<<<dim3(splits, co_tiles, groups), kWgThreads, kWgSmemTotal, st>>>(prm);
+    else wgrad_mnmajor_kernel<<<dim3(splits, co_tiles, groups), kWgThreads, kWgSmemTotal, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("wgrad_mnmajor");
     return TSB_OK;
 }
@@ -154,7 +182,7 @@ int launch_wg(const WgParams& prm, int splits, int co_tiles, int groups, cudaStr
 // =================================================================================================
 static int fprop_impl(const tsb_conv_shape* s, const void* x, int xcs, const void* w, const float* bias, void* y, int ydtype,
                       int ycs, float* sum, float* sumsq, float* ws, long long ws_floats, const void* res, int relu,
-                      tsb_stream_t stream) {
+                      tsb_stream_t stream, const float* in_scale = nullptr, const float* in_shift = nullptr) {
     int rc = check_conv_shape(s, "tsb_conv2d_fprop");
     if (rc) return rc;
     TSB_REQUIRE(x && w && y, "tsb_conv2d_fprop: null pointer");
@@ -187,6 +215,7 @@ static int fprop_impl(const tsb_conv_shape* s, const void* x, int xcs, const voi
     d.bias = bias; d.sum = sum; d.sumsq = sumsq; d.out = y;
     d.relu = relu; d.res = res;
     d.ws = ws; d.ws_floats = ws_floats;
+    d.in_scale = in_scale; d.in_shift = in_shift;
     return convv2::launch(d, st);
 }
 
@@ -202,6 +231,38 @@ extern "C" int tsb_conv2d_fprop_fused(const tsb_conv_shape* s, const void* x, in
     TSB_REQUIRE(res == nullptr || (rescs == ycs && ydtype == TSB_BF16 && tsb_aligned16(res)),
                 "tsb_conv2d_fprop_fused: the residual must be a bf16 tensor laid out exactly like the output (rescs == ycs)");
     return fprop_impl(s, x, xcs, w, bias, y, ydtype, ycs, nullptr, nullptr, nullptr, 0, res, relu != 0, stream);
+}
+
+// The input-prologue checks of the two tsb_conv1x1_bnrelu_* entry points: a 1x1 stride-1 unpadded geometry (anything
+// else is TSB_ERR_UNSUPPORTED), C % 64 == 0, 16-byte aligned per-channel vectors.
+static int check_bnrelu_1x1(const tsb_conv_shape* s, const float* in_scale, const float* in_shift, const char* who) {
+    int rc = check_conv_shape(s, who);
+    if (rc) return rc;
+    if (!(s->R == 1 && s->S == 1 && s->stride == 1 && s->pad == 0))
+        TSB_FAIL(TSB_ERR_UNSUPPORTED, "%s: only 1x1 stride-1 convolutions without padding (got R %d, stride %d, pad %d)", who,
+                 s->R, s->stride, s->pad);
+    TSB_REQUIRE(in_scale && in_shift, "%s: null in_scale / in_shift", who);
+    TSB_REQUIRE(tsb_aligned16(in_scale) && tsb_aligned16(in_shift), "%s: in_scale and in_shift must be 16-byte aligned", who);
+    TSB_REQUIRE(s->C % 64 == 0, "%s: C must be a multiple of 64 (got %d)", who, s->C);
+    return TSB_OK;
+}
+
+extern "C" int tsb_conv1x1_bnrelu_fprop(const tsb_conv_shape* s, const void* x, int xcs, const float* in_scale,
+                                        const float* in_shift, const void* w, const float* bias, int relu, void* y,
+                                        int ydtype, int ycs, float* sum, float* sumsq, float* ws, long long ws_floats,
+                                        tsb_stream_t stream) {
+    const char* who = "tsb_conv1x1_bnrelu_fprop";
+    int rc = check_bnrelu_1x1(s, in_scale, in_shift, who);
+    if (rc) return rc;
+    TSB_REQUIRE(x && w && y, "%s: null pointer", who);
+    TSB_REQUIRE(xcs % 8 == 0 && xcs >= s->C && tsb_aligned16(x) && tsb_aligned16(w),
+                "%s: x channel stride must be a multiple of 8 and at least C, x and w 16-byte aligned (got xcs %d, C %d)", who,
+                xcs, s->C);
+    TSB_REQUIRE(ycs % 8 == 0 && ycs >= s->K && tsb_aligned16(y),
+                "%s: y channel stride must be a multiple of 8 and at least K (got ycs %d, K %d)", who, ycs, s->K);
+    TSB_REQUIRE(!(sum && relu), "%s: the statistics epilogue (training) takes no ReLU", who);
+    return fprop_impl(s, x, xcs, w, bias, y, ydtype, ycs, sum, sumsq, ws, ws_floats, nullptr, relu != 0, stream, in_scale,
+                      in_shift);
 }
 
 // The dgrad-form launches of conv geometry `s`: out[N,H,W,·] (channel stride ocs) = the transposed convolution of
@@ -343,14 +404,15 @@ int wgrad_common(WgParams& prm, int N, int P, int Q, int K, float* ws, long long
 }
 }  // namespace
 
-extern "C" int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs, const void* dy, int dycs, float* dw,
-                                float* ws, long long ws_floats, tsb_stream_t stream) {
-    int rc = check_conv_shape(s, "tsb_conv2d_wgrad");
+static int wgrad_impl(const tsb_conv_shape* s, const void* x, int xcs, const void* dy, int dycs, float* dw, float* ws,
+                      long long ws_floats, tsb_stream_t stream, const char* who, const float* in_scale = nullptr,
+                      const float* in_shift = nullptr) {
+    int rc = check_conv_shape(s, who);
     if (rc) return rc;
-    TSB_REQUIRE(x && dy && dw, "tsb_conv2d_wgrad: null pointer");
-    TSB_REQUIRE(s->C % 64 == 0, "tsb_conv2d_wgrad: C must be a multiple of 64 (got %d)", s->C);
+    TSB_REQUIRE(x && dy && dw, "%s: null pointer", who);
+    TSB_REQUIRE(s->C % 64 == 0, "%s: C must be a multiple of 64 (got %d)", who, s->C);
     TSB_REQUIRE(xcs % 8 == 0 && xcs >= s->C && dycs % 8 == 0 && dycs >= s->K && tsb_aligned16(x) && tsb_aligned16(dy) &&
-                tsb_aligned16(dw), "tsb_conv2d_wgrad: layout (xcs >= C, dycs >= K, multiples of 8, 16-byte aligned)");
+                tsb_aligned16(dw), "%s: layout (xcs >= C, dycs >= K, multiples of 8, 16-byte aligned)", who);
     cudaStream_t st = (cudaStream_t)stream;
     int N = s->N, H = s->H, W = s->W, P = s->P, Q = s->Q;
     const bool flat = (s->R == 1 && s->stride == 1 && s->pad == 0);
@@ -389,7 +451,21 @@ extern "C" int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs,
     prm.C = s->C;
     prm.dw_row_stride = dw_row_stride;
     prm.dw = dw;
+    prm.in_scale = in_scale; prm.in_shift = in_shift; prm.pro_q = Q;   // set only for flat launches
     return wgrad_common(prm, N, P, Q, s->K, ws, ws_floats, st);
+}
+
+extern "C" int tsb_conv2d_wgrad(const tsb_conv_shape* s, const void* x, int xcs, const void* dy, int dycs, float* dw,
+                                float* ws, long long ws_floats, tsb_stream_t stream) {
+    return wgrad_impl(s, x, xcs, dy, dycs, dw, ws, ws_floats, stream, "tsb_conv2d_wgrad");
+}
+
+extern "C" int tsb_conv1x1_bnrelu_wgrad(const tsb_conv_shape* s, const void* x, int xcs, const float* in_scale,
+                                        const float* in_shift, const void* dy, int dycs, float* dw, float* ws,
+                                        long long ws_floats, tsb_stream_t stream) {
+    const char* who = "tsb_conv1x1_bnrelu_wgrad";
+    int rc = check_bnrelu_1x1(s, in_scale, in_shift, who);
+    return rc ? rc : wgrad_impl(s, x, xcs, dy, dycs, dw, ws, ws_floats, stream, who, in_scale, in_shift);
 }
 
 // ---------------------------------------------------------------------------------- 7x7/2 stem

@@ -55,6 +55,9 @@ struct alignas(64) V2Params {
     void* out;
     // shared-memory plan
     int nstages, stage_bytes, res_bytes;
+    // input prologue (flat 1x1 only): A = bf16(relu(x·in_scale[c] + in_shift[c])), applied to each landed stage
+    const float* in_scale;
+    const float* in_shift;
 };
 
 // BN = 64 epilogue: each consumer warp turns its 16 channels x 16 pixels of the transposed fragment into pixel-major
@@ -63,318 +66,12 @@ struct alignas(64) V2Params {
 constexpr int kStgStride = 20;
 constexpr int kStgWarpBytes = 16 * kStgStride * 4;
 
-template <int BN, bool RES>
-__global__ void __launch_bounds__(kThreads, 1) igemm_v2_kernel(const __grid_constant__ V2Params p) {
-    // BN = 64: D^T[64 out-ch, px] = W[64, k] · X[px, k]^T. The weight tile is the wgmma A operand, shared by both
-    // warpgroups, and each warpgroup takes its own 128-pixel m-tile as B (m64n128k16): a CTA work unit is a pair of
-    // m-tiles. BN = 128: D[px, 128 out-ch] = X · W^T, one m-tile per unit, rows 0-63 / 64-127 per warpgroup.
-    // CTA b takes the m-tiles b, b + G, b + 2G, ... (G = gridDim.x) in that order, kTiles per unit, at either BN.
-    constexpr bool kPixN = (BN == 64);
-    constexpr int kTiles = kPixN ? 2 : 1;            // m-tiles per work unit = activation boxes per stage
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* res_b = smem;                       // resident weights (RES)
-    uint8_t* stages = smem + p.res_bytes;        // ring of A (+B) stages
-    uint8_t* tail = stages + p.nstages * p.stage_bytes;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
-    uint64_t* b_ready = full_bar + 2 * kMaxStages;
-    float* s_stage = reinterpret_cast<float*>(tail + 256);  // BN = 64: [consumer warp][16 px][kStgStride]
-    // BN = 64 with statistics: the rounded outputs of a unit, [tile][128 px][64 ch] bf16, 16-byte chunks of a pixel row
-    // swizzled by px & 7. The per-warp statistics slots [consumer warp][2*BN] share the space: they are written after
-    // the last unit.
-    uint8_t* s_out = tail + 256 + (kPixN ? kConsumers * 4 * kStgWarpBytes : 0);
-    float* s_stats = reinterpret_cast<float*>(s_out);
-    StageRing ring(full_bar, full_bar + kMaxStages, p.nstages);
-
-    const int warp = warp_uniform_idx(), lane = threadIdx.x & 31;
-    const int n0 = blockIdx.y * BN;
-    const int my_tiles = (p.m_tiles > (int)blockIdx.x) ? (p.m_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-    const int my_units = (my_tiles + kTiles - 1) / kTiles;
-    constexpr int kBTile = BN * 128;
-    constexpr int kWOff = kTiles * kAStageBytes;     // streamed weights follow the activation boxes of a stage
-    constexpr int kProducer = kConsumers * 4;
-
-    if (warp == kProducer && lane == 0) {
-        tma_prefetch_desc(&p.mapB);
-        tma_prefetch_desc(&p.mapA[0]);
-        ring.init(kConsumers * 4);
-        mbar_init(b_ready, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
-
-    if (warp == kProducer) {
-        if (lane == 0 && my_units > 0) {
-            if (RES) {  // weights of this N-tile: loaded once per CTA
-                mbar_arrive_expect_tx(b_ready, (uint32_t)(p.ntaps_total * p.kchunks * kBTile));
-                for (int g = 0; g < p.ngroups; ++g)
-                    for (int t = 0; t < p.groups[g].ntaps; ++t)
-                        for (int kc = 0; kc < p.kchunks; ++kc)
-                            tma_load_2d(res_b + (p.groups[g].tap_idx[t] * p.kchunks + kc) * kBTile, &p.mapB, b_ready,
-                                        p.groups[g].bk[t] + kc * 64, n0);
-            }
-            for (int i = 0; i < my_units; ++i) {
-                // the last unit of an odd tile count has one box: the second warpgroup's slot is left as it was and its
-                // results are not stored
-                const int nbox = min(kTiles, my_tiles - i * kTiles);
-                int q0[kTiles], p0[kTiles], n_img[kTiles];
-#pragma unroll
-                for (int b = 0; b < kTiles; ++b) {
-                    const int tile = blockIdx.x + (i * kTiles + b) * gridDim.x;
-                    q0[b] = (tile % p.tiles_w) * p.TW;
-                    p0[b] = ((tile / p.tiles_w) % p.tiles_h) * p.TH;
-                    n_img[b] = tile / (p.tiles_w * p.tiles_h);
-                }
-                for (int g = 0; g < p.ngroups; ++g) {
-                    const int gmap = p.groups[g].map, ntaps = p.groups[g].ntaps;
-                    const uint32_t bytes = (uint32_t)(nbox * p.a_bytes[gmap]) + (RES ? 0u : (uint32_t)(ntaps * kBTile));
-                    for (int kc = 0; kc < p.kchunks; ++kc) {
-                        ring.acquire();
-                        uint8_t* a_s = stages + ring.slot * p.stage_bytes;
-                        mbar_arrive_expect_tx(ring.full_bar(), bytes);
-#pragma unroll
-                        for (int b = 0; b < kTiles; ++b)
-                            if (b < nbox)
-                                tma_load_4d(a_s + b * kAStageBytes, &p.mapA[gmap], ring.full_bar(), kc * 64,
-                                            q0[b] + p.groups[g].dw0, p0[b] + p.groups[g].dh, n_img[b]);
-                        if (!RES) {
-                            for (int t = 0; t < ntaps; ++t)
-                                tma_load_2d(a_s + kWOff + t * kBTile, &p.mapB, ring.full_bar(), p.groups[g].bk[t] + kc * 64, n0);
-                        }
-                        ring.advance();
-                    }
-                }
-            }
-        }
-    } else {
-        const int c = warp >> 2, wq = warp & 3;
-        const bool do_stats = (p.sum != nullptr);
-        const uint64_t desc_hi = desc_hi_sw128(16, 1024);   // K-major, 8-row groups 1024 B apart (both operands)
-        const uint32_t stages_lo = smem_u32(stages) >> 4;
-        const uint32_t res_lo = smem_u32(res_b) >> 4;
-        // this warpgroup's activation rows in a stage: its own box (BN = 64) or its 64-pixel half of the box (BN = 128)
-        const uint32_t x_off = (uint32_t)c * (kPixN ? (uint32_t)(kAStageBytes >> 4) : 512u);
-        // running column sums over all tiles of the CTA (columns 8j + cq + e) of thread fragment rows m0 and m0 + 8 of
-        // every tile, in tile order; at BN = 64 read back from the unit's rounded outputs in shared memory, so that both
-        // tile widths sum every channel in the same order
-        const int m0 = c * 64 + wq * 16 + (lane >> 2);
-        const int cq = 2 * (lane & 3);                 // first of the thread's two columns in every 8-column group
-        float run1[BN / 4], run2[BN / 4];
-#pragma unroll
-        for (int q = 0; q < BN / 4; ++q) { run1[q] = 0.f; run2[q] = 0.f; }
-        if (RES && my_units > 0) mbar_wait(b_ready, 0);
-        for (int i = 0; i < my_units; ++i) {   // the ring's slot and phase run on across units; each unit drains
-            float acc[64];
-#pragma unroll
-            for (int q = 0; q < 64; ++q) acc[q] = 0.f;
-            fence_operands(acc);
-            for (int g = 0; g < p.ngroups; ++g) {
-                const int ntaps = p.groups[g].ntaps;
-                for (int kc = 0; kc < p.kchunks; ++kc) {
-                    ring.wait_full();
-                    const uint32_t st_lo = stages_lo + (uint32_t)(ring.slot * p.stage_bytes >> 4);
-                    // a group has at most 3 taps: unrolled by 2, the issue code holds 12 HGMMA (by default ptxas unrolls
-                    // the streamed-weights variant by 4)
-#pragma unroll 2
-                    for (int t = 0; t < ntaps; ++t) {
-                        const uint32_t x_lo = st_lo + x_off + (uint32_t)p.groups[g].row_off[t] * 8u;
-                        const uint32_t w_lo = RES ? res_lo + (uint32_t)((p.groups[g].tap_idx[t] * p.kchunks + kc) * kBTile >> 4)
-                                                  : st_lo + (uint32_t)((kWOff + t * kBTile) >> 4);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {  // 16 bf16 = 32 B = 2 descriptor units inside the swizzle atom
-                            const uint64_t dx = desc_at(desc_hi, x_lo + 2 * k), dw = desc_at(desc_hi, w_lo + 2 * k);
-                            if constexpr (kPixN) wgmma_m64n128<0, 0>(acc, dw, dx, 1u);
-                            else wgmma_m64n128<0, 0>(acc, dx, dw, 1u);
-                        }
-                    }
-                    ring.commit_release_prev();
-                }
-            }
-            ring.drain();
-            fence_operands(acc);
-            if constexpr (kPixN) {
-                const int tile = blockIdx.x + (2 * i + c) * gridDim.x;
-                const bool tile_ok = 2 * i + c < my_tiles;   // false for the empty half of the last unit
-                const int tw_i = tile % p.tiles_w;
-                const int th_i = (tile / p.tiles_w) % p.tiles_h;
-                const int n_img = tile / (p.tiles_w * p.tiles_h);
-                // fragment: acc[4j + 2h + e] = D^T[channel 16 wq + lane/4 + 8h][pixel 8j + 2 (lane % 4) + e]
-                const int ch = n0 + 16 * wq + (lane >> 2);
-                const bool bias0 = p.bias != nullptr && ch < p.k_real, bias1 = p.bias != nullptr && ch + 8 < p.k_real;
-                const float b0 = bias0 ? __ldg(p.bias + ch) : 0.f, b1 = bias1 ? __ldg(p.bias + ch + 8) : 0.f;
-                float* stg = s_stage + (threadIdx.x >> 5) * (16 * kStgStride);
-                // after the transpose a lane holds one pixel and 8 consecutive channels
-                const int px = lane & 15;
-                const int col = n0 + 16 * wq + 8 * (lane >> 4);   // multiple of 8, as is k_store: all 8 stored or none
-                const float* rd = stg + px * kStgStride + 8 * (lane >> 4);
-#pragma unroll
-                for (int k = 0; k < 8; ++k) {   // 16 pixels (fragment columns j = 2k, 2k + 1) per step
-#pragma unroll
-                    for (int jj = 0; jj < 2; ++jj)
-#pragma unroll
-                        for (int h = 0; h < 2; ++h)
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                float a = acc[4 * (2 * k + jj) + 2 * h + e];
-                                if (h ? bias1 : bias0) a += h ? b1 : b0;
-                                stg[(8 * jj + 2 * (lane & 3) + e) * kStgStride + (lane >> 2) + 8 * h] = a;
-                            }
-                    __syncwarp();
-                    const float4 lo = *reinterpret_cast<const float4*>(rd), hi = *reinterpret_cast<const float4*>(rd + 4);
-                    __syncwarp();
-                    float v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-                    const int m = 16 * k + px;
-                    const int pp = th_i * p.TH + (m >> p.tw_shift), qq = tw_i * p.TW + (m & (p.TW - 1));
-                    const bool valid = tile_ok && (pp < p.P) && (qq < p.Q);
-                    const bool st = valid && col < p.k_store;
-                    const long long off = p.out_base + (long long)n_img * p.out_n_stride + (long long)pp * p.out_p_stride +
-                                          (long long)qq * p.out_q_stride + col;
-                    if (p.res != nullptr && st) {     // folded-BN inference tail of a residual block: + shortcut
-                        float r[8];
-                        unpack8(*reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + off), r);
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) v[e] += r[e];
-                    }
-                    if (p.relu) {
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) v[e] = fmaxf(v[e], 0.f);
-                    }
-                    if (p.out_f32) {
-                        if (st) {
-                            float4* o = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + off);
-                            o[0] = make_float4(v[0], v[1], v[2], v[3]);
-                            o[1] = make_float4(v[4], v[5], v[6], v[7]);
-                        }
-                    } else {
-                        uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + off);
-                        if (p.accumulate && st) {
-                            float r[8];
-                            unpack8(*o, r);
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) v[e] += r[e];
-                        }
-                        // round once to bf16; statistics are taken of the rounded values the next layer will see
-                        const uint4 u = pack8(v);
-                        if (st) *o = u;
-                        if (do_stats)
-                            *reinterpret_cast<uint4*>(s_out + (c * 128 + m) * 128 + (((2 * wq + (lane >> 4)) ^ (px & 7)) << 4)) = u;
-                    }
-                }
-                if (do_stats) {
-                    // every value the statistics see, in the order of the fragment rows of one 128-pixel tile; (pp, qq)
-                    // are launch-grid coordinates (a stride-2 parity class's own sub-grid for the transposed forward), so
-                    // only the stores above use the output strides
-                    asm volatile("bar.sync 1, %0;" ::"n"(kConsumers * 128) : "memory");
-#pragma unroll
-                    for (int s = 0; s < 2; ++s) {
-                        if (2 * i + s < my_tiles) {
-                            const int t2 = blockIdx.x + (2 * i + s) * gridDim.x;
-                            const int tw2 = t2 % p.tiles_w, th2 = (t2 / p.tiles_w) % p.tiles_h;
-#pragma unroll
-                            for (int h = 0; h < 2; ++h) {
-                                const int m = m0 + 8 * h;
-                                const int pp = th2 * p.TH + (m >> p.tw_shift), qq = tw2 * p.TW + (m & (p.TW - 1));
-                                if (pp < p.P && qq < p.Q) {
-                                    const uint8_t* row = s_out + (s * 128 + m) * 128 + 2 * cq;
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) {
-                                        const uint32_t u = *reinterpret_cast<const uint32_t*>(row + ((j ^ (m & 7)) << 4));
-                                        const float v0 = bf16lo(u), v1 = bf16hi(u);
-                                        run1[2 * j] += v0; run2[2 * j] = fmaf(v0, v0, run2[2 * j]);
-                                        run1[2 * j + 1] += v1; run2[2 * j + 1] = fmaf(v1, v1, run2[2 * j + 1]);
-                                    }
-                                }
-                            }
-                        }
-                    }
-                    asm volatile("bar.sync 1, %0;" ::"n"(kConsumers * 128) : "memory");   // s_out is free again
-                }
-            } else {
-                // warpgroup c owns pixel rows [64c, 64c + 64) of the tile; thread fragment rows m0 and m0 + 8
-                const int tile = blockIdx.x + i * gridDim.x;
-                const int tw_i = tile % p.tiles_w;
-                const int th_i = (tile / p.tiles_w) % p.tiles_h;
-                const int n_img = tile / (p.tiles_w * p.tiles_h);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int m = m0 + 8 * h;
-                    const int pp = th_i * p.TH + (m >> p.tw_shift), qq = tw_i * p.TW + (m & (p.TW - 1));
-                    const bool valid = (pp < p.P) && (qq < p.Q);
-                    const long long pix_off = p.out_base + (long long)n_img * p.out_n_stride + (long long)pp * p.out_p_stride +
-                                              (long long)qq * p.out_q_stride;
-#pragma unroll
-                    for (int j = 0; j < BN / 8; ++j) {
-                        const int col = n0 + 8 * j + cq;     // even; k_store is a multiple of 8, so col + 1 is in range too
-                        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                        if (p.bias != nullptr) {
-                            if (col < p.k_real) v0 += __ldg(p.bias + col);
-                            if (col + 1 < p.k_real) v1 += __ldg(p.bias + col + 1);
-                        }
-                        const bool st = valid && col < p.k_store;
-                        if (p.res != nullptr && st) {     // folded-BN inference tail of a residual block: + shortcut
-                            const uint32_t u = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + pix_off + col);
-                            v0 += bf16lo(u);
-                            v1 += bf16hi(u);
-                        }
-                        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                        if (p.out_f32) {
-                            if (st) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix_off + col) = make_float2(v0, v1);
-                        } else {
-                            uint32_t* o = reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + pix_off + col);
-                            if (p.accumulate && st) {
-                                const uint32_t u = *o;
-                                v0 += bf16lo(u);
-                                v1 += bf16hi(u);
-                            }
-                            // round once to bf16; statistics are taken of the rounded values the next layer will see
-                            const uint32_t u = pack_bf16(v0, v1);
-                            v0 = bf16lo(u);
-                            v1 = bf16hi(u);
-                            if (st) *o = u;
-                        }
-                        if (do_stats && valid) {
-                            run1[2 * j] += v0; run2[2 * j] = fmaf(v0, v0, run2[2 * j]);
-                            run1[2 * j + 1] += v1; run2[2 * j + 1] = fmaf(v1, v1, run2[2 * j + 1]);
-                        }
-                    }
-                }
-            }
-        }
-        if (do_stats) {
-            // lanes with the same lane % 4 hold the same columns: reduce over lane / 4, then across warps in smem
-#pragma unroll
-            for (int q = 0; q < BN / 4; ++q) {
-#pragma unroll
-                for (int off = 4; off < 32; off <<= 1) {
-                    run1[q] += __shfl_xor_sync(0xffffffffu, run1[q], off);
-                    run2[q] += __shfl_xor_sync(0xffffffffu, run2[q], off);
-                }
-            }
-            if (lane < 4) {
-                float* sw = s_stats + (threadIdx.x >> 5) * 2 * BN;   // re-derived: keeping `warp` live spills at BN = 128
-#pragma unroll
-                for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        sw[8 * j + cq + e] = run1[2 * j + e];
-                        sw[BN + 8 * j + cq + e] = run2[2 * j + e];
-                    }
-            }
-            asm volatile("bar.sync 1, %0;" ::"n"(kConsumers * 128) : "memory");  // the consumer warpgroups only
-            // fixed summation order everywhere (no float atomics): per-warp slots, summed in warp order; the CTA's
-            // totals go to its workspace slot and tsb_det_reduce adds the slots in CTA order
-            float* part = p.part + (long long)blockIdx.x * 2 * p.k_real;
-            for (int i = threadIdx.x; i < BN; i += kConsumers * 128) {
-                if (n0 + i < p.k_real) {
-                    float t1 = 0.f, t2 = 0.f;
-                    for (int w = 0; w < kConsumers * 4; ++w) { t1 += s_stats[w * 2 * BN + i]; t2 += s_stats[w * 2 * BN + BN + i]; }
-                    part[n0 + i] = t1;
-                    part[p.k_real + n0 + i] = t2;
-                }
-            }
-        }
-    }
-}
+#define IGEMM_V2_NAME igemm_v2_kernel
+#define IGEMM_V2_PRO false
+#include "igemm_v2_kernel.inc"
+#define IGEMM_V2_NAME igemm_v2_bnrelu_kernel
+#define IGEMM_V2_PRO true
+#include "igemm_v2_kernel.inc"
 
 // ------------------------------------------------------------------------------------------------
 // wgrad, row-tile variant: the horizontal taps of one filter row share ONE activation box.
@@ -491,8 +188,11 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_rows_kernel(const __grid_co
 
 template <int BN, bool RES>
 int launch_v2(const V2Params& prm, int grid_x, int n_tiles, size_t smem, cudaStream_t st) {
-    { int rc_ = tsb_ensure_dyn_smem(reinterpret_cast<const void*>(igemm_v2_kernel<BN, RES>), smem); if (rc_) return rc_; }
-    igemm_v2_kernel<BN, RES><<<dim3(grid_x, n_tiles), kThreads, smem, st>>>(prm);
+    const void* k = prm.in_scale ? reinterpret_cast<const void*>(igemm_v2_bnrelu_kernel<BN, RES>)
+                                 : reinterpret_cast<const void*>(igemm_v2_kernel<BN, RES>);
+    { int rc_ = tsb_ensure_dyn_smem(k, smem); if (rc_) return rc_; }
+    if (prm.in_scale) igemm_v2_bnrelu_kernel<BN, RES><<<dim3(grid_x, n_tiles), kThreads, smem, st>>>(prm);
+    else igemm_v2_kernel<BN, RES><<<dim3(grid_x, n_tiles), kThreads, smem, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("igemm_v2");
     return TSB_OK;
 }
@@ -517,10 +217,14 @@ int launch(const Desc& d, cudaStream_t st, int* stat_slots) {
     for (int t = 0; t < d.ntaps; ++t) {
         const Tap& T = d.taps[t];
         int g = -1;
-        if (rows) {
-            for (int k = 0; k < ng; ++k)
-                if (prm.groups[k].map == T.map && prm.groups[k].dh == T.dh && prm.groups[k].ntaps < 3 &&
-                    abs(T.dw - prm.groups[k].dw0) <= 8) { g = k; break; }
+        if (rows) {   // join a group when its box stays within 8 extra pixels (taps may arrive in either dw order)
+            for (int k = 0; k < ng; ++k) {
+                const TapGroup& G = prm.groups[k];
+                if (G.map != T.map || G.dh != T.dh || G.ntaps >= 3) continue;
+                int hi = G.dw0;
+                for (int j = 0; j < G.ntaps; ++j) hi = max(hi, G.dw0 + G.row_off[j]);
+                if (max(hi, T.dw) - min(G.dw0, T.dw) <= 8) { g = k; break; }
+            }
         }
         if (g < 0) {
             g = ng++;
@@ -565,6 +269,8 @@ int launch(const Desc& d, cudaStream_t st, int* stat_slots) {
     prm.k_real = d.k_real; prm.k_store = d.k_store; prm.out_f32 = d.out_f32; prm.accumulate = d.accumulate;
     prm.bias = d.bias; prm.sum = d.sum; prm.sumsq = d.sumsq; prm.out = d.out;
     prm.relu = d.relu; prm.res = d.res;
+    TSB_REQUIRE(d.in_scale == nullptr || (d.flat && !d.stem && d.ntaps == 1), "conv_v2: the input prologue needs a flat 1x1 launch");
+    prm.in_scale = d.in_scale; prm.in_shift = d.in_shift;
     // ---- shared-memory plan: resident weights, then the stage ring (one activation box per m-tile of a work unit,
     // + the streamed weight tiles), then barriers and the epilogue space: BN = 128, the statistics slots; BN = 64, the
     // transpose buffers and, with statistics, the unit's rounded outputs (which the statistics slots reuse)

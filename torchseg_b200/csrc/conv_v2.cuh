@@ -33,6 +33,9 @@ struct Desc {
     const void* res;   // bf16 residual addressed exactly like `out`
     float* ws;         // caller's workspace for the per-CTA statistics (needed when sum != nullptr)
     long long ws_floats;
+    // flat 1x1 only: the A operand is bf16(relu(act·in_scale[c] + in_shift[c])), normalised in shared memory
+    const float* in_scale;
+    const float* in_shift;
 };
 
 struct WgradDesc {

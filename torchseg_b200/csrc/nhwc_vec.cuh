@@ -60,29 +60,6 @@ template <> struct Vec8<float> {
     }
 };
 
-__device__ __forceinline__ void ldg8f(const float* p, float f[8]) {
-    float4 a = __ldg(reinterpret_cast<const float4*>(p));
-    float4 b = __ldg(reinterpret_cast<const float4*>(p + 4));
-    f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
-    f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-
-// BatchNorm apply on one 8-channel vector, v = act(v·scale + shift + r): the arithmetic of tsb_bn_apply, also run by
-// the fused BN-apply + max-pool pass (resize_pool.cu) so that both give the same bits.
-template <bool kRelu, bool kRes>
-__device__ __forceinline__ void bn_act8(float (&v)[8], const float (&sc)[8], const float (&sh)[8], const float* r) {
-#pragma unroll
-    for (int k = 0; k < 8; ++k) v[k] = fmaf(v[k], sc[k], sh[k]);
-    if (kRes) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) v[k] += r[k];
-    }
-    if (kRelu) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) v[k] = fmaxf(v[k], 0.f);
-    }
-}
-
 // Grid-stride walk over (pixel, 8-channel group) pairs: i = pixel * C8 + c8 advances by `stride` per trip. The naive
 // `i % C8`, `i / C8` costs a 64-bit integer division per 16-byte vector (~100 issue slots — half the issue bandwidth of
 // a streaming kernel, ncu: 50 % issue-active on bn_apply); the walker divides once per thread.

@@ -148,6 +148,53 @@ __device__ __forceinline__ uint4 pack8(const float f[8]) {
     return u;
 }
 
+__device__ __forceinline__ void ldg8f(const float* p, float f[8]) {
+    float4 a = __ldg(reinterpret_cast<const float4*>(p));
+    float4 b = __ldg(reinterpret_cast<const float4*>(p + 4));
+    f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
+    f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+
+// BatchNorm apply on one 8-channel (N-channel) vector, v = act(v·scale + shift + r): the arithmetic of tsb_bn_apply,
+// also run by the fused BN-apply + max-pool pass (resize_pool.cu) and by the input prologue of the 1x1 convolutions
+// (tsb_conv1x1_bnrelu_*, 4 channels at a time) so that all give the same bits.
+template <bool kRelu, bool kRes, int N = 8>
+__device__ __forceinline__ void bn_act8(float (&v)[N], const float (&sc)[N], const float (&sh)[N], const float* r) {
+#pragma unroll
+    for (int k = 0; k < N; ++k) v[k] = fmaf(v[k], sc[k], sh[k]);
+    if (kRes) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) v[k] += r[k];
+    }
+    if (kRelu) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) v[k] = fmaxf(v[k], 0.f);
+    }
+}
+
+// Normalise-on-load of a landed 128B-swizzled activation box in shared memory (rows of 64 bf16 channels, 16-byte chunk
+// j of row r at chunk j ^ (r & 7)) by NT threads. A half-warp covers one 128-byte row, 8 bytes (4 channels) per thread:
+// thread rt takes byte 8 (rt & 15) of rows rt / 16 + (NT / 16) k, all of the same r & 7, hence the same 4 channels,
+// 8 j + 4 (rt & 1) with j = ((rt >> 1) & 7) ^ ((rt >> 4) & 7), whose scale / shift start at sc_p / sh_p. Rows at or past
+// `nrows` are TMA's zero fill past the last pixel and stay zero, so they add nothing to the GEMM. Four channels and one
+// row at a time: the kernels that call this hold their accumulators (and BN-statistics sums) in registers throughout.
+template <int ROWS, int NT>
+__device__ __forceinline__ void bnrelu_box(uint8_t* box, int nrows, int rt, const float* sc_p, const float* sh_p) {
+    constexpr int kRowStep = NT / 16;
+    const int c0 = 8 * (((rt >> 1) & 7) ^ ((rt >> 4) & 7)) + 4 * (rt & 1);
+    const float4 a = __ldg(reinterpret_cast<const float4*>(sc_p + c0)), b = __ldg(reinterpret_cast<const float4*>(sh_p + c0));
+    const float sc[4] = {a.x, a.y, a.z, a.w}, sh[4] = {b.x, b.y, b.z, b.w};
+    uint8_t* base = box + (rt >> 4) * 128 + (rt & 15) * 8;
+    const int end = min(nrows, ROWS);
+#pragma unroll 1
+    for (int r = rt >> 4; r < end; r += kRowStep, base += kRowStep * 128) {
+        const uint2 u = *reinterpret_cast<const uint2*>(base);
+        float v[4] = {bf16lo(u.x), bf16hi(u.x), bf16lo(u.y), bf16hi(u.y)};
+        bn_act8<true, false>(v, sc, sh, nullptr);
+        *reinterpret_cast<uint2*>(base) = make_uint2(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]));
+    }
+}
+
 // Generic element load/store as float for the two boundary dtypes.
 template <typename T> __device__ __forceinline__ float ld_as_float(const T* p);
 template <> __device__ __forceinline__ float ld_as_float<float>(const float* p) { return __ldg(p); }

@@ -6,3 +6,4 @@ from .psanet import PSANet, PointwiseSpatialAttention
 from .deeplabv3plus import DeepLabV3Plus, ASPP, Decoder
 from .encnet import EncNet, EncModule, EncHead
 from .ocnet import OCNet
+from .denseaspp import DenseASPP

@@ -587,10 +587,11 @@ def _bn_forward(raw, stats, count, gamma, beta, residual, running_mean, running_
     return _bn_apply(raw, aux, residual, relu), aux
 
 
-def _bn_backward(dy, y, raw, aux, gamma, beta, count, relu, has_res, grads, draw=None):
+def _bn_backward(dy, y, raw, aux, gamma, beta, count, relu, has_res, grads, draw=None, add=False):
     """the BatchNorm half of ConvBNActFn.backward: (draw, dres). raw / draw may be channel slices of wider NHWC buffers
     (draw None: a fresh dense one), aux the matching [4, K] slice. gamma / beta take their gradients through `grads`
-    (_ParamGrads): accumulated into their flat .grad views when direct, else handed to autograd."""
+    (_ParamGrads): accumulated into their flat .grad views when direct, else handed to autograd. add: draw is added to
+    (tsb_bn_bwd_apply_add) instead of overwritten."""
     N, K, P, Q = raw.shape
     dev = raw.device
     npix = N * P * Q
@@ -614,7 +615,8 @@ def _bn_backward(dy, y, raw, aux, gamma, beta, count, relu, has_res, grads, draw
     if draw is None:
         draw = nhwc_empty(N, K, P, Q, device=dev)
     dres = nhwc_empty(N, K, P, Q, device=dev) if has_res else None
-    call("tsb_bn_bwd_apply", ptr(dy), cs_of(dy), y_mask, ycs, ptr(raw), cs_of(raw), ptr(aux[0]), ptr(aux[1]), ptr(gamma),
+    call("tsb_bn_bwd_apply_add" if add else "tsb_bn_bwd_apply", ptr(dy), cs_of(dy), y_mask, ycs, ptr(raw), cs_of(raw),
+         ptr(aux[0]), ptr(aux[1]), ptr(gamma),
          ptr(red[0]), ptr(red[1]), count, int(relu), ptr(draw), cs_of(draw), ptr(dres), K if has_res else 0, npix, K,
          ptr(gamma.grad) if fold else None, ptr(beta.grad) if fold else None, ptr(aux[2]), ptr(aux[3]), stream())
     return draw, dres
@@ -710,6 +712,149 @@ class ConvBNActFn(torch.autograd.Function):
             dres = ctx.res_share.contribute(dres)
         dw_view, dgamma, dbeta = grads.result()
         return dx, dw_view, dgamma, dbeta, dres, None, None, None, None, None, None, None, None, None, None, None, None, None
+
+
+def conv1x1_bnrelu_fprop(x, aux, wb, K, bias=None, relu=False, stats=None):
+    """y = relu?(conv1x1(x̂, wb) + bias) with x̂ = bf16(relu(x·aux[2] + aux[3])) normalised in the conv's shared memory
+    (tsb_conv1x1_bnrelu_fprop): the pre-activation input of a DenseASPP block is never written. Optional BN statistics
+    of the rounded output into stats = [Σ; Σ²]."""
+    N, C, H, W = x.shape
+    shp = make_shape(N, H, W, C, K, 1, 1, 0, 1)
+    out = nhwc_empty(N, K, H, W, device=x.device)
+    s1, s2 = (None, None) if stats is None else (stats[0], stats[1])
+    conv_prof.launch(_conv_flops(shp), "tsb_conv1x1_bnrelu_fprop", ctypes.byref(shp), ptr(x), cs_of(x), ptr(aux[2]),
+                     ptr(aux[3]), ptr(wb), ptr(bias), int(relu), ptr(out), BF16, cs_of(out), ptr(s1), ptr(s2), *det_ws(),
+                     stream())
+    return out
+
+
+def conv1x1_bnrelu_wgrad(x, aux, dy, K, dw_krsc):
+    """dW += Σ dy ⊗ x̂ with the prologue of conv1x1_bnrelu_fprop (tsb_conv1x1_bnrelu_wgrad)"""
+    N, C, H, W = x.shape
+    shp = make_shape(N, H, W, C, K, 1, 1, 0, 1)
+    conv_prof.launch(_conv_flops(shp), "tsb_conv1x1_bnrelu_wgrad", ctypes.byref(shp), ptr(x), cs_of(x), ptr(aux[2]),
+                     ptr(aux[3]), ptr(dy), cs_of(dy), ptr(dw_krsc), *det_ws(), stream())
+
+
+def _slice_stats(stats, t):
+    """per-channel Σ / Σ² of the NHWC slice t into stats = [Σ; Σ²] (zeroed, a column range of a wider buffer), summed
+    over the SyncBN group"""
+    N, C, H, W = t.shape
+    call("tsb_bn_stats", ptr(t), cs_of(t), N * H * W, C, ptr(stats[0]), ptr(stats[1]), *det_ws(), stream())
+    if _sync["world"] > 1:
+        tmp = stats.contiguous()
+        _allreduce_stats(tmp)
+        stats.copy_(tmp)
+
+
+class DenseAsppFn(torch.autograd.Function):
+    """The densely connected atrous stack of DenseASPPModule in training: returns the concatenation
+    [a_{n-1} | ... | a_1 | a_0 | x] (one NHWC buffer; block i writes its slice in place and reads the suffix after it).
+
+    Forward, block i: pre_bn (i > 0) from the shared per-channel statistics of the buffer (one tsb_bn_stats per slice,
+    taken once), the 1x1 `reduce` conv reading relu(pre_bn(suffix)) through the conv's input prologue with the
+    BN-statistics epilogue (block 0: plain conv, its input is already post-ReLU), reduce's BatchNorm + ReLU, the dilated
+    3x3 conv with bias into the slice, Dropout2d on the slice. No normalised copy of the suffix is written or saved.
+
+    Backward walks the blocks from the last to the first over ONE bf16 gradient buffer of the concatenation (the
+    incoming gradient, added to in place): a block's slice gradient is complete when its turn comes, because only
+    later blocks read it. Block i > 0 hands its input gradient to the buffer's suffix through tsb_bn_bwd_apply_add
+    (the pre_bn backward, mask recomputed from scale / shift); block 0 through the accumulating dgrad."""
+
+    @staticmethod
+    def forward(ctx, x, mod, p_drop, *params):
+        blocks = mod.blocks
+        N, Cx, H, W = x.shape
+        dev = x.device
+        nb = len(blocks)
+        oc = blocks[0].conv.out_channels
+        Ct = Cx + nb * oc
+        npix = N * H * W
+        count = float(npix) * _sync["world"]
+        cat = nhwc_empty(N, Ct, H, W, device=dev)
+        cat[:, nb * oc:].copy_(x)
+        stats = zero_arena.take((2, Ct), dev)
+        _slice_stats(stats[:, nb * oc:], cat[:, nb * oc:])
+        saved, cfg = [], []
+        for i, blk in enumerate(blocks):
+            off = (nb - i) * oc
+            xin = cat[:, off:]
+            red, bn, conv = blk.reduce.conv, blk.reduce.bn, blk.conv
+            mid = red.out_channels
+            pre = None
+            if i > 0:
+                pb = blk.pre_bn
+                pre = torch.empty((4, Ct - off), dtype=torch.float32, device=dev)
+                _bn_finalize(pre, stats[:, off:], count, pb.weight, pb.bias, pb.running_mean, pb.running_var,
+                             float(pb.eps), float(pb.momentum if pb.momentum is not None else 0.1), True)
+            rs = zero_arena.take((2, mid), dev)
+            wb, _ = pack_cache.get(red.weight, False)
+            if pre is None:
+                raw = conv_fprop(xin, wb, mid, 1, 1, 0, 1, stats=rs)
+            else:
+                raw = conv1x1_bnrelu_fprop(xin, pre, wb, mid, stats=rs)
+            y, aux = _bn_forward(raw, rs, count, bn.weight, bn.bias, None, bn.running_mean, bn.running_var, True,
+                                 float(bn.eps), float(bn.momentum if bn.momentum is not None else 0.1), True)
+            d = conv.dilation[0]
+            wb3, _ = pack_cache.get(conv.weight, False)
+            sl = cat[:, off - oc:off]
+            conv_fprop(y, wb3, oc, 3, 1, d, d, bias=conv.bias, out=sl)
+            mask = None
+            if p_drop > 0:
+                mask = (torch.bernoulli(torch.full((N, oc, 1, 1), 1 - p_drop, device=dev)) / (1 - p_drop)).to(_BF)
+                sl.mul_(mask)
+            _slice_stats(stats[:, off - oc:off], sl)
+            saved += [raw, y, aux, pre if pre is not None else aux, mask if mask is not None else aux]
+            cfg.append((off, d, pre is not None, mask is not None))
+        ctx.save_for_backward(cat, *saved)
+        ctx.mod, ctx.cfg, ctx.count, ctx.oc = mod, cfg, count, oc
+        ctx.nparams = len(params)
+        return cat
+
+    @staticmethod
+    def backward(ctx, dcat):
+        cat, *saved = ctx.saved_tensors
+        mod, cfg, count, oc = ctx.mod, ctx.cfg, ctx.count, ctx.oc
+        blocks = mod.blocks
+        params = [p for blk in blocks for p in _dense_block_params(blk)]
+        grads = _ParamGrads(*params)
+        if not (dcat.dtype == _BF and dcat.stride(1) == 1 and cs_of(dcat) == cat.shape[1]):
+            dcat = to_nhwc(dcat)
+        N, _, H, W = cat.shape
+        npix = N * H * W
+        for i in reversed(range(len(blocks))):
+            blk = blocks[i]
+            raw, y, aux, pre, mask = saved[5 * i:5 * i + 5]
+            off, d, has_pre, has_mask = cfg[i]
+            xin = cat[:, off:]
+            red, bn, conv = blk.reduce.conv, blk.reduce.bn, blk.conv
+            mid = red.out_channels
+            g = dcat[:, off - oc:off]
+            if has_mask:
+                g.mul_(mask)
+            _bias_grad(grads, conv.bias, g, cs_of(g), npix, oc)
+            conv_wgrad(y, g, oc, 3, 1, d, d, grads.buffer(conv.weight, krsc=True))
+            _, wt3 = pack_cache.get(conv.weight, True)
+            dy = conv_dgrad(g, wt3, y.shape, oc, 3, 1, d, d)
+            draw, _ = _bn_backward(dy, y, raw, aux, bn.weight, bn.bias, count, True, False, grads)
+            _, wt1 = pack_cache.get(red.weight, True)
+            if not has_pre:
+                conv_wgrad(xin, draw, mid, 1, 1, 0, 1, grads.buffer(red.weight, krsc=True))
+                conv_dgrad(draw, wt1, xin.shape, mid, 1, 1, 0, 1, out=dcat[:, off:], accumulate=True)
+            else:
+                conv1x1_bnrelu_wgrad(xin, pre, draw, mid, grads.buffer(red.weight, krsc=True))
+                dxh = conv_dgrad(draw, wt1, xin.shape, mid, 1, 1, 0, 1)
+                pb = blk.pre_bn
+                _bn_backward(dxh, None, xin, pre, pb.weight, pb.bias, count, True, False, grads, draw=dcat[:, off:],
+                             add=True)
+        dx = dcat[:, len(blocks) * oc:] if ctx.needs_input_grad[0] else None
+        return (dx, None, None) + grads.result()
+
+
+def _dense_block_params(blk):
+    """the parameters of one DenseAsppBlock in DenseAsppFn's argument order"""
+    pre = [blk.pre_bn.weight, blk.pre_bn.bias] if blk.pre_bn is not None else []
+    return pre + [blk.reduce.conv.weight, blk.reduce.bn.weight, blk.reduce.bn.bias, blk.conv.weight, blk.conv.bias]
 
 
 class StemPairFn(torch.autograd.Function):

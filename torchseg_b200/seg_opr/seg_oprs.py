@@ -369,6 +369,79 @@ class BaseOCModule(nn.Module):
         return _dropout2d(out, self.conv_bn_dropout[1].p, self.training)
 
 
+class DenseAsppBlock(nn.Module):
+    """One pre-activation atrous layer of DenseASPP (Yang et al., CVPR 2018): pre_bn → ReLU → `reduce` (1x1 ConvBnRelu,
+    in → mid) → the dilated 3x3 `conv` (mid → out, bias) → Dropout2d(dropout). bn_start=False drops pre_bn (and its
+    ReLU): the first block's input is already post-ReLU. Children in checkpoint order: pre_bn, reduce, conv. The block
+    runs inside DenseASPPModule, which shares one concatenated buffer and its statistics between all blocks."""
+
+    def __init__(self, in_planes, mid_planes, out_planes, dilation, dropout=0.1, bn_start=True,
+                 norm_layer=nn.BatchNorm2d):
+        super(DenseAsppBlock, self).__init__()
+        self.pre_bn = norm_layer(in_planes) if bn_start else None
+        self.reduce = ConvBnRelu(in_planes, mid_planes, 1, 1, 0, has_bn=True, has_relu=True, has_bias=False,
+                                 norm_layer=norm_layer)
+        self.conv = nn.Conv2d(mid_planes, out_planes, 3, padding=dilation, dilation=dilation, bias=True)
+        self.dropout = dropout
+
+
+class DenseASPPModule(nn.Module):
+    """DenseASPP's densely connected atrous head: block i reads in_planes + i·out_planes channels, the input and every
+    earlier block's output, and the module returns [a_{n-1} | ... | a_1 | a_0 | x] (DenseASPP's `cat((new, feature))`
+    order; 2688 channels at the defaults). Every block's input is a contiguous suffix of ONE NHWC buffer that the 3x3
+    convs write their slices into, so there are no concatenation copies, and every pre_bn normalises that suffix in the
+    input prologue of its 1x1 conv (tsb_conv1x1_bnrelu_*): no normalised copy of it is ever written. The per-channel
+    batch statistics of the buffer are taken once per slice and shared by all pre_bn layers (each keeps its own γ, β
+    and running statistics). Training runs on ops.DenseAsppFn; eval applies pre_bn from its running statistics in the
+    same prologue and folds reduce's BatchNorm into the 1x1 conv (bias + ReLU epilogue). Block 0 has no pre_bn (its
+    input, layer4's output, is post-ReLU). Channel counts must be multiples of 64."""
+
+    def __init__(self, in_planes=2048, mid_planes=512, out_planes=128, rates=(3, 6, 12, 18, 24), dropout=0.1,
+                 norm_layer=nn.BatchNorm2d):
+        super(DenseASPPModule, self).__init__()
+        for c in (in_planes, mid_planes, out_planes):
+            if c % 64 != 0:
+                raise NotImplementedError("DenseASPPModule: channel counts must be multiples of 64 (got %d)" % c)
+        self.blocks = nn.ModuleList([
+            DenseAsppBlock(in_planes + i * out_planes, mid_planes, out_planes, d, dropout, bn_start=i > 0,
+                           norm_layer=norm_layer) for i, d in enumerate(rates)])
+        self.out_channels = in_planes + len(rates) * out_planes
+
+    def forward(self, x):
+        x = _as_act(x)
+        p = self.blocks[0].dropout if self.training else 0.0
+        if self.training:
+            params = [q for blk in self.blocks for q in ops._dense_block_params(blk)]
+            return ops.DenseAsppFn.apply(x, self, float(p), *params)
+        return self._infer(x)
+
+    @torch.no_grad()
+    def _infer(self, x):
+        """eval: running statistics, reduce's BatchNorm folded into its conv, no normalised copy"""
+        N, Cx, H, W = x.shape
+        nb, oc = len(self.blocks), self.blocks[0].conv.out_channels
+        Ct = Cx + nb * oc
+        cat = ops.nhwc_empty(N, Ct, H, W, device=x.device)
+        cat[:, nb * oc:].copy_(x)
+        for i, blk in enumerate(self.blocks):
+            off = (nb - i) * oc
+            xin = cat[:, off:]
+            red = blk.reduce
+            wb, bias = ops.fold_cache.get(red.conv.weight, red.bn, False)
+            if blk.pre_bn is None:
+                y = ops.conv_fprop_fused(xin, wb, red.conv.out_channels, 1, 1, 0, 1, bias, relu=True)
+            else:
+                pb = blk.pre_bn
+                pre = torch.empty((4, Ct - off), dtype=torch.float32, device=x.device)
+                ops._bn_finalize(pre, None, 1.0, pb.weight, pb.bias, pb.running_mean, pb.running_var, float(pb.eps),
+                                 0.0, False)
+                y = ops.conv1x1_bnrelu_fprop(xin, pre, wb, red.conv.out_channels, bias=bias, relu=True)
+            wb3, _ = ops.pack_cache.get(blk.conv.weight, False)
+            d = blk.conv.dilation[0]
+            ops.conv_fprop(y, wb3, oc, 3, 1, d, d, bias=blk.conv.bias, out=cat[:, off - oc:off])
+        return cat
+
+
 class ReluFn(torch.autograd.Function):
     """stand-alone ReLU on a small tensor (FFM squeeze branch [N,C,1,1], seg_oprs.py:224-226): expressed through
     tsb_bn_apply with scale 1 / shift 0 so it stays on the library path"""
