@@ -448,8 +448,7 @@ extern "C" int tsb_bn_stats(const void* x, int cs, long long npix, int C, float*
     TSB_REQUIRE(tsb_aligned16(ws), "tsb_bn_stats: ws must be 16B aligned");
     bn_stats_kernel<<<grid, kThreads, colred_smem(C8, 2), (cudaStream_t)stream>>>((const __nv_bfloat16*)x, cs, npix, C8, ws, ws + C, 2LL * C);
     TSB_CUDA_CHECK_LAUNCH("bn_stats");
-    int rc = tsb_det_reduce(sum, ws, grid, C, 2LL * C, (cudaStream_t)stream);
-    return rc ? rc : tsb_det_reduce(sumsq, ws + C, grid, C, 2LL * C, (cudaStream_t)stream);
+    return tsb_det_reduce_pair(sum, sumsq, ws, grid, C, (cudaStream_t)stream);
 }
 
 extern "C" int tsb_bn_finalize(const float* sum, const float* sumsq, double count, int C, const float* gamma,
@@ -497,8 +496,7 @@ extern "C" int tsb_bn_bwd_reduce(const void* dy, int dycs, const void* y, int yc
     if (mode == 0) L(0); else if (mode == 1) L(1); else L(2);
 #undef L
     TSB_CUDA_CHECK_LAUNCH("bn_bwd_reduce");
-    int rc = tsb_det_reduce(sum_dz, ws, grid, C, 2LL * C, st);
-    return rc ? rc : tsb_det_reduce(sum_dz_xhat, ws + C, grid, C, 2LL * C, st);
+    return tsb_det_reduce_pair(sum_dz, sum_dz_xhat, ws, grid, C, st);
 }
 
 template <bool kAdd>

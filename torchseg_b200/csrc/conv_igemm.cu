@@ -335,9 +335,8 @@ static int adjoint_launches(const tsb_conv_shape* s, const void* act, int acs, c
         slots += used;
     }
     if (epi.sum == nullptr || slots == 0) return TSB_OK;
-    const int rc = tsb_det_reduce(epi.sum, epi.ws, slots, s->C, 2LL * s->C, st);
     // the sumsq slots follow the sum slots of the same CTA: a stride of 2·C between slots
-    return rc ? rc : tsb_det_reduce(epi.sumsq, epi.ws + s->C, slots, s->C, 2LL * s->C, st);
+    return tsb_det_reduce_pair(epi.sum, epi.sumsq, epi.ws, slots, s->C, st);
 }
 
 extern "C" int tsb_conv2d_dgrad(const tsb_conv_shape* s, const void* dy, int dycs, const void* wt, void* dx, int dxcs,

@@ -313,10 +313,8 @@ int launch(const Desc& d, cudaStream_t st, int* stat_slots) {
                          : (resident ? launch_v2<128, true>(prm, grid_x, n_tiles, smem, st) : launch_v2<128, false>(prm, grid_x, n_tiles, smem, st));
     if (rc2 || d.sum == nullptr) return rc2;
     if (stat_slots != nullptr) { *stat_slots = grid_x; return TSB_OK; }
-    rc2 = tsb_det_reduce(d.sum, prm.part, grid_x, d.k_real, 2LL * d.k_real, st);
-    if (rc2) return rc2;
     // the sumsq slots follow the sum slots of the same CTA: a stride of 2·k_real between CTAs
-    return tsb_det_reduce(d.sumsq, prm.part + d.k_real, grid_x, d.k_real, 2LL * d.k_real, st);
+    return tsb_det_reduce_pair(d.sum, d.sumsq, prm.part, grid_x, d.k_real, st);
 }
 
 

@@ -18,8 +18,13 @@ int tsb_ensure_dyn_smem(const void* func, size_t bytes);   // per-(device, funct
 // Deterministic cross-CTA sums. A kernel that would add per-CTA partials into one output with float atomics (whose
 // order, hence rounding, changes from run to run) instead stores partial b into slot b of the caller's workspace
 // (`ws`, `ws_floats` of the entry point); tsb_det_reduce then adds sum_b slot[b][i] (b in increasing order) to out[i].
-// Slot b of the partials starts at parts + b * stride.
-int tsb_det_reduce(float* out, const float* parts, int nparts, long long n, long long stride, cudaStream_t st);
+// Slot b of the partials starts at parts + b * stride. C linkage (not part of include/tsb.h) so that tests can call the
+// ordered sum on its own.
+extern "C" int tsb_det_reduce(float* out, const float* parts, int nparts, long long n, long long stride, cudaStream_t st);
+// The Σ / Σ² (Σdz / Σdz·x̂) pair of a statistics reduction: slot b holds [2][C] at parts + 2C·b, the first half summed
+// into out_a, the second into out_b. One launch over 2C outputs when out_b == out_a + C (the two rows of one [2, C]
+// tensor), else two.
+int tsb_det_reduce_pair(float* out_a, float* out_b, const float* parts, int nparts, long long C, cudaStream_t st);
 
 #define TSB_FAIL(code, ...)            \
     do {                               \
