@@ -15,6 +15,7 @@ import torch
 import torch.nn.functional as F
 
 from util import rel_err, norm_err, make_labels, bf16_round
+from net_checks import randomize_bn
 
 pytestmark = pytest.mark.gpu
 BN = torch.nn.BatchNorm2d
@@ -479,14 +480,7 @@ def test_bisenet_eval_forward_matches_oracle(cuda):
     torch.manual_seed(11)
     model = BiSeNet(19, False, None, None, BN)
     init_weight(model.business_layer, torch.nn.init.kaiming_normal_, BN, 1e-5, 0.1, mode='fan_in', nonlinearity='relu')
-    g = torch.Generator().manual_seed(12)
-    with torch.no_grad():   # non-trivial running statistics and affine parameters
-        for m in model.modules():
-            if isinstance(m, BN):
-                m.running_mean.copy_(torch.randn(m.running_mean.shape, generator=g) * 0.2)
-                m.running_var.copy_(torch.rand(m.running_var.shape, generator=g) * 1.5 + 0.5)
-                m.weight.copy_(torch.rand(m.weight.shape, generator=g) + 0.5)
-                m.bias.copy_(torch.randn(m.bias.shape, generator=g) * 0.1)
+    g = randomize_bn(model, 12)
     sd = {k: v.detach().clone() for k, v in model.state_dict().items()}
     x = torch.randn(2, 3, 128, 160, generator=g)
     tr.set_bf16_emulation(True)
@@ -520,14 +514,7 @@ def test_bisenet_eval_bn_folding_matches_unfolded(cuda):
     torch.manual_seed(13)
     model = BiSeNet(19, False, None, None, BN)
     init_weight(model.business_layer, torch.nn.init.kaiming_normal_, BN, 1e-5, 0.1, mode='fan_in', nonlinearity='relu')
-    g = torch.Generator().manual_seed(14)
-    with torch.no_grad():
-        for m in model.modules():
-            if isinstance(m, BN):
-                m.running_mean.copy_(torch.randn(m.running_mean.shape, generator=g) * 0.2)
-                m.running_var.copy_(torch.rand(m.running_var.shape, generator=g) * 1.5 + 0.5)
-                m.weight.copy_(torch.rand(m.weight.shape, generator=g) + 0.5)
-                m.bias.copy_(torch.randn(m.bias.shape, generator=g) * 0.1)
+    g = randomize_bn(model, 14)
     model.to(cuda)
     torchseg_b200.prepare_model(model)
     model.eval()

@@ -17,6 +17,7 @@ import torch
 import torch.nn.functional as F
 
 from util import rel_err, norm_err, make_labels, bf16_round
+from net_checks import randomize_bn
 
 pytestmark = pytest.mark.gpu
 BN = torch.nn.BatchNorm2d
@@ -70,19 +71,6 @@ def _groups(model):
     for m in model.business_layer:
         groups = group_weight(groups, m, BN, 1e-1)
     return groups
-
-
-def _random_bn(model, seed):
-    """non-trivial running statistics and affine parameters for the eval tests"""
-    g = torch.Generator().manual_seed(seed)
-    with torch.no_grad():
-        for m in model.modules():
-            if isinstance(m, BN):
-                m.running_mean.copy_(torch.randn(m.running_mean.shape, generator=g) * 0.2)
-                m.running_var.copy_(torch.rand(m.running_var.shape, generator=g) * 1.5 + 0.5)
-                m.weight.copy_(torch.rand(m.weight.shape, generator=g) + 0.5)
-                m.bias.copy_(torch.randn(m.bias.shape, generator=g) * 0.1)
-    return g
 
 
 # ------------------------------------------------------------------------------------------ the loss at label resolution
@@ -331,7 +319,7 @@ def test_eval_forward_matches_oracle(cuda, line):
     torch.manual_seed(11)
     model = _net(line, False)
     init_weight(model.business_layer, torch.nn.init.kaiming_normal_, BN, 1e-5, 0.1, mode='fan_in', nonlinearity='relu')
-    g = _random_bn(model, 12)
+    g = randomize_bn(model, 12)
     sd = {k: v.detach().clone() for k, v in model.state_dict().items()}
     H, W = 128, 192
     x = torch.randn(2, 3, H, W, generator=g)
@@ -360,7 +348,7 @@ def test_training_checkpoint_loads_into_eval_network(cuda, line):
     from torchseg_b200.utils.pyt_utils import load_model
     torch.manual_seed(21)
     train_net = _net(line, True)
-    g = _random_bn(train_net, 22)
+    g = randomize_bn(train_net, 22)
     ckpt = {k: v.detach().clone() for k, v in train_net.state_dict().items()}
     eval_net = load_model(_net(line, False), ckpt)
     x = torch.randn(2, 3, 128, 256, generator=g).to(cuda)
@@ -383,7 +371,7 @@ def test_eval_batch1_graph_matches_eager(cuda, line):
     import torchseg_b200
     torch.manual_seed(31)
     model = _net(line, False)
-    g = _random_bn(model, 32)
+    g = randomize_bn(model, 32)
     model.to(cuda)
     torchseg_b200.prepare_model(model)
     model.eval()

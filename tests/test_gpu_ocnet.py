@@ -7,6 +7,8 @@ import pytest
 import torch
 
 from util import norm_err, bf16_round
+from net_checks import (check_step_vs_oracle, check_train_reproducible, check_graphed_matches_eager,
+                        check_eval_vs_oracle_and_sliding)
 
 pytestmark = pytest.mark.gpu
 BN = torch.nn.BatchNorm2d
@@ -327,39 +329,8 @@ def test_ocnet_step_matches_oracle(cuda):
     import ocnet_oracle as tr
     model, sd, x, y = _build(cuda)
     assert float(model.context[1].stages[0].W.weight.abs().max()) > 0
-    for k in sd:
-        if sd[k].is_floating_point() and "running" not in k:
-            sd[k].requires_grad_(True)
-    loss_ref, _ = tr.ocnet_loss(x, y, sd)
-    loss_ref.backward()
-    ref = {k: v.grad.clone() for k, v in sd.items() if v.grad is not None}
-    for v in sd.values():
-        v.grad = None
-    tr.set_bf16_emulation(True)
-    try:
-        loss_emu, _ = tr.ocnet_loss(x, y, sd)
-        loss_emu.backward()
-    finally:
-        tr.set_bf16_emulation(False)
-    emu = {k: v.grad.clone() for k, v in sd.items() if v.grad is not None}
-    loss = model(x.to(cuda), y.to(cuda))
-    loss.backward()
-    torch.cuda.synchronize()
-    assert abs(loss.item() - loss_ref.item()) < 1e-2 * abs(loss_ref.item()), (loss.item(), loss_ref.item())
-    P = dict(model.named_parameters())
-    for n in ("cls.weight", "cls.bias", "aux_layer.2.weight", "aux_layer.2.bias"):
-        a, b = P[n].grad.float().cpu().reshape(-1), ref[n].reshape(-1)
-        cos = float(torch.dot(a, b) / (a.norm() * b.norm()).clamp_min(1e-30))
-        assert cos > 0.9, (n, cos)
-    bad = []
-    for n, p in P.items():
-        assert bool(torch.isfinite(p.grad).all()), n
-        if p.dim() >= 2:
-            gn = float(p.grad.float().norm().cpu())
-            r_emu, r_ref = (gn / float(o[n].norm().clamp_min(1e-30)) for o in (emu, ref))
-            if not (0.75 < r_emu < 1.33 or 0.75 < r_ref < 1.33):
-                bad.append((n, round(r_emu, 3), round(r_ref, 3)))
-    assert not bad, "|grad| / |emulating oracle's|, / |fp32 oracle's|: %s" % bad[:10]
+    check_step_vs_oracle(cuda, model, sd, x, y, tr.ocnet_loss,
+                         ("cls.weight", "cls.bias", "aux_layer.2.weight", "aux_layer.2.bias"))
 
 
 def _groups(model):
@@ -372,76 +343,29 @@ def _groups(model):
 
 def test_ocnet_train_steps_decrease_loss_and_reproduce(cuda):
     from torchseg_b200 import optim
-    runs = []
-    for _ in range(2):
+
+    def make():
         model, _, x, y = _build(cuda, N=2, H=97, W=113, seed=3)
-        opt = optim.SGD(_groups(model), lr=1e-2, momentum=0.9, weight_decay=5e-4)
-        xs, ys = x.to(cuda), y.to(cuda)
-        losses = []
-        for _ in range(5):
-            opt.zero_grad()
-            loss = model(xs, ys)
-            loss.backward()
-            opt.step()
-            losses.append(loss.detach().clone())
-        torch.cuda.synchronize()
-        runs.append((losses, [p.detach().clone() for p in model.parameters()]))
-        del model, opt
-    (l0, p0), (l1, p1) = runs
-    vals = [float(l) for l in l0]
-    assert all(v == v for v in vals) and vals[-1] < vals[0], vals
-    for a, b in zip(l0, l1):
-        assert torch.equal(a.view(torch.int32), b.view(torch.int32)), (vals, [float(l) for l in l1])
-    for a, b in zip(p0, p1):
-        assert torch.equal(a.view(torch.int32), b.view(torch.int32))
+        return model, optim.SGD(_groups(model), lr=1e-2, momentum=0.9, weight_decay=5e-4), x.to(cuda), y.to(cuda)
+
+    check_train_reproducible(make)
 
 
 def test_ocnet_graphed_step_matches_eager_and_runs_no_aten_gemm(cuda):
-    from torch.profiler import ProfilerActivity, profile
     from torchseg_b200 import optim
-    from torchseg_b200.engine.graph import GraphedTrainStep
     from torchseg_b200.seg_opr.loss_opr import ProbOhemCrossEntropy2d
-    torch.cuda.set_stream(torch.cuda.Stream())
-    try:
-        def make():
-            crit = ProbOhemCrossEntropy2d(255, thresh=0.7, min_kept=2 * 96 * 96 // 16)
-            model, _, x, y = _build(cuda, N=2, H=96, W=96, seed=7, criterion=crit)
-            return model, optim.SGD(_groups(model), lr=1e-2, momentum=0.9, weight_decay=5e-4), x.to(cuda), y.to(cuda)
 
-        model, opt, x, y = make()
-        eager = []
-        for i in range(4):
-            opt.zero_grad()
-            if i == 3:
-                with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
-                    loss = model(x, y)
-                    loss.backward()
-                    torch.cuda.synchronize()
-            else:
-                loss = model(x, y)
-                loss.backward()
-            opt.step()
-            eager.append(loss.detach().clone())
-        names = [e.name for e in prof.events()]
-        aten = ("aten::conv", "aten::_conv", "aten::cudnn", "aten::mm", "aten::bmm", "aten::baddbmm", "aten::matmul",
-                "aten::addmm", "aten::linear", "aten::scaled_dot_product", "aten::_scaled_dot_product",
-                "aten::_flash_attention", "aten::_efficient_attention", "aten::softmax", "aten::_softmax")
-        bad = [n for n in names if n.startswith(aten) or any(t in n.lower() for t in ("cudnn", "cublas", "cutlass", "xmma",
-                                                                                      "gemv", "flash", "fmha"))]
-        assert not bad, sorted(set(bad))[:10]
-        for k in ("attn_fwd_kernel", "attn_bwd_kv_kernel", "attn_bwd_q_kernel", "attn_delta_kernel"):
-            assert any(k in n for n in names), k
-        model, opt, x, y = make()
-        step = GraphedTrainStep(model, opt, [x, y], warmup=2)
-        assert step.graph is not None, step.error
-        graphed = [step(x, y).detach().clone() for _ in range(2)]
-        torch.cuda.synchronize()
-        for a, b in zip(eager[2:], graphed):
-            assert torch.equal(a.view(torch.int32), b.view(torch.int32)), ([float(e) for e in eager],
-                                                                           [float(e) for e in graphed])
-        step.release()
-    finally:
-        torch.cuda.set_stream(torch.cuda.default_stream())
+    def make():
+        crit = ProbOhemCrossEntropy2d(255, thresh=0.7, min_kept=2 * 96 * 96 // 16)
+        model, _, x, y = _build(cuda, N=2, H=96, W=96, seed=7, criterion=crit)
+        return model, optim.SGD(_groups(model), lr=1e-2, momentum=0.9, weight_decay=5e-4), x.to(cuda), y.to(cuda)
+
+    check_graphed_matches_eager(make, kernels=("attn_fwd_kernel", "attn_bwd_kv_kernel", "attn_bwd_q_kernel",
+                                               "attn_delta_kernel"),
+                                extra_aten=("aten::scaled_dot_product", "aten::_scaled_dot_product",
+                                            "aten::_flash_attention", "aten::_efficient_attention", "aten::softmax",
+                                            "aten::_softmax"),
+                                extra_libs=("flash", "fmha"))
 
 
 def test_ocnet_full_size_step_runs(cuda):
@@ -462,44 +386,6 @@ def test_ocnet_full_size_step_runs(cuda):
 
 
 def test_ocnet_eval_forward_matches_oracle_and_sliding_eval(cuda):
-    import numpy as np
-    import torchseg_b200
-    from torchseg_b200.engine.evaluator import Evaluator
     from torchseg_b200.networks import OCNet
-    from torchseg_b200.utils.init_func import init_weight
     import ocnet_oracle as tr
-    torch.manual_seed(11)
-    model = OCNet(19, None)
-    init_weight(model.business_layer, torch.nn.init.kaiming_normal_, BN, 1e-5, 0.1, mode='fan_in', nonlinearity='relu')
-    g = torch.Generator().manual_seed(12)
-    with torch.no_grad():
-        for m in model.modules():
-            if isinstance(m, BN):
-                m.running_mean.copy_(torch.randn(m.running_mean.shape, generator=g) * 0.2)
-                m.running_var.copy_(torch.rand(m.running_var.shape, generator=g) * 1.5 + 0.5)
-                m.weight.copy_(torch.rand(m.weight.shape, generator=g) + 0.5)
-                m.bias.copy_(torch.randn(m.bias.shape, generator=g) * 0.1)
-    sd = {k: v.detach().clone() for k, v in model.state_dict().items()}
-    x = torch.randn(2, 3, 96, 130, generator=g)
-    tr.set_bf16_emulation(True)
-    try:
-        with torch.no_grad():
-            ref = tr.ocnet_eval(x, sd)
-    finally:
-        tr.set_bf16_emulation(False)
-    model.to(cuda)
-    torchseg_b200.prepare_model(model)
-    model.eval()
-    with torch.no_grad():
-        out = model(x.to(cuda))
-    assert tuple(out.shape) == (2, 19, 96, 130) and out.dtype == torch.float32
-    assert norm_err(out, ref) < 2e-2, norm_err(out, ref)
-    assert (out.argmax(1).cpu() == ref.argmax(1)).float().mean() > 0.97
-    ev = Evaluator(dataset=None, class_num=19, image_mean=np.array([0.485, 0.456, 0.406]),
-                   image_std=np.array([0.229, 0.224, 0.225]), network=None, multi_scales=[0.75, 1.0], is_flip=True,
-                   devices=[0], crop_batch=2)
-    ev.val_func = model
-    img = np.random.default_rng(0).integers(0, 256, (150, 171, 3), dtype=np.uint8)
-    host = ev.sliding_eval(img, 128, 2 / 3.0, cuda)
-    dev = ev.sliding_eval_device(img, 128, 2 / 3.0, cuda)
-    assert np.array_equal(dev.cpu().numpy(), host)
+    check_eval_vs_oracle_and_sliding(cuda, lambda: OCNet(19, None), tr.ocnet_eval, 19)
