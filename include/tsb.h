@@ -395,10 +395,12 @@ int tsb_se_loss_fwd_bwd(const int64_t* labels, int B, long long HW, const float*
 
 /* ---- OCNet: fused self-attention over the pixels of each image ------------------------------------------------------
  *   o[b,i,:] = Σ_j softmax_j(scale · q[b,i,:]·k[b,j,:]) · v[b,j,:]     b < B, i, j < N
- * q, k, v, o, dout and the gradients are bf16 rows [B·N][d] (row b·N + i) with channel stride *cs: multiples of 8 and
- * >= d, every pointer 16-byte aligned. Only d_k = d_v = 256 is implemented (anything else is TSB_ERR_UNSUPPORTED);
- * B·N < 2^31, B <= 65535, 0 < scale < inf. S = q·kᵀ and its softmax are never written to global memory; every output
- * element has one writer, so results are bit-identical from run to run. */
+ * q, k, v, o, dout and the gradients are bf16 rows [B·N][d] (row b·N + i) with channel stride *cs: multiples of 8, every
+ * pointer 16-byte aligned; q, k, dq and dk have d = d_k (stride >= d_k), v, o, dout and dv have d = d_v (stride >= d_v).
+ * Two (d_k, d_v) pairs are implemented: (256, 256) (OCNet) and (64, 512) (DANet's position attention, whose value side
+ * runs in two 256-channel slices); anything else is TSB_ERR_UNSUPPORTED. B·N < 2^31, B <= 65535, 0 < scale < inf.
+ * S = q·kᵀ and its softmax are never written to global memory; every output element has one writer, so results are
+ * bit-identical from run to run. */
 /* lse: fp32 [B·N], m_i + log Σ_j exp(scale·s_ij − m_i) per query row (the softmax normaliser), or NULL (inference). */
 int tsb_attention_fwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, void* o, int ocs, float* lse,
                       int B, int N, int dim_k, int dim_v, float scale, tsb_stream_t stream);
@@ -409,6 +411,25 @@ int tsb_attention_bwd(const void* q, int qcs, const void* k, int kcs, const void
                       const void* dout, int docs, const float* lse, float* delta_ws, void* dq, int dqcs, void* dk,
                       int dkcs, void* dv, int dvcs, int dq_accumulate, int B, int N, int dim_k, int dim_v, float scale,
                       tsb_stream_t stream);
+
+/* ---- DANet: channel attention (CAM) and the learnable-gamma residual --------------------------------------------------
+ * CAM per image b with C channels: E = X Xᵀ (fp32 [C][C], tsb_conv2d_wgrad with dy = x), A = softmax_row(rowmax(E) − E),
+ * out = A X (a 1x1 tsb_conv2d_fprop with A as the weight). E, dA: fp32 [B][C][C]; A, G: bf16 [B][C][C], row-major.
+ * fwd: A from E; t_ij = rowmax_i − E_ij in fp32 as written, exp(t_ij − max_j t_ij) normalised over the row, rounded once.
+ * bwd: G = −(dẼ + dẼᵀ), dẼ = A ∘ (dA − Σ_j A_ij dA_ij) (the gradient through rowmax, zero in exact arithmetic, is
+ *      dropped). G is exactly symmetric; dX += G·X is then a tsb_conv2d_dgrad with accumulate = 1 and G as the pack.
+ *      rowdot_ws: fp32 [B·C] scratch. B <= 65535, C·C <= 2^30. */
+int tsb_chan_attn_softmax_fwd(const float* E, void* A, int B, int C, tsb_stream_t stream);
+int tsb_chan_attn_softmax_bwd(const void* A, const float* dA, float* rowdot_ws, void* G, int B, int C,
+                              tsb_stream_t stream);
+/* y = bf16(fmaf(gamma, o, x)) over npix pixels of C channels (DANet's `gamma * out + x`), gamma read on the device from
+ * the fp32 parameter (no host synchronisation). bwd: dout = bf16(gamma · dy), and dgamma (fp32 [1]) += Σ dy·o, the
+ * per-CTA partials summed in slot order through the workspace (ws, ws_floats). C % 8 == 0; x, o, y, dy, dout bf16 NHWC,
+ * 16-byte aligned, channel strides multiples of 8 and >= C. */
+int tsb_gamma_residual_fwd(const void* x, int xcs, const void* o, int ocs, const float* gamma, void* y, int ycs,
+                           long long npix, int C, tsb_stream_t stream);
+int tsb_gamma_residual_bwd(const void* dy, int dycs, const void* o, int ocs, const float* gamma, void* dout, int docs,
+                           float* dgamma, long long npix, int C, float* ws, long long ws_floats, tsb_stream_t stream);
 
 /* ================================================================================================
  * Optimiser — fused flat-buffer momentum SGD replacing torch.optim.SGD.step (train.py:86-89,142) with

@@ -99,6 +99,10 @@ _SIGS = {
     "tsb_se_loss_fwd_bwd": [P, I, L, P, I, I, P, P, P, I, P],
     "tsb_attention_fwd": [P, I, P, I, P, I, P, I, P, I, I, I, I, F, P],
     "tsb_attention_bwd": [P, I, P, I, P, I, P, I, P, I, P, P, P, I, P, I, P, I, I, I, I, I, I, F, P],
+    "tsb_chan_attn_softmax_fwd": [P, P, I, I, P],
+    "tsb_chan_attn_softmax_bwd": [P, P, P, P, I, I, P],
+    "tsb_gamma_residual_fwd": [P, I, P, I, P, P, I, L, I, P],
+    "tsb_gamma_residual_bwd": [P, I, P, I, P, P, I, P, L, I, P, L, P],
 }
 EXPORTS = sorted(list(_SIGS) + ["tsb_last_error", "tsb_version", "tsb_launch_count", "tsb_p2p_buffer_bytes", "tsb_edge_labels_workspace_bytes"])
 

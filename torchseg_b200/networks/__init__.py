@@ -7,3 +7,4 @@ from .deeplabv3plus import DeepLabV3Plus, ASPP, Decoder
 from .encnet import EncNet, EncModule, EncHead
 from .ocnet import OCNet
 from .denseaspp import DenseASPP
+from .danet import DANet, DANetHead

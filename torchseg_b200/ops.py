@@ -1200,11 +1200,12 @@ class SELossFn(torch.autograd.Function):
 # OCNet: dense self-attention over the pixels of each image
 # --------------------------------------------------------------------------------------------------
 class AttentionFn(torch.autograd.Function):
-    """o = softmax(scale · q kᵀ) v over the h·w pixels of each image (OCNet's object context), fused on
-    tsb_attention_{fwd,bwd}: the [N, N] scores never reach memory, and the backward recomputes them from the saved
-    q, k, v, o and the per-row log-sum-exp (O(N·d) saved, not O(N²)). q, k, v: bf16 NHWC [B, 256, h, w] (channel slices
-    allowed). k = None means k is q (OCNet's shared f_key): the backward then returns dQ + dK as q's gradient, formed by
-    the kernels in one buffer. Without any input needing a gradient the forward skips the log-sum-exp."""
+    """o = softmax(scale · q kᵀ) v over the h·w pixels of each image (OCNet's object context, DANet's position
+    attention), fused on tsb_attention_{fwd,bwd}: the [N, N] scores never reach memory, and the backward recomputes them
+    from the saved q, k, v, o and the per-row log-sum-exp (O(N·d) saved, not O(N²)). q, k: bf16 NHWC [B, d_k, h, w],
+    v: [B, d_v, h, w] (channel slices allowed), (d_k, d_v) = (256, 256) or (64, 512). k = None means k is q (OCNet's
+    shared f_key): the backward then returns dQ + dK as q's gradient, formed by the kernels in one buffer. Without any
+    input needing a gradient the forward skips the log-sum-exp."""
 
     @staticmethod
     def forward(ctx, q, k, v, scale):
@@ -1238,6 +1239,81 @@ class AttentionFn(torch.autograd.Function):
              cs_of(do), ptr(lse), ptr(delta), ptr(dq), dk, ptr(dkt), dk, ptr(dvt), dv, int(shared), B, h * w, dk, dv,
              scale, stream())
         return dq, (None if shared else dkt), dvt, None
+
+
+# --------------------------------------------------------------------------------------------------
+# DANet: channel attention and the learnable-gamma residual
+# --------------------------------------------------------------------------------------------------
+class ChannelAttentionFn(torch.autograd.Function):
+    """DANet's channel attention before its residual: out = A X with A = softmax_row(rowmax(E) − E) and E = X Xᵀ over
+    the C channels of each image (X is [C, h·w]). x: bf16 NHWC [B, C, h, w], C a multiple of 64 (channel slices
+    allowed). The products run on the wgmma conv kernels, one launch per image: E is a wgrad with dy = x, A X a 1x1
+    fprop with A as the weight; backward, dA is a wgrad, Aᵀ·dout a dgrad with the transposed A, and the Gram term
+    X·(dE + dEᵀ) a dgrad with accumulate = 1 whose operand is symmetric. The soft-max and its gradient run on
+    tsb_chan_attn_softmax_{fwd,bwd}. Saves x and A (bf16 [B, C, C]); E and dA are fp32."""
+
+    @staticmethod
+    def forward(ctx, x):
+        B, C, h, w = x.shape
+        assert C % 64 == 0, "channel attention needs a multiple of 64 channels"
+        dev = x.device
+        E = torch.zeros((B, C, C), dtype=torch.float32, device=dev)
+        for n in range(B):
+            conv_wgrad(x[n:n + 1], x[n:n + 1], C, 1, 1, 0, 1, E[n])
+        A = torch.empty((B, C, C), dtype=_BF, device=dev)
+        call("tsb_chan_attn_softmax_fwd", ptr(E), ptr(A), B, C, stream())
+        out = nhwc_empty(B, C, h, w, device=dev)
+        for n in range(B):
+            conv_fprop(x[n:n + 1], A[n], C, 1, 1, 0, 1, out=out[n:n + 1])
+        if ctx.needs_input_grad[0]:
+            ctx.save_for_backward(x, A)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        x, A = ctx.saved_tensors
+        B, C, h, w = x.shape
+        dev = x.device
+        dout = as_nhwc_bf16(dout)
+        dA = torch.zeros((B, C, C), dtype=torch.float32, device=dev)
+        At = torch.empty((C, C), dtype=_BF, device=dev)
+        dx = nhwc_empty(B, C, h, w, device=dev)
+        for n in range(B):
+            conv_wgrad(x[n:n + 1], dout[n:n + 1], C, 1, 1, 0, 1, dA[n])
+            call("tsb_transpose_pad", ptr(A[n]), BF16, C, ptr(At), C, C, C, C, stream())
+            conv_dgrad(dout[n:n + 1], At, (1, C, h, w), C, 1, 1, 0, 1, out=dx[n:n + 1])
+        G = torch.empty((B, C, C), dtype=_BF, device=dev)
+        rowdot = torch.empty((B, C), dtype=torch.float32, device=dev)
+        call("tsb_chan_attn_softmax_bwd", ptr(A), ptr(dA), ptr(rowdot), ptr(G), B, C, stream())
+        for n in range(B):
+            conv_dgrad(x[n:n + 1], G[n], (1, C, h, w), C, 1, 1, 0, 1, out=dx[n:n + 1], accumulate=True)
+        return dx
+
+
+class GammaResidualFn(torch.autograd.Function):
+    """y = gamma · o + x, DANet's PAM / CAM output with gamma a learnable fp32 scalar [1], on
+    tsb_gamma_residual_{fwd,bwd}. gamma is read on the device (no host synchronisation, so the step stays one graph);
+    dgamma = Σ dy·o is summed in a fixed order. x, o: bf16 NHWC of one shape."""
+
+    @staticmethod
+    def forward(ctx, x, o, gamma):
+        N, C, H, W = x.shape
+        assert tuple(o.shape) == tuple(x.shape) and gamma.dtype == torch.float32 and gamma.numel() == 1
+        y = nhwc_empty(N, C, H, W, device=x.device)
+        call("tsb_gamma_residual_fwd", ptr(x), cs_of(x), ptr(o), cs_of(o), ptr(gamma), ptr(y), C, N * H * W, C, stream())
+        ctx.save_for_backward(o, gamma)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        o, gamma = ctx.saved_tensors
+        N, C, H, W = o.shape
+        dy = as_nhwc_bf16(dy)
+        do = nhwc_empty(N, C, H, W, device=o.device)
+        grads = _ParamGrads(gamma)
+        call("tsb_gamma_residual_bwd", ptr(dy), cs_of(dy), ptr(o), cs_of(o), ptr(gamma), ptr(do), C,
+             ptr(grads.buffer(gamma)), N * H * W, C, *det_ws(), stream())
+        return (dy, do) + grads.result()
 
 
 # --------------------------------------------------------------------------------------------------

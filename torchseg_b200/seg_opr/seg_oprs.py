@@ -442,6 +442,41 @@ class DenseASPPModule(nn.Module):
         return cat
 
 
+class PAM_Module(nn.Module):
+    """DANet's position attention module (Fu et al., "Dual Attention Network for Scene Segmentation", `PAM_Module`):
+    query_conv and key_conv are 1x1 convs in_dim → in_dim/8 with bias, value_conv a 1x1 conv in_dim → in_dim with bias,
+    gamma a zero-initialised scalar. forward(x) = gamma · softmax(q kᵀ) v + x over the h·w pixels of each image, with
+    no 1/√d scale; the attention runs on ops.AttentionFn at (d_k, d_v) = (in_dim/8, in_dim), which the kernels implement
+    for in_dim = 512."""
+
+    def __init__(self, in_dim):
+        super(PAM_Module, self).__init__()
+        self.query_conv = nn.Conv2d(in_dim, in_dim // 8, kernel_size=1)
+        self.key_conv = nn.Conv2d(in_dim, in_dim // 8, kernel_size=1)
+        self.value_conv = nn.Conv2d(in_dim, in_dim, kernel_size=1)
+        self.gamma = nn.Parameter(torch.zeros(1))
+
+    def forward(self, x):
+        x = _as_act(x)
+        out = ops.AttentionFn.apply(conv_plain(x, self.query_conv), conv_plain(x, self.key_conv),
+                                    conv_plain(x, self.value_conv), 1.0)
+        return ops.GammaResidualFn.apply(x, out, self.gamma)
+
+
+class CAM_Module(nn.Module):
+    """DANet's channel attention module (`CAM_Module`): forward(x) = gamma · A X + x with A = softmax_row(rowmax(E) − E),
+    E = X Xᵀ over the C channels of each image (X is [C, h·w]), gamma a zero-initialised scalar; no convolutions. On
+    ops.ChannelAttentionFn and ops.GammaResidualFn."""
+
+    def __init__(self, in_dim):
+        super(CAM_Module, self).__init__()
+        self.gamma = nn.Parameter(torch.zeros(1))
+
+    def forward(self, x):
+        x = _as_act(x)
+        return ops.GammaResidualFn.apply(x, ops.ChannelAttentionFn.apply(x), self.gamma)
+
+
 class ReluFn(torch.autograd.Function):
     """stand-alone ReLU on a small tensor (FFM squeeze branch [N,C,1,1], seg_oprs.py:224-226): expressed through
     tsb_bn_apply with scale 1 / shift 0 so it stays on the library path"""

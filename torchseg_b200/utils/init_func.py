@@ -27,12 +27,14 @@ def init_weight(module_list, conv_init, norm_layer, bn_eps, bn_momentum, **kwarg
 
 def group_weight(weight_group, module, norm_layer, lr, no_decay_lr=None):
     """init_func.py:34-57: [decay: conv/linear weights] + [no decay: biases, norm γ/β]; asserts completeness."""
-    from ..seg_opr.seg_oprs import Encoding
+    from ..seg_opr.seg_oprs import CAM_Module, Encoding, PAM_Module
     decay, no_decay = [], []
     for m in module.modules():
         if isinstance(m, Encoding):   # EncNet: the codewords decay, the smoothing factors do not
             decay.append(m.codewords)
             no_decay.append(m.scale)
+        elif isinstance(m, (PAM_Module, CAM_Module)):   # DANet: gamma does not decay (the convs are visited on their own)
+            no_decay.append(m.gamma)
         elif isinstance(m, nn.Linear) or isinstance(m, _CONV):
             decay.append(m.weight)
             if m.bias is not None:
