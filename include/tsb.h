@@ -411,6 +411,34 @@ int tsb_attention_bwd(const void* q, int qcs, const void* k, int kcs, const void
                       const void* dout, int docs, const float* lse, float* delta_ws, void* dq, int dqcs, void* dk,
                       int dkcs, void* dv, int dvcs, int dq_accumulate, int B, int N, int dim_k, int dim_v, float scale,
                       tsb_stream_t stream);
+/* Cross attention (OCRNet's pixel-region relation): Nq queries and Nk keys / values per image,
+ *   o[b,i,:] = Σ_j softmax_j(scale · q[b,i,:]·k[b,j,:]) · v[b,j,:]     b < B, i < Nq, j < Nk
+ * on the (256, 256) kernels of tsb_attention_*, with their conventions: q, o, dout, dq, lse and delta_ws have B·Nq rows
+ * (row b·Nq + i), k, v, dk and dv B·Nk rows (row b·Nk + j). Only (d_k, d_v) = (256, 256); anything else is
+ * TSB_ERR_UNSUPPORTED. B·Nq, B·Nk < 2^31, B <= 65535. dq is written (there is no shared query / key form). With
+ * Nq = Nk = N the results are those of tsb_attention_* bit for bit. */
+int tsb_cross_attention_fwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, void* o, int ocs,
+                            float* lse, int B, int Nq, int Nk, int dim_k, int dim_v, float scale, tsb_stream_t stream);
+int tsb_cross_attention_bwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, const void* o,
+                            int ocs, const void* dout, int docs, const float* lse, float* delta_ws, void* dq, int dqcs,
+                            void* dk, int dkcs, void* dv, int dvcs, int B, int Nq, int Nk, int dim_k, int dim_v,
+                            float scale, tsb_stream_t stream);
+
+/* ---- OCRNet: soft-max over the pixels of each image (the soft object regions of the SpatialGather module) -------------
+ * logits: fp32 NHWC rows [B·N][lcs] (row b·N + n), K valid channels, 1 <= K <= 256, lcs a multiple of 8 and >= K
+ * rounded up to 8, 16-byte aligned; channels K..lcs−1 are never used. B·N < 2^31, B <= 65535.
+ * fwd: per (b, k) M = max_n l and S = Σ_n exp(l − M) in fp32, into stats (fp32 [B][2][K]: M, then S); P = exp(l − M) / S
+ *      rounded once into bf16 P [B·N][Kp] (dense, Kp = K rounded up to 64, channels K..Kp−1 written as exact zeros), an
+ *      operand of the per-image tsb_conv2d_* products.
+ * bwd: dl[n, k] = P[n, k] · (dP[n, k] − Σ_n' P[n', k] · dP[n', k]) with P recomputed in fp32 from the logits and stats;
+ *      dP fp32 [B·N][dpcs], dl fp32 [B·N][dlcs] (channels < K written), strides multiples of 8 and >= K rounded up to 8.
+ * Sums over the pixels run over fixed pixel ranges set by N and K whose partials (ws, ws_floats: B · ranges · 2K floats,
+ * at most 64 ranges per image until N exceeds 64 · 4 · 256 / ceil(K/8) pixels) are added in a fixed order: bit-identical
+ * from run to run and independent of the other images. */
+int tsb_spatial_softmax_fwd(const float* logits, int lcs, void* P, float* stats, int B, int N, int K, float* ws,
+                            long long ws_floats, tsb_stream_t stream);
+int tsb_spatial_softmax_bwd(const float* logits, int lcs, const float* stats, const float* dP, int dpcs, float* dl,
+                            int dlcs, int B, int N, int K, float* ws, long long ws_floats, tsb_stream_t stream);
 
 /* ---- DANet: channel attention (CAM) and the learnable-gamma residual --------------------------------------------------
  * CAM per image b with C channels: E = X Xᵀ (fp32 [C][C], tsb_conv2d_wgrad with dy = x), A = softmax_row(rowmax(E) − E),

@@ -99,6 +99,10 @@ _SIGS = {
     "tsb_se_loss_fwd_bwd": [P, I, L, P, I, I, P, P, P, I, P],
     "tsb_attention_fwd": [P, I, P, I, P, I, P, I, P, I, I, I, I, F, P],
     "tsb_attention_bwd": [P, I, P, I, P, I, P, I, P, I, P, P, P, I, P, I, P, I, I, I, I, I, I, F, P],
+    "tsb_cross_attention_fwd": [P, I, P, I, P, I, P, I, P, I, I, I, I, I, F, P],
+    "tsb_cross_attention_bwd": [P, I, P, I, P, I, P, I, P, I, P, P, P, I, P, I, P, I, I, I, I, I, I, F, P],
+    "tsb_spatial_softmax_fwd": [P, I, P, P, I, I, I, P, L, P],
+    "tsb_spatial_softmax_bwd": [P, I, P, P, I, P, I, I, I, I, P, L, P],
     "tsb_chan_attn_softmax_fwd": [P, P, I, I, P],
     "tsb_chan_attn_softmax_bwd": [P, P, P, P, I, I, P],
     "tsb_gamma_residual_fwd": [P, I, P, I, P, P, I, L, I, P],

@@ -1,19 +1,22 @@
 // Fused dense self-attention over the pixels of each image (OCNet's object context, Base-OC) on Hopper wgmma (sm_90a):
 //
-//   o[b,i,:] = Σ_j softmax_j(scale · q[b,i,:]·k[b,j,:]) · v[b,j,:]        i, j < N, d_k = d_v = 256
+//   o[b,i,:] = Σ_j softmax_j(scale · q[b,i,:]·k[b,j,:]) · v[b,j,:]        i < Nq, j < Nk, d_k = d_v = 256
 //
-// and its gradient. S = QKᵀ and P = softmax(S) live in registers and shared memory only; nothing of size N² reaches HBM.
+// and its gradient. S = QKᵀ and P = softmax(S) live in registers and shared memory only; nothing of size Nq·Nk reaches
+// HBM. Self-attention has Nq = Nk = N; OCRNet's pixel-region relation has the Nq pixels of an image as queries and its
+// Nk = K class regions as keys and values (the tsb_cross_attention_* entry points).
 // DANet's position attention, d_k = 64 and d_v = 512, has its own kernels further down (the "(64, 512)" section); what
 // follows up to there describes the (256, 256) plan.
 //
 // Tiling: every operand tile is 64 rows x 256 channels bf16 (32 KB), loaded by TMA through a 3-D map (channels, N, B)
-// as four 64-channel boxes with the 128-byte swizzle; rows past N are zero-filled by the map and never leave the image.
+// as four 64-channel boxes with the 128-byte swizzle; rows past Nq (q, dO) or Nk (k, v) are zero-filled by the map and
+// never leave the image.
 // Score products (QKᵀ, KQᵀ, dO·Vᵀ, V·dOᵀ) are m64n64k16 wgmmas with both operands K-major; the products with a
 // probability tile (P·V, Pᵀ·dO, dS·K, dSᵀ·Q) take P / dS from shared memory (written by the threads, K-major, swizzled
 // like a TMA tile) and the value-side tile as an MN-major B operand, as two m64n128k16 halves.
 //
-// Masking: zero-filled keys would score 0, so keys j >= N are set to −∞ (forward) or given P = 0 (backward); query rows
-// i >= N are computed on zeros and never stored.
+// Masking: zero-filled keys would score 0, so keys j >= Nk are set to −∞ (forward) or given P = 0 (backward); query rows
+// i >= Nq are computed on zeros, never stored, and their lse / δ never read.
 //
 // Determinism: no atomics. The forward and the dQ pass are query-stationary, the dK/dV pass is key-stationary, so every
 // output element has exactly one writer and a fixed summation order.
@@ -39,7 +42,7 @@ struct alignas(64) AttnParams {
     int cs0, cs1;
     float* lse;                 // forward output (may be null) / backward input
     const float* delta;
-    int N;
+    int Nq, Nk;                 // queries and keys (= values) per image; the (64, 512) kernels have Nq = Nk
     float c2;                   // scale · log2(e): the softmax runs in base 2
     float scale;
     int accumulate;             // query pass: dq += result
@@ -108,8 +111,8 @@ __global__ void __launch_bounds__(kThreads, 1) attn_fwd_kernel(const __grid_cons
     uint8_t* s_kv = smem + 2 * kTile;
     uint8_t* s_p = smem + 6 * kTile;
     uint64_t* bar = reinterpret_cast<uint64_t*>(s_p + 2 * kChunk);   // [0] Q, [1 + s] stage s
-    const int b = blockIdx.y, q0 = blockIdx.x * 128, N = p.N;
-    const int ntiles = (N + 63) / 64;
+    const int b = blockIdx.y, q0 = blockIdx.x * 128, Nq = p.Nq, Nk = p.Nk;
+    const int ntiles = (Nk + 63) / 64;
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31, wg = warp >> 2, wq = warp & 3;
 
     if (threadIdx.x == 0) {
@@ -155,7 +158,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_fwd_kernel(const __grid_cons
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     float& x = sc[4 * j + 2 * h + e];
-                    x = (key0 + 8 * j + e < N) ? x * p.c2 : -INFINITY;
+                    x = (key0 + 8 * j + e < Nk) ? x * p.c2 : -INFINITY;
                     mx[h] = fmaxf(mx[h], x);
                 }
         float corr[2];
@@ -205,16 +208,16 @@ __global__ void __launch_bounds__(kThreads, 1) attn_fwd_kernel(const __grid_cons
         l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
         l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
         const int row = q0 + 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
-        if (row >= N) continue;
+        if (row >= Nq) continue;
         const float inv = 1.f / l[h];
-        __nv_bfloat16* dst = p.out0 + ((long long)b * N + row) * p.cs0 + 2 * (lane & 3);
+        __nv_bfloat16* dst = p.out0 + ((long long)b * Nq + row) * p.cs0 + 2 * (lane & 3);
 #pragma unroll
         for (int half = 0; half < 2; ++half)
 #pragma unroll
             for (int j = 0; j < 16; ++j)
                 *reinterpret_cast<uint32_t*>(dst + 128 * half + 8 * j) =
                     pack_bf16(o[half][4 * j + 2 * h] * inv, o[half][4 * j + 2 * h + 1] * inv);
-        if (p.lse != nullptr && (lane & 3) == 0) p.lse[(long long)b * N + row] = (m2[h] + log2f(l[h])) * kLn2;
+        if (p.lse != nullptr && (lane & 3) == 0) p.lse[(long long)b * Nq + row] = (m2[h] + log2f(l[h])) * kLn2;
     }
 }
 
@@ -238,7 +241,7 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// backward, key-stationary: 64 keys per CTA, query tiles double-buffered. Warpgroup 0 recomputes Sᵀ = K·Qᵀ, forms Pᵀ and
+// backward, key-stationary: 64 keys per CTA, the image's query tiles double-buffered. Warpgroup 0 recomputes Sᵀ = K·Qᵀ, forms Pᵀ and
 // accumulates dV = Pᵀ·dO; warpgroup 1 computes dPᵀ = V·dOᵀ, takes Pᵀ (fp32) from warpgroup 0 through shared memory, forms
 // dSᵀ = Pᵀ ⊙ (dPᵀ − δ) and accumulates dK = scale · dSᵀ·Q. Each warpgroup holds one [64 x 256] fp32 accumulator.
 // smem: K | V | stage 0: Q, dO | stage 1: Q, dO | Pᵀ bf16 | dSᵀ bf16 | Pᵀ fp32 (fragment order) | barriers
@@ -255,8 +258,8 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_kv_kernel(const __grid_c
     uint8_t* s_ds = s_p + kChunk;
     float* s_pf = reinterpret_cast<float*>(s_ds + kChunk);
     uint64_t* bar = reinterpret_cast<uint64_t*>(s_pf + 32 * 128);   // [0] K/V, [1 + s] stage s
-    const int b = blockIdx.y, k0 = blockIdx.x * 64, N = p.N;
-    const int ntiles = (N + 63) / 64;
+    const int b = blockIdx.y, k0 = blockIdx.x * 64, Nq = p.Nq, Nk = p.Nk;
+    const int ntiles = (Nq + 63) / 64;
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31, wg = warp >> 2, wq = warp & 3;
     const int tid = threadIdx.x & 127;
 
@@ -282,8 +285,8 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_kv_kernel(const __grid_c
     for (int i = 0; i < 64; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
     const uint32_t k_lo = smem_u32(s_k) >> 4, v_lo = smem_u32(s_v) >> 4;
     const uint32_t p_lo = smem_u32(s_p) >> 4, ds_lo = smem_u32(s_ds) >> 4;
-    const float* lse = p.lse + (long long)b * N;
-    const float* delta = p.delta + (long long)b * N;
+    const float* lse = p.lse + (long long)b * Nq;
+    const float* delta = p.delta + (long long)b * Nq;
     mbar_wait(&bar[0], 0);
     for (int t = 0; t < ntiles; ++t) {
         const int s = t & 1;
@@ -301,11 +304,11 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_kv_kernel(const __grid_c
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int qi = qc + 8 * j + e;
-                    const float l2 = qi < N ? __ldg(lse + qi) * kLog2e : 0.f;
+                    const float l2 = qi < Nq ? __ldg(lse + qi) * kLog2e : 0.f;
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         float& x = f[4 * j + 2 * h + e];
-                        x = qi < N ? exp2f(x * p.c2 - l2) : 0.f;
+                        x = qi < Nq ? exp2f(x * p.c2 - l2) : 0.f;
                     }
                 }
 #pragma unroll
@@ -325,7 +328,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_kv_kernel(const __grid_c
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int qi = qc + 8 * j + e;
-                    const float dl = qi < N ? __ldg(delta + qi) : 0.f;
+                    const float dl = qi < Nq ? __ldg(delta + qi) : 0.f;
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const int i = 4 * j + 2 * h + e;
@@ -357,8 +360,8 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_kv_kernel(const __grid_c
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int row = k0 + 16 * wq + (lane >> 2) + 8 * h;
-        if (row >= N) continue;
-        __nv_bfloat16* dst = out + ((long long)b * N + row) * cs + 2 * (lane & 3);
+        if (row >= Nk) continue;
+        __nv_bfloat16* dst = out + ((long long)b * Nk + row) * cs + 2 * (lane & 3);
 #pragma unroll
         for (int half = 0; half < 2; ++half)
 #pragma unroll
@@ -369,7 +372,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_kv_kernel(const __grid_c
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// backward, query-stationary: 64 queries per CTA, key tiles double-buffered. Warpgroup 0 recomputes S = Q·Kᵀ and P,
+// backward, query-stationary: 64 queries per CTA, the image's key tiles double-buffered. Warpgroup 0 recomputes S = Q·Kᵀ and P,
 // warpgroup 1 computes dP = dO·Vᵀ and dS = P ⊙ (dP − δ); then warpgroup w accumulates channels [128w, 128w + 128) of
 // dQ = scale · dS·K.
 // smem: Q | dO | stage 0: K, V | stage 1: K, V | dS bf16 | P fp32 (fragment order) | barriers
@@ -385,8 +388,8 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_q_kernel(const __grid_co
     uint8_t* s_ds = smem + 6 * kTile;
     float* s_pf = reinterpret_cast<float*>(s_ds + kChunk);
     uint64_t* bar = reinterpret_cast<uint64_t*>(s_pf + 32 * 128);
-    const int b = blockIdx.y, q0 = blockIdx.x * 64, N = p.N;
-    const int ntiles = (N + 63) / 64;
+    const int b = blockIdx.y, q0 = blockIdx.x * 64, Nq = p.Nq, Nk = p.Nk;
+    const int ntiles = (Nk + 63) / 64;
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31, wg = warp >> 2, wq = warp & 3;
     const int tid = threadIdx.x & 127;
 
@@ -415,7 +418,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_q_kernel(const __grid_co
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int row = q0 + 16 * wq + (lane >> 2) + 8 * h;
-        rv[h] = row < N ? (wg == 0 ? p.lse[(long long)b * N + row] * kLog2e : p.delta[(long long)b * N + row]) : 0.f;
+        rv[h] = row < Nq ? (wg == 0 ? p.lse[(long long)b * Nq + row] * kLog2e : p.delta[(long long)b * Nq + row]) : 0.f;
     }
     const uint32_t q_lo = smem_u32(s_q) >> 4, do_lo = smem_u32(s_do) >> 4, ds_lo = smem_u32(s_ds) >> 4;
     mbar_wait(&bar[0], 0);
@@ -437,7 +440,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_q_kernel(const __grid_co
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         float& x = f[4 * j + 2 * h + e];
-                        x = kc + 8 * j + e < N ? exp2f(x * p.c2 - rv[h]) : 0.f;
+                        x = kc + 8 * j + e < Nk ? exp2f(x * p.c2 - rv[h]) : 0.f;
                     }
 #pragma unroll
             for (int i = 0; i < 32; ++i) s_pf[i * 128 + tid] = f[i];
@@ -465,8 +468,8 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_q_kernel(const __grid_co
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int row = q0 + 16 * wq + (lane >> 2) + 8 * h;
-        if (row >= N) continue;
-        __nv_bfloat16* dst = p.out0 + ((long long)b * N + row) * p.cs0 + 128 * wg + 2 * (lane & 3);
+        if (row >= Nq) continue;
+        __nv_bfloat16* dst = p.out0 + ((long long)b * Nq + row) * p.cs0 + 128 * wg + 2 * (lane & 3);
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
             uint32_t* d = reinterpret_cast<uint32_t*>(dst + 8 * j);
@@ -534,7 +537,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_fwd_wide_kernel(const __grid
     uint8_t* s_kv = smem + 2 * kChunk;
     uint8_t* s_p = s_kv + 2 * kWideStage;
     uint64_t* bar = reinterpret_cast<uint64_t*>(s_p + 2 * kChunk);   // [0] Q, [1 + s] stage s
-    const int b = blockIdx.y, q0 = blockIdx.x * 128, vc = blockIdx.z * kSlice, N = p.N;
+    const int b = blockIdx.y, q0 = blockIdx.x * 128, vc = blockIdx.z * kSlice, N = p.Nq;
     const int ntiles = (N + 63) / 64;
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31, wg = warp >> 2, wq = warp & 3;
 
@@ -680,7 +683,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_dv_wide_kernel(const __g
     uint8_t* s_st = smem + 2 * kChunk;
     uint8_t* s_p = s_st + 2 * kWideStage;
     uint64_t* bar = reinterpret_cast<uint64_t*>(s_p + 2 * kChunk);   // [0] K, [1 + s] stage s
-    const int b = blockIdx.y, k0 = blockIdx.x * 128, vc = blockIdx.z * kSlice, N = p.N;
+    const int b = blockIdx.y, k0 = blockIdx.x * 128, vc = blockIdx.z * kSlice, N = p.Nq;
     const int ntiles = (N + 63) / 64;
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31, wg = warp >> 2, wq = warp & 3;
 
@@ -790,7 +793,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_bwd_ds_wide_kernel(const __g
     const CUtensorMap* mxs = kKeyPass ? &p.a : &p.b;
     const CUtensorMap* my = kKeyPass ? &p.c : &p.d;
     const CUtensorMap* mys = kKeyPass ? &p.d : &p.c;
-    const int b = blockIdx.y, r0 = blockIdx.x * 64, N = p.N;
+    const int b = blockIdx.y, r0 = blockIdx.x * 64, N = p.Nq;
     const int ntiles = (N + 63) / 64;
     const int warp = warp_uniform_idx(), lane = threadIdx.x & 31, wg = warp >> 2, wq = warp & 3;
     const int tid = threadIdx.x & 127;
@@ -928,18 +931,27 @@ int check_shape(const char* who, int B, int N, int dim_k, int dim_v, float scale
     return TSB_OK;
 }
 
+// cross attention (Nq queries, Nk keys / values per image): (d_k, d_v) = (256, 256) only
+int check_cross_shape(const char* who, int B, int Nq, int Nk, int dim_k, int dim_v, float scale) {
+    TSB_REQUIRE(B >= 1 && Nq >= 1 && Nk >= 1, "%s: bad shape B=%d Nq=%d Nk=%d", who, B, Nq, Nk);
+    TSB_REQUIRE((long long)B * Nq < (1LL << 31) && (long long)B * Nk < (1LL << 31) && B <= 65535,
+                "%s: B*Nq and B*Nk must be below 2^31 and B at most 65535", who);
+    TSB_REQUIRE(scale > 0.f && scale < INFINITY, "%s: scale must be positive and finite", who);
+    if (!(dim_k == kDim && dim_v == kDim))
+        TSB_FAIL(TSB_ERR_UNSUPPORTED, "%s: d_k=%d d_v=%d, only (d_k, d_v) = (%d, %d) is supported", who, dim_k, dim_v,
+                 kDim, kDim);
+    return TSB_OK;
+}
+
 int encode_rows(CUtensorMap* m, const void* x, int cs, int B, int N, int dim) {
     return convhost::encode_3d(m, x, dim, (uint64_t)N, (uint64_t)B, (uint64_t)cs * 2, (uint64_t)N * cs * 2, 64, 64, 1);
 }
 
 #define ATTN_CHECK(expr) do { int rc_ = (expr); if (rc_) return rc_; } while (0)
 
-}  // namespace
-
-extern "C" int tsb_attention_fwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, void* o, int ocs,
-                                 float* lse, int B, int N, int dim_k, int dim_v, float scale, tsb_stream_t stream) {
-    const char* who = "tsb_attention_fwd";
-    ATTN_CHECK(check_shape(who, B, N, dim_k, dim_v, scale));
+// the forward after the shape check: q and o have Nq rows per image, k and v Nk (Nq == Nk at (64, 512))
+int attention_fwd(const char* who, const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, void* o,
+                  int ocs, float* lse, int B, int Nq, int Nk, int dim_k, int dim_v, float scale, cudaStream_t st) {
     ATTN_CHECK(check_operand(who, "q", q, qcs, dim_k));
     ATTN_CHECK(check_operand(who, "k", k, kcs, dim_k));
     ATTN_CHECK(check_operand(who, "v", v, vcs, dim_v));
@@ -947,25 +959,22 @@ extern "C" int tsb_attention_fwd(const void* q, int qcs, const void* k, int kcs,
     TSB_REQUIRE(lse == nullptr || tsb_aligned16(lse), "%s: lse must be 16-byte aligned", who);
     AttnParams prm;
     memset(&prm, 0, sizeof(prm));
-    ATTN_CHECK(encode_rows(&prm.a, q, qcs, B, N, dim_k));
-    ATTN_CHECK(encode_rows(&prm.b, k, kcs, B, N, dim_k));
-    ATTN_CHECK(encode_rows(&prm.c, v, vcs, B, N, dim_v));
+    ATTN_CHECK(encode_rows(&prm.a, q, qcs, B, Nq, dim_k));
+    ATTN_CHECK(encode_rows(&prm.b, k, kcs, B, Nk, dim_k));
+    ATTN_CHECK(encode_rows(&prm.c, v, vcs, B, Nk, dim_v));
     prm.out0 = (__nv_bfloat16*)o; prm.cs0 = ocs;
-    prm.lse = lse; prm.N = N; prm.c2 = scale * kLog2e; prm.scale = scale;
-    cudaStream_t st = (cudaStream_t)stream;
+    prm.lse = lse; prm.Nq = Nq; prm.Nk = Nk; prm.c2 = scale * kLog2e; prm.scale = scale;
     if (dim_k == kNarrow) {
         ATTN_CHECK(tsb_ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_wide_kernel), kFwdWideSmem));
-        attn_fwd_wide_kernel<<<dim3((N + 127) / 128, B, kWide / kSlice), kThreads, kFwdWideSmem, st>>>(prm);
+        attn_fwd_wide_kernel<<<dim3((Nq + 127) / 128, B, kWide / kSlice), kThreads, kFwdWideSmem, st>>>(prm);
         TSB_CUDA_CHECK_LAUNCH("attention_fwd_wide");
         return TSB_OK;
     }
     ATTN_CHECK(tsb_ensure_dyn_smem(reinterpret_cast<const void*>(attn_fwd_kernel), kFwdSmem));
-    attn_fwd_kernel<<<dim3((N + 127) / 128, B), kThreads, kFwdSmem, st>>>(prm);
+    attn_fwd_kernel<<<dim3((Nq + 127) / 128, B), kThreads, kFwdSmem, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("attention_fwd");
     return TSB_OK;
 }
-
-namespace {
 
 // the (64, 512) backward: δ, then dV per value slice, dK, and dQ (after dK, so that dq == dk with dq_accumulate adds
 // onto the finished dK)
@@ -994,14 +1003,11 @@ int attention_bwd_wide(AttnParams& prm, const void* o, int ocs, const void* dout
     return TSB_OK;
 }
 
-}  // namespace
-
-extern "C" int tsb_attention_bwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, const void* o,
-                                 int ocs, const void* dout, int docs, const float* lse, float* delta_ws, void* dq, int dqcs,
-                                 void* dk, int dkcs, void* dv, int dvcs, int dq_accumulate, int B, int N, int dim_k,
-                                 int dim_v, float scale, tsb_stream_t stream) {
-    const char* who = "tsb_attention_bwd";
-    ATTN_CHECK(check_shape(who, B, N, dim_k, dim_v, scale));
+// the backward after the shape check: q, o, dout, dq, lse and δ have Nq rows per image, k, v, dk and dv Nk
+int attention_bwd(const char* who, const void* q, int qcs, const void* k, int kcs, const void* v, int vcs,
+                  const void* o, int ocs, const void* dout, int docs, const float* lse, float* delta_ws, void* dq,
+                  int dqcs, void* dk, int dkcs, void* dv, int dvcs, int dq_accumulate, int B, int Nq, int Nk, int dim_k,
+                  int dim_v, float scale, cudaStream_t st) {
     ATTN_CHECK(check_operand(who, "q", q, qcs, dim_k));
     ATTN_CHECK(check_operand(who, "k", k, kcs, dim_k));
     ATTN_CHECK(check_operand(who, "v", v, vcs, dim_v));
@@ -1011,33 +1017,69 @@ extern "C" int tsb_attention_bwd(const void* q, int qcs, const void* k, int kcs,
     ATTN_CHECK(check_operand(who, "dk", dk, dkcs, dim_k));
     ATTN_CHECK(check_operand(who, "dv", dv, dvcs, dim_v));
     TSB_REQUIRE(lse != nullptr && delta_ws != nullptr, "%s: null lse or delta_ws", who);
-    cudaStream_t st = (cudaStream_t)stream;
     AttnParams prm;
     memset(&prm, 0, sizeof(prm));
-    ATTN_CHECK(encode_rows(&prm.a, q, qcs, B, N, dim_k));
-    ATTN_CHECK(encode_rows(&prm.b, k, kcs, B, N, dim_k));
-    ATTN_CHECK(encode_rows(&prm.c, v, vcs, B, N, dim_v));
-    ATTN_CHECK(encode_rows(&prm.d, dout, docs, B, N, dim_v));
+    ATTN_CHECK(encode_rows(&prm.a, q, qcs, B, Nq, dim_k));
+    ATTN_CHECK(encode_rows(&prm.b, k, kcs, B, Nk, dim_k));
+    ATTN_CHECK(encode_rows(&prm.c, v, vcs, B, Nk, dim_v));
+    ATTN_CHECK(encode_rows(&prm.d, dout, docs, B, Nq, dim_v));
     prm.lse = const_cast<float*>(lse); prm.delta = delta_ws;
-    prm.N = N; prm.c2 = scale * kLog2e; prm.scale = scale;
+    prm.Nq = Nq; prm.Nk = Nk; prm.c2 = scale * kLog2e; prm.scale = scale;
     if (dim_k == kNarrow)
-        return attention_bwd_wide(prm, o, ocs, dout, docs, delta_ws, dq, dqcs, dk, dkcs, dv, dvcs, dq_accumulate, B, N, st);
-    const int rows = B * N;
+        return attention_bwd_wide(prm, o, ocs, dout, docs, delta_ws, dq, dqcs, dk, dkcs, dv, dvcs, dq_accumulate, B, Nq,
+                                  st);
+    const int rows = B * Nq;
     attn_delta_kernel<<<tsb_grid_for(rows, 8, 8), 256, 0, st>>>((const __nv_bfloat16*)o, ocs, (const __nv_bfloat16*)dout,
                                                                 docs, delta_ws, rows);
     TSB_CUDA_CHECK_LAUNCH("attention_delta");
-    const dim3 grid((N + 63) / 64, B);
     // key pass first: with dq == dk and dq_accumulate the query pass then adds dQ onto the finished dK
     prm.out0 = (__nv_bfloat16*)dk; prm.cs0 = dkcs;
     prm.out1 = (__nv_bfloat16*)dv; prm.cs1 = dvcs;
     ATTN_CHECK(tsb_ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_kv_kernel), kKvSmem));
-    attn_bwd_kv_kernel<<<grid, kThreads, kKvSmem, st>>>(prm);
+    attn_bwd_kv_kernel<<<dim3((Nk + 63) / 64, B), kThreads, kKvSmem, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("attention_bwd_kv");
     prm.out0 = (__nv_bfloat16*)dq; prm.cs0 = dqcs;
     prm.out1 = nullptr; prm.cs1 = 0;
     prm.accumulate = dq_accumulate ? 1 : 0;
     ATTN_CHECK(tsb_ensure_dyn_smem(reinterpret_cast<const void*>(attn_bwd_q_kernel), kQSmem));
-    attn_bwd_q_kernel<<<grid, kThreads, kQSmem, st>>>(prm);
+    attn_bwd_q_kernel<<<dim3((Nq + 63) / 64, B), kThreads, kQSmem, st>>>(prm);
     TSB_CUDA_CHECK_LAUNCH("attention_bwd_q");
     return TSB_OK;
+}
+
+}  // namespace
+
+extern "C" int tsb_attention_fwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, void* o, int ocs,
+                                 float* lse, int B, int N, int dim_k, int dim_v, float scale, tsb_stream_t stream) {
+    const char* who = "tsb_attention_fwd";
+    ATTN_CHECK(check_shape(who, B, N, dim_k, dim_v, scale));
+    return attention_fwd(who, q, qcs, k, kcs, v, vcs, o, ocs, lse, B, N, N, dim_k, dim_v, scale, (cudaStream_t)stream);
+}
+
+extern "C" int tsb_attention_bwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, const void* o,
+                                 int ocs, const void* dout, int docs, const float* lse, float* delta_ws, void* dq, int dqcs,
+                                 void* dk, int dkcs, void* dv, int dvcs, int dq_accumulate, int B, int N, int dim_k,
+                                 int dim_v, float scale, tsb_stream_t stream) {
+    const char* who = "tsb_attention_bwd";
+    ATTN_CHECK(check_shape(who, B, N, dim_k, dim_v, scale));
+    return attention_bwd(who, q, qcs, k, kcs, v, vcs, o, ocs, dout, docs, lse, delta_ws, dq, dqcs, dk, dkcs, dv, dvcs,
+                         dq_accumulate, B, N, N, dim_k, dim_v, scale, (cudaStream_t)stream);
+}
+
+extern "C" int tsb_cross_attention_fwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs, void* o,
+                                       int ocs, float* lse, int B, int Nq, int Nk, int dim_k, int dim_v, float scale,
+                                       tsb_stream_t stream) {
+    const char* who = "tsb_cross_attention_fwd";
+    ATTN_CHECK(check_cross_shape(who, B, Nq, Nk, dim_k, dim_v, scale));
+    return attention_fwd(who, q, qcs, k, kcs, v, vcs, o, ocs, lse, B, Nq, Nk, dim_k, dim_v, scale, (cudaStream_t)stream);
+}
+
+extern "C" int tsb_cross_attention_bwd(const void* q, int qcs, const void* k, int kcs, const void* v, int vcs,
+                                       const void* o, int ocs, const void* dout, int docs, const float* lse,
+                                       float* delta_ws, void* dq, int dqcs, void* dk, int dkcs, void* dv, int dvcs, int B,
+                                       int Nq, int Nk, int dim_k, int dim_v, float scale, tsb_stream_t stream) {
+    const char* who = "tsb_cross_attention_bwd";
+    ATTN_CHECK(check_cross_shape(who, B, Nq, Nk, dim_k, dim_v, scale));
+    return attention_bwd(who, q, qcs, k, kcs, v, vcs, o, ocs, dout, docs, lse, delta_ws, dq, dqcs, dk, dkcs, dv, dvcs, 0,
+                         B, Nq, Nk, dim_k, dim_v, scale, (cudaStream_t)stream);
 }

@@ -8,3 +8,4 @@ from .encnet import EncNet, EncModule, EncHead
 from .ocnet import OCNet
 from .denseaspp import DenseASPP
 from .danet import DANet, DANetHead
+from .ocrnet import OCRNet

@@ -1205,7 +1205,10 @@ class AttentionFn(torch.autograd.Function):
     from the saved q, k, v, o and the per-row log-sum-exp (O(N·d) saved, not O(N²)). q, k: bf16 NHWC [B, d_k, h, w],
     v: [B, d_v, h, w] (channel slices allowed), (d_k, d_v) = (256, 256) or (64, 512). k = None means k is q (OCNet's
     shared f_key): the backward then returns dQ + dK as q's gradient, formed by the kernels in one buffer. Without any
-    input needing a gradient the forward skips the log-sum-exp."""
+    input needing a gradient the forward skips the log-sum-exp.
+
+    k and v may have another pixel count than q (OCRNet's [B, 256, K, 1] object-region keys and values, (256, 256)
+    only): the queries then attend over k's pixels of the same image, on tsb_cross_attention_{fwd,bwd}."""
 
     @staticmethod
     def forward(ctx, q, k, v, scale):
@@ -1213,32 +1216,101 @@ class AttentionFn(torch.autograd.Function):
         k = q if shared else k
         B, dk, h, w = q.shape
         dv = v.shape[1]
-        assert k.shape == q.shape and v.shape[0] == B and v.shape[2:] == q.shape[2:], "attention: shape mismatch"
+        assert k.shape[:2] == q.shape[:2] and v.shape[0] == B and v.shape[2:] == k.shape[2:], "attention: shape mismatch"
+        cross = k.shape[2:] != q.shape[2:]
         need = any(ctx.needs_input_grad)
         o = nhwc_empty(B, dv, h, w, device=q.device)
         lse = torch.empty((B, h * w), dtype=torch.float32, device=q.device) if need else None
-        call("tsb_attention_fwd", ptr(q), cs_of(q), ptr(k), cs_of(k), ptr(v), cs_of(v), ptr(o), dv, ptr(lse), B, h * w,
-             dk, dv, float(scale), stream())
+        if cross:
+            call("tsb_cross_attention_fwd", ptr(q), cs_of(q), ptr(k), cs_of(k), ptr(v), cs_of(v), ptr(o), dv, ptr(lse),
+                 B, h * w, k.shape[2] * k.shape[3], dk, dv, float(scale), stream())
+        else:
+            call("tsb_attention_fwd", ptr(q), cs_of(q), ptr(k), cs_of(k), ptr(v), cs_of(v), ptr(o), dv, ptr(lse), B,
+                 h * w, dk, dv, float(scale), stream())
         if need:
             ctx.save_for_backward(q, k, v, o, lse)
-            ctx.cfg = (shared, float(scale))
+            ctx.cfg = (shared, float(scale), cross)
         return o
 
     @staticmethod
     def backward(ctx, do):
         q, k, v, o, lse = ctx.saved_tensors
-        shared, scale = ctx.cfg
+        shared, scale, cross = ctx.cfg
         B, dk, h, w = q.shape
         dv = v.shape[1]
         do = as_nhwc_bf16(do)
         dq = nhwc_empty(B, dk, h, w, device=q.device)
-        dkt = dq if shared else nhwc_empty(B, dk, h, w, device=q.device)
-        dvt = nhwc_empty(B, dv, h, w, device=q.device)
+        dkt = dq if shared else nhwc_empty(B, dk, k.shape[2], k.shape[3], device=q.device)
+        dvt = nhwc_empty(B, dv, v.shape[2], v.shape[3], device=q.device)
         delta = torch.empty((B, h * w), dtype=torch.float32, device=q.device)
-        call("tsb_attention_bwd", ptr(q), cs_of(q), ptr(k), cs_of(k), ptr(v), cs_of(v), ptr(o), cs_of(o), ptr(do),
-             cs_of(do), ptr(lse), ptr(delta), ptr(dq), dk, ptr(dkt), dk, ptr(dvt), dv, int(shared), B, h * w, dk, dv,
-             scale, stream())
+        if cross:
+            call("tsb_cross_attention_bwd", ptr(q), cs_of(q), ptr(k), cs_of(k), ptr(v), cs_of(v), ptr(o), cs_of(o),
+                 ptr(do), cs_of(do), ptr(lse), ptr(delta), ptr(dq), dk, ptr(dkt), dk, ptr(dvt), dv, B, h * w,
+                 k.shape[2] * k.shape[3], dk, dv, scale, stream())
+        else:
+            call("tsb_attention_bwd", ptr(q), cs_of(q), ptr(k), cs_of(k), ptr(v), cs_of(v), ptr(o), cs_of(o), ptr(do),
+                 cs_of(do), ptr(lse), ptr(delta), ptr(dq), dk, ptr(dkt), dk, ptr(dvt), dv, int(shared), B, h * w, dk,
+                 dv, scale, stream())
         return dq, (None if shared else dkt), dvt, None
+
+
+# --------------------------------------------------------------------------------------------------
+# OCRNet: the object-region proxy (soft-max over the pixels of each image, then a per-image GEMM)
+# --------------------------------------------------------------------------------------------------
+class SpatialGatherFn(torch.autograd.Function):
+    """OCRNet's SpatialGather: ctx[b, :, k] = Σ_n softmax_n(l[b, k, n]) · f[b, :, n] over the h·w pixels n of image b.
+    f: bf16 NHWC [B, C, h, w], C a multiple of 64; logits: fp32 NHWC [B, >= K, h, w] (channel stride a multiple of 8);
+    returns the bf16 proxy [B, C, K, 1] (dense NHWC: row b·K + k holds region k of image b). The soft-max runs on
+    tsb_spatial_softmax_fwd, which writes P as a bf16 [B·N][Kp] operand (Kp = K rounded up to 64, zero past K); the
+    product Pᵀ·f is a wgrad per image into fp32 [Kp][C], cast once to the proxy. Backward, per image: dP = f·dctxᵀ is a
+    1x1 fprop with the zero-padded dctx as the weight (fp32 out), df = P·dctx a dgrad with dctx transposed, then
+    tsb_spatial_softmax_bwd forms the logits' gradient. No host synchronisation."""
+
+    @staticmethod
+    def forward(ctx, f, logits, K):
+        B, C, h, w = f.shape
+        K = int(K)
+        assert C % 64 == 0 and logits.dtype == torch.float32 and logits.shape[0] == B and logits.shape[1] >= K
+        assert tuple(logits.shape[2:]) == (h, w), "spatial gather: shape mismatch"
+        dev = f.device
+        Kp = (K + 63) // 64 * 64
+        P = nhwc_empty(B, Kp, h, w, device=dev)
+        stats = torch.empty((B, 2, K), dtype=torch.float32, device=dev)
+        call("tsb_spatial_softmax_fwd", ptr(logits), cs_of(logits), ptr(P), ptr(stats), B, h * w, K, *det_ws(), stream())
+        acc = torch.zeros((B, Kp, C), dtype=torch.float32, device=dev)
+        for n in range(B):
+            conv_wgrad(f[n:n + 1], P[n:n + 1], Kp, 1, 1, 0, 1, acc[n])
+        proxy = nhwc_empty(B, C, K, 1, device=dev)
+        call("tsb_cast_scale", ptr(acc), F32, Kp * C, ptr(proxy), BF16, K * C, B, K * C, None, stream())
+        if any(ctx.needs_input_grad[:2]):
+            ctx.save_for_backward(f, logits, P, stats)
+            ctx.K = K
+        return proxy
+
+    @staticmethod
+    def backward(ctx, dproxy):
+        f, logits, P, stats = ctx.saved_tensors
+        K = ctx.K
+        B, C, h, w = f.shape
+        Kp = P.shape[1]
+        dev = f.device
+        dproxy = as_nhwc_bf16(dproxy)
+        if cs_of(dproxy) != C:
+            dproxy = to_nhwc(dproxy)
+        dctx = torch.empty((B, Kp, C), dtype=_BF, device=dev)   # the fprop weights: dctx with zero rows K..Kp-1
+        call("tsb_cast_pad", ptr(dproxy), BF16, K * C, K * C, ptr(dctx), Kp * C, Kp * C, B, stream())
+        dctx_t = torch.empty((C, Kp), dtype=_BF, device=dev)
+        dP = nhwc_empty(B, Kp, h, w, dtype=torch.float32, device=dev)
+        df = nhwc_empty(B, C, h, w, device=dev)
+        for n in range(B):
+            conv_fprop(f[n:n + 1], dctx[n], Kp, 1, 1, 0, 1, out_dtype=torch.float32, out=dP[n:n + 1])
+            call("tsb_transpose_pad", ptr(dproxy[n]), BF16, C, ptr(dctx_t), Kp, K, C, Kp, stream())
+            conv_dgrad(P[n:n + 1], dctx_t, (1, C, h, w), Kp, 1, 1, 0, 1, out=df[n:n + 1])
+        lcs = cs_of(logits)
+        dl = nhwc_zeros(B, logits.shape[1], h, w, dtype=torch.float32, device=dev, cs=lcs)
+        call("tsb_spatial_softmax_bwd", ptr(logits), lcs, ptr(stats), ptr(dP), Kp, ptr(dl), lcs, B, h * w, K,
+             *det_ws(), stream())
+        return df, dl, None
 
 
 # --------------------------------------------------------------------------------------------------

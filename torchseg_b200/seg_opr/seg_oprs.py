@@ -369,6 +369,72 @@ class BaseOCModule(nn.Module):
         return _dropout2d(out, self.conv_bn_dropout[1].p, self.training)
 
 
+class SpatialGatherModule(nn.Module):
+    """OCRNet's object-region proxy (Yuan, Chen & Wang, "Object-Contextual Representations for Semantic Segmentation",
+    the SpatialGather module at scale 1): forward(f, l) = ctx with ctx[b, :, k] = Σ_n softmax_n(l[b, k, n]) · f[b, :, n],
+    the soft-max over the h·w pixels of image b, shaped [B, C, K, 1]. f: the features [B, C, h, w], l: the fp32 aux
+    logits [B, K, h, w]. No parameters; on ops.SpatialGatherFn."""
+
+    def __init__(self, cls_num=0, scale=1):
+        super(SpatialGatherModule, self).__init__()
+        if scale != 1:
+            raise NotImplementedError("SpatialGatherModule: scale != 1 is not implemented")
+        self.cls_num = cls_num
+        self.scale = scale
+
+    def forward(self, feats, probs):
+        return ops.SpatialGatherFn.apply(_as_act(feats), probs, int(probs.shape[1]))
+
+
+def _cbr1x1(cin, cout, norm_layer):
+    return ConvBnRelu(cin, cout, 1, 1, 0, has_bn=True, has_relu=True, has_bias=False, norm_layer=norm_layer)
+
+
+class ObjectAttentionBlock(nn.Module):
+    """OCRNet's pixel-region relation (`ObjectAttentionBlock2D` at scale 1): f_pixel and f_object are two 1x1
+    ConvBnRelu each (in → key → key), f_down and f_up one 1x1 ConvBnRelu each (in → key, key → in).
+    forward(x, proxy) = f_up(softmax_k(f_pixel(x) · f_object(proxy)ᵀ / √key) · f_down(proxy)): every pixel attends over
+    the K object regions of its image, on ops.AttentionFn's cross form (key_channels = 256)."""
+
+    def __init__(self, in_channels, key_channels, scale=1, norm_layer=nn.BatchNorm2d):
+        super(ObjectAttentionBlock, self).__init__()
+        if scale > 1:
+            raise NotImplementedError("ObjectAttentionBlock: scale > 1 (OCR's pooled form) is not implemented")
+        self.scale = scale
+        self.in_channels = in_channels
+        self.key_channels = key_channels
+        self.f_pixel = nn.Sequential(_cbr1x1(in_channels, key_channels, norm_layer),
+                                     _cbr1x1(key_channels, key_channels, norm_layer))
+        self.f_object = nn.Sequential(_cbr1x1(in_channels, key_channels, norm_layer),
+                                      _cbr1x1(key_channels, key_channels, norm_layer))
+        self.f_down = _cbr1x1(in_channels, key_channels, norm_layer)
+        self.f_up = _cbr1x1(key_channels, in_channels, norm_layer)
+
+    def forward(self, x, proxy):
+        x, proxy = _as_act(x), _as_act(proxy)
+        query = self.f_pixel(x)
+        key = self.f_object(proxy)
+        value = self.f_down(proxy)
+        return self.f_up(ops.AttentionFn.apply(query, key, value, self.key_channels ** -0.5))
+
+
+class SpatialOCRModule(nn.Module):
+    """OCRNet's object-contextual representation (`SpatialOCR_Module`): the ObjectAttentionBlock's context concatenated
+    in front of the input, then `conv_bn_dropout` = 1x1 ConvBnRelu(2·in → out) and Dropout2d"""
+
+    def __init__(self, in_channels, key_channels, out_channels, scale=1, dropout=0.1, norm_layer=nn.BatchNorm2d):
+        super(SpatialOCRModule, self).__init__()
+        self.object_context_block = ObjectAttentionBlock(in_channels, key_channels, scale, norm_layer)
+        self.conv_bn_dropout = nn.Sequential(_cbr1x1(2 * in_channels, out_channels, norm_layer), nn.Dropout2d(dropout))
+
+    def forward(self, feats, proxy_feats):
+        from ..networks.pspnet import _dropout2d
+        feats = _as_act(feats)
+        context = self.object_context_block(feats, proxy_feats)
+        out = self.conv_bn_dropout[0](ops.ConcatFn.apply(context, feats))
+        return _dropout2d(out, self.conv_bn_dropout[1].p, self.training)
+
+
 class DenseAsppBlock(nn.Module):
     """One pre-activation atrous layer of DenseASPP (Yang et al., CVPR 2018): pre_bn → ReLU → `reduce` (1x1 ConvBnRelu,
     in → mid) → the dilated 3x3 `conv` (mid → out, bias) → Dropout2d(dropout). bn_start=False drops pre_bn (and its
